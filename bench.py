@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- CPI frames/s of the passive-radar hot path (clutter filter -> fast_xambg) on B200.
+"""bench.py -- CPI frames/s of the passive-radar hot path (clutter filter -> fast_xambg) on H100.
 
     python bench.py --gpus N --steps K --warmup W                     # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K --warmup W    # the reference's CPU path on the host cores
@@ -8,7 +8,7 @@
 
 One "step" = ``--frames-per-step`` CPI frames pushed through the frame pipeline: the rank's resident set of
 ``--resident`` DISTINCT frames (default 125 = BASELINE config 3's 1000-frame stream over 8 GPUs; 2.1 GB, far larger
-than the 126 MB L2, so no pass finds its inputs cached) is walked as many times as the step needs.  With the defaults
+than the 50 MB L2, so no pass finds its inputs cached) is walked as many times as the step needs.  With the defaults
 the timed region is 20 steps x 4000 frames = a few seconds; the SM clocks in the line are sampled INSIDE it.
 ``value`` = frames/s with the frames already resident in HBM; ``e2e`` = the same through
 ``FramePipeline.run_host`` with pinned HOST buffers, H2D of both channels and D2H of the map inside the timed region;
@@ -16,6 +16,10 @@ the timed region is 20 steps x 4000 frames = a few seconds; the SM clocks in the
 thread pool the way main.py's dask scheduler does.  Rank r processes its own frames (weak scaling, no data-path
 collective); time = max over ranks.  With N > 1 the line also carries ``config3_stream``: the 1000-frame stream held by
 rank 0 and staged to the other ranks over NCCL (double buffered against compute).
+``--dump-outputs DIR`` writes, after the timed steps, the maps the timed path computed in its last step for a fixed,
+seeded sample of the resident frames (DIR/maps.npy, float32, [frame][Doppler][range][re, im]; DIR/frames.npy, the
+sampled frame indices): the inputs are seeded, so two builds run with the same arguments can be compared output for
+output.
 """
 from __future__ import annotations
 
@@ -65,12 +69,14 @@ def parse_args():
     ap.add_argument("--resident", type=int, default=0, help="distinct frames resident in HBM per GPU (0 = per config)")
     ap.add_argument("--frames-per-step", type=int, default=0, help="frames per step per GPU (0 = per config)")
     ap.add_argument("--batch", type=int, default=25, help="frames per library call (one launch of each kernel); 125 resident frames = 5 calls")
-    ap.add_argument("--slots", type=int, default=5, help="concurrent CUDA streams of the frame pipeline (measured: 25 x 5 38.2k, 16 x 3 34.9k frames/s)")
+    ap.add_argument("--slots", type=int, default=5, help="concurrent CUDA streams of the frame pipeline")
     ap.add_argument("--profile", default="P1", choices=["P0", "P1"])
     ap.add_argument("--nlms-block", type=int, default=1, help="config c4: block_len of block_NLMS (1 = NLMS_filter)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-stream", action="store_true", help="skip the config-3 NCCL staging measurement at N > 1")
     ap.add_argument("--cpu-procs", type=int, default=0, help="worker processes of the CPU arm (0 = auto)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's maps to DIR/*.npy (float32)")
     return ap.parse_args()
 
 
@@ -161,9 +167,9 @@ class ClockSampler:
 
 # ----------------------------------------------------------------------------- CPU arm
 def _ref_modules():
-    """(LS_Filter, NLMS_filter, fast_xambg, kind): the UNMODIFIED reference functions from baseline/_ref when the
-    recipe baseline/install_ref.py has been run (kind "reference"), else the oracle port (kind "port")."""
-    ref_dir = os.path.join(ROOT, "baseline", "_ref")
+    """(LS_Filter, NLMS_filter, fast_xambg, kind): the UNMODIFIED reference functions from oracle/_ref when the
+    recipe oracle/install_ref.py has been run (kind "reference"), else the oracle port (kind "port")."""
+    ref_dir = os.path.join(ROOT, "oracle", "_ref")
     if os.path.isdir(os.path.join(ref_dir, "passiveRadar")):
         if ref_dir not in sys.path:
             sys.path.insert(0, ref_dir)
@@ -292,9 +298,8 @@ class CpuArm:
             mem_gb = os.sysconf("SC_PHYS_PAGES") * os.sysconf("SC_PAGE_SIZE") / 2 ** 30
         except (ValueError, OSError):
             mem_gb = 16
-        # measured on the GPU box's host (128 logical CPUs, profiles/r02_cpu_pool.log): the workers are memory-bandwidth
-        # bound; 32 workers x 4 BLAS threads give the best whole-pool rate (0.51 frames/s; 64 x 2: 0.47, 16 x 8: 0.44,
-        # 8 x 16: 0.27), so the arm uses one worker per four logical CPUs
+        # the workers are memory-bandwidth bound: one worker per four logical CPUs, four BLAS threads each, gave the
+        # best whole-pool rate of the worker x thread shapes tried, so the arm uses that shape
         self.procs = procs if procs > 0 else max(1, min(ncpu // 4 if ncpu >= 8 else ncpu, int(mem_gb // 3), 64))
         self.blas_threads = blas_threads if blas_threads > 0 else max(1, ncpu // self.procs)
         for k in ("OPENBLAS_NUM_THREADS", "OMP_NUM_THREADS", "MKL_NUM_THREADS"):
@@ -322,7 +327,7 @@ class CpuArm:
     def sample_text(self):
         c = self.cfg
         flt = {"ls": "LS_Filter", "multi": "LS_Filter_Multiple"}.get(c["clutter"], "NLMS_filter")
-        src = "the reference's own functions (baseline/_ref, unmodified)" if self.kind == "reference" else "the oracle port"
+        src = "the reference's own functions (oracle/_ref, unmodified)" if self.kind == "reference" else "the oracle port"
         ext = (f"{flt} on n/{self.div} = {c['n'] // self.div} samples with all {c['filter_len'] + c['peek']} taps, time x{self.div} "
                f"(EXTRAPOLATED: cost linear in n)") if self.div > 1 else f"{flt} on the full frame"
         lags = (f"all {c['R'] + 1} range lags (measured" if self.lag_div == 1 else
@@ -369,9 +374,9 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             p = json.load(f)
-        return {"hbm_gbs": float(p["hbm_gbs"]), "sm_max_mhz": float(p.get("sm_max_mhz", 1965.0)),
+        return {"hbm_gbs": float(p["hbm_gbs"]), "sm_max_mhz": float(p.get("sm_max_mhz", 1980.0)),
                 "source": "MEASURED_PEAKS.json (measured copy bandwidth)", "of": "of measured"}
-    return {"hbm_gbs": 6650.0, "sm_max_mhz": 1965.0, "source": "fallback (B200_PROFILING.md)", "of": "of fallback"}
+    return {"hbm_gbs": 3350.0, "sm_max_mhz": 1980.0, "source": "H100 SXM data sheet (3.35 TB/s HBM3)", "of": "of data sheet"}
 
 
 def make_resident(torch, dev, n, profile, count, rank, base=8):
@@ -464,6 +469,21 @@ class Workload:
         torch.cuda.synchronize(self.dev)
 
 
+DUMP_FRAMES = 16            # maps written by --dump-outputs: 16 frames of config c2 are 9.9 MB of float32
+DUMP_SEED = 20240601
+
+
+def dump_outputs(out_dir, maps_d):
+    """The maps of a fixed, seeded sample of the resident frames, as float32 (re, im) pairs."""
+    import torch
+    nres = maps_d.shape[0]
+    idx = np.sort(np.random.default_rng(DUMP_SEED).choice(nres, size=min(DUMP_FRAMES, nres), replace=False))
+    maps = torch.view_as_real(maps_d[torch.from_numpy(idx).to(maps_d.device)]).cpu().numpy().astype(np.float32)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "maps.npy"), maps)
+    np.save(os.path.join(out_dir, "frames.npy"), idx.astype(np.float64))
+
+
 def time_passes(torch, dev, work, ref_d, srv_d, maps_d, frames):
     """Walk the resident set until `frames` frames have been processed (enqueue only)."""
     res = ref_d.shape[0]
@@ -490,7 +510,8 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
     n, F, R = cfg["n"], cfg["F"], cfg["R"]
     nlms = cfg["clutter"] == "nlms"
     direct = cfg["clutter"] != "ls"          # clutter filter and CAF as two batched library calls (no FramePipeline)
-    resident = args.resident or (444 if nlms else 125)
+    nsm = torch.cuda.get_device_properties(dev).multi_processor_count
+    resident = args.resident or (3 * nsm if nlms else 125)      # NLMS: one CTA per frame, three per SM
     fps_guess = 450.0 if nlms else 25000.0
     frames_per_step = args.frames_per_step or (resident if nlms else 4000)
     work = Workload(args, cfg, torch, dev, local_rank)
@@ -532,11 +553,13 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
     clocks = sampler.stop(t_begin, t_end) if rank == 0 else None
     frames_total = frames_per_step * args.steps * world
     value = frames_total / (ms * 1e-3)
+    if args.dump_outputs and rank == 0 and not quiet:
+        dump_outputs(args.dump_outputs, maps_d)
 
     # ---- end to end through the public API with host buffers (pinned), copies inside the timed region
     nb_host = ref_base.shape[0]
     if nlms:
-        nb_host = 148                # NLMS runs one CTA per frame: a call must carry enough frames to use the GPU
+        nb_host = nsm                # NLMS runs one CTA per frame: a call must carry enough frames to use the GPU
     ref_h = pinned_empty((nb_host, n))
     srv_h = pinned_empty((nb_host, n))
     for i in range(nb_host):
@@ -547,7 +570,7 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
     if direct:
         stage = (torch.empty((nb_host, n), dtype=torch.complex64, device=dev), torch.empty((nb_host, n), dtype=torch.complex64, device=dev),
                  torch.empty((nb_host, F, R + 1), dtype=torch.complex64, device=dev))
-    e2e_frames_per_step = max(nb_host, int(round((148 if nlms else 640) / nb_host)) * nb_host)
+    e2e_frames_per_step = max(nb_host, int(round((nsm if nlms else 640) / nb_host)) * nb_host)
     passes = e2e_frames_per_step // nb_host
     for _ in range(2):
         work.run_host(ref_h, srv_h, maps_h, stage)
@@ -638,14 +661,6 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
         dom = max(per_kernel, key=lambda k: prof[k][0])
         fpl = per_kernel[dom]["frames_per_launch"]
         traffic, traffic_note = None, None
-        tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")
-        if os.path.exists(tpath):
-            with open(tpath) as f:
-                tj = json.load(f)
-            ent = tj.get(args.config, {}).get(dom)
-            if ent:
-                traffic = ent["dram_bytes_per_frame"] * fpl
-                traffic_note = ent.get("note")
         ach = per_kernel[dom]["alg_GBps"]
         frame_gbps = bytes_frame(n, F, R) * value / world / 1e9
         roofline = {"kernel": dom, "bound": "hbm", "achieved": ach, "peak": peaks["hbm_gbs"], "unit": "GB/s",
@@ -659,7 +674,7 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
                             "LS lag sums, levinson = float64 Toeplitz solve (one CTA per frame, latency-bound), lagcorr_caf = CAF block "
                             "sums (clutter filter fused in), doppler_fft, misc = taps spectrum.",
                     "peak_source": peaks["source"] + ", " + peaks["of"],
-                    "path": "fft" if _lib.get_option("fft") else "direct (tcgen05 / FP32)"}
+                    "path": "fft" if _lib.get_option("fft") else "direct (wgmma / FP32)"}
         # single-frame latency: one frame, one stream, synchronised
         if not direct:
             lat = Workload(args1, cfg, torch, dev, local_rank)
@@ -707,7 +722,7 @@ def run_b200(args, cfg, rank, world, local_rank, quiet=False):
             "data": "synthetic", "config": config_dict(cfg, args, world),
             "run": {"frames_per_step_per_gpu": frames_per_step, "resident_distinct_frames_per_gpu": resident,
                     "frames_per_call": args.batch, "slots": args.slots, "timed_region_s": round(ms * 1e-3, 3),
-                    "cache": f"resident set {resident * 2 * n * 8 / 2 ** 20:.0f} MiB per GPU > 126 MB L2 (no flush needed)"},
+                    "cache": f"resident set {resident * 2 * n * 8 / 2 ** 20:.0f} MiB per GPU > 50 MB L2 (no flush needed)"},
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": e2e_frames_per_step * 2 * n * 8,
                     "d2h_bytes_per_step": e2e_frames_per_step * F * (R + 1) * 8, "frames_per_step_per_gpu": e2e_frames_per_step,
                     "api": "passiveradar_b200.frames.FramePipeline.run_host (pinned host ndarrays)" if not direct else
@@ -745,7 +760,7 @@ def run_sweep(args, rank, world, local_rank):
             a = argparse.Namespace(**vars(args))
             a.resident = max(20, min(125, (2 ** 31) // (16 * n))) // 5 * 5
             a.batch = a.resident // 5                      # five even calls per pass, one per slot
-            a.steps = min(base_steps, 5)
+            a.steps = base_steps
             a.frames_per_step = max(a.resident, int(8000 * 2 ** 20 / n / a.steps))      # ~0.3 s of GPU time per point
             a.no_cpu_baseline = True
             a.no_stream = True
@@ -773,6 +788,9 @@ def main():
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    if args.dump_outputs and (args.config == "c5" or args.impl == "reference"):
+        raise SystemExit("--dump-outputs writes the maps of a single-configuration GPU run; "
+                         "--config c5 and --impl reference compute none to write")
     if args.config == "c5":
         if args.impl == "reference":
             raise SystemExit("the sweep has no CPU arm")

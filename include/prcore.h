@@ -1,5 +1,5 @@
 /*
- * prcore.h -- C ABI of libprcore.so, the B200 (sm_100a) passive-radar DSP core.
+ * prcore.h -- C ABI of libprcore.so, the H100 (sm_90a) passive-radar DSP core.
  *
  * This is the drop-in boundary for the hot path of Max-Manning/passiveRadar.
  * The reference has no FFI of its own (it is pure Python), so each entry point
@@ -189,7 +189,7 @@ int prc_xambg_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
 
 /* ---- run-time switches (also read once from the environment: PRC_FFT, PRC_FFT_MIN_N) ----------------
  *   "fft"        1 (default): LS correlations, clutter FIR and CAF block sums as FFT-domain block correlations
- *                (csrc/fftcorr.cuh);  0: direct form on tcgen05 / FP32 (csrc/toepcorr.cuh, firtc.cuh, lagstream.cuh)
+ *                (csrc/fftcorr.cuh);  0: direct form on wgmma / FP32 (csrc/toepcorr.cuh, firtc.cuh, lagstream.cuh)
  *   "fft_min_n"  smallest channel length the FFT-domain path takes (default 8192)
  */
 int prc_set_option(const char* name, int value);

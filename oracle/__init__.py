@@ -24,7 +24,7 @@ How it is pinned
 ----------------
 The reference is pure Python and imports in the build container, so the goldens
 under ``tests/golden/`` were produced by *executing the reference's own
-functions* (``tests/golden/make_golden.py``, run with ``/root/reference`` on the
+functions* (``tests/golden/make_golden.py``, run with the reference checkout on the
 path) on the seeded inputs of ``passiveradar_b200.synth``.  ``tests/test_oracle_golden.py``
 checks every function here against those files, so "oracle == reference" is a
 tested statement, not an assumption.  The reference itself has no tests,

@@ -1,7 +1,7 @@
 """Oracle for the clutter cancellers (TEST INFRASTRUCTURE ONLY, see oracle/__init__.py).
 
 ``ls_filter_oracle``   follows ``LS_Filter``, reference
-                       ``/root/reference/passiveRadar/clutter_removal.py:6-56``:
+                       ``passiveRadar/clutter_removal.py:6-56``:
                        :31 lags = -peek .. filterLen-1, :34-36 A[:,k] = roll(ref, lags[k]),
                        :39 Gram A^H A, :42-45 Tikhonov solve, :51 srv - A @ taps.
                        All arithmetic stays complex64 (OpenBLAS cgemm/cgemv, LAPACK cgesv)

@@ -1,7 +1,7 @@
 /* nlms_oracle.c -- TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
  *
  * Plain-C restatement of the reference's NLMS_filter
- * (/root/reference/passiveRadar/clutter_removal.py:189-249, update rule :211-215)
+ * (passiveRadar/clutter_removal.py:189-249, update rule :211-215)
  * extended with the block_NLMS definition of oracle/clutter_oracle.py, so that the
  * 2M-sample BASELINE config can be checked in seconds instead of the ~18 s/frame the
  * Python loop needs.  Arithmetic is complex float (as numpy's complex64 path), with the

@@ -1,7 +1,7 @@
 """Oracle for the cross-ambiguity function (TEST INFRASTRUCTURE ONLY, see oracle/__init__.py).
 
 Restates ``fast_xambg`` of the reference
-(``/root/reference/passiveRadar/range_doppler_processing.py:12-90``):
+(``passiveRadar/range_doppler_processing.py:12-90``):
 
     :46-49   shape check                       -> ``_check_pair``
     :52-55   zero-pad to ``inputLen``          -> ``_pad_to``

@@ -1,4 +1,4 @@
-"""passiveradar_b200 -- B200-native (sm_100a) core for the passive-radar hot path.
+"""passiveradar_b200 -- H100-native (sm_90a) core for the passive-radar hot path.
 
 Drop-in operators with the reference's call signatures (Max-Manning/passiveRadar):
 

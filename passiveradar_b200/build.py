@@ -1,8 +1,8 @@
-"""Build libprcore.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libprcore.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m passiveradar_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the repo snapshot.
+The .so is git-ignored; it is rebuilt whenever a source, header or flag changes (source_hash).
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ HEADERS = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
     "-Xptxas", "-v",

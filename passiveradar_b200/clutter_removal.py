@@ -1,4 +1,4 @@
-"""Adaptive clutter cancellers on the B200 -- same call signatures as the reference.
+"""Adaptive clutter cancellers on the H100 -- same call signatures as the reference.
 
 Drop-ins for ``passiveRadar.clutter_removal.LS_Filter`` (reference
 ``passiveRadar/clutter_removal.py:6-56``) and ``NLMS_filter`` (``:189-249``), plus

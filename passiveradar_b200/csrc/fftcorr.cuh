@@ -20,7 +20,7 @@
 //
 // All kernels take a batch of frames in gridDim.y (frame_stride samples apart).  Every hot loop has ONE transform
 // call site (a loop body with two or three inlined transforms is 37-43 KB of SASS and misses the 32 KB instruction
-// cache on every iteration: ncu `stall_no_instruction` 0.96 per issue in the first version) and its input is
+// cache on every iteration) and its input is
 // staged one transform ahead with cp.async.  Algebra pinned on the CPU by scripts/fft/model.py (numpy) and
 // scripts/fft/emul.cu (thread-by-thread run of fftcore.cuh).
 #pragma once

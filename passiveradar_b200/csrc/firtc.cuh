@@ -1,4 +1,4 @@
-// firtc.cuh -- the clutter FIR  out[i] = srv[i] - sum_k w[k] ref[i + peek - k]  on tcgen05 tensor cores.
+// firtc.cuh -- the clutter FIR  out[i] = srv[i] - sum_k w[k] ref[i + peek - k]  on the Hopper tensor cores (wgmma).
 //
 // (reference clutter_removal.py:51 `srv - A @ filterTaps`, and np.convolve at :153-155 for the Toeplitz
 // variant).  With interleaved real data z = (re0, im0, re1, im1, ...) a block of 64 complex outputs is a
@@ -9,11 +9,9 @@
 // where Wm (KV x 128, KV = 2 (64 + peek + PRE)) is a constant band matrix made of the taps: for output
 // (io, ao) and input (iq, bq) the tap index is k = io + peek + PRE - iq and the entry is the (ao, bq)
 // element of [[wr, -wi], [wi, wr]].  So the FIR is a plain GEMM, M = row blocks a, N = 128, K = KV, with
-// K-major operands: A rows are overlapping windows of the signal planes (copied by the loader warps,
-// 128 contiguous bytes per row and K-atom), B is Wm^T, built once per frame by fir_bmat_kernel.
-// Same BF16x3 split as toepcorr.cuh (six products, fp32 accumulation in TMEM).  The a0*b0 chain is
-// spread over two accumulators (even / odd K-atoms) and the five cross terms go to a third, so no
-// accumulator sees more than ~K/128 truncating additions of full-size products.
+// K-major operands: A rows are overlapping windows of the signal planes, B is Wm^T, built once per frame
+// by fir_bmat_kernel.  Same BF16x3 split as toepcorr.cuh (six products, fp32 accumulation); the a0*b0
+// chain and the five cross terms are accumulated apart.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -23,8 +21,8 @@
 namespace prc {
 namespace tc {
 
-constexpr int FIR_ROWS = 128;                 // row blocks per CTA (UMMA M)
-constexpr int FIR_N = 128;                    // reals per row block (UMMA N)
+constexpr int FIR_ROWS = 128;                 // row blocks per CTA (two warpgroups of wgmma M = 64)
+constexpr int FIR_N = 128;                    // reals per row block (wgmma N)
 constexpr int FIR_KATOM = 64;                 // K elements per 128-byte swizzle atom
 constexpr int FIR_STAGES = 2;                 // pipeline stages of the taps-matrix (B) tiles
 constexpr int FIR_TILE_BYTES = FIR_ROWS * 128;               // one B plane, one K-atom: 16 KB
@@ -32,14 +30,13 @@ constexpr int FIR_BSTAGE_BYTES = NPLANE * FIR_TILE_BYTES;    // 48 KB
 constexpr int FIR_MAX_ATOMS = 16;             // kvp <= 1024  (M + peek up to ~440 taps)
 // The A operand of K-atom kc = 2 j + h is "signal row (m + j), half h": successive atoms are the same
 // data shifted by one row.  So the CTA keeps the raw rows [a0, a0 + 128 + j_max] resident (two swizzled
-// half-buffers per plane, loaded ONCE) and only moves the descriptor start address by j rows per atom
-// instead of re-reading a 6x Toeplitz-expanded operand from L2.
+// half-buffers per plane, loaded ONCE); the consumers read the row-shifted operand with ldmatrix into
+// registers (wgmma's register-A form) instead of re-reading a 6x Toeplitz-expanded operand from L2.
 constexpr int FIR_AROWS = FIR_ROWS + FIR_MAX_ATOMS / 2;      // 136 = 17 groups of 8
 constexpr int FIR_AHALF_BYTES = FIR_AROWS * 128;             // 17 KB
 constexpr int FIR_A_BYTES = NPLANE * 2 * FIR_AHALF_BYTES;    // 102 KB
-constexpr int FIR_LOAD_WARPS = 4, FIR_EPI_WARPS = 4;
-constexpr int FIR_THREADS = 32 * (FIR_EPI_WARPS + 1 + FIR_LOAD_WARPS);
-constexpr int FIR_TMEM_COLS = 512;            // three 128-column accumulators
+constexpr int FIR_MMA_WG = 2, FIR_LOAD_WARPS = 4;
+constexpr int FIR_THREADS = 32 * (4 * FIR_MMA_WG + FIR_LOAD_WARPS);
 constexpr int FIR_EPI_STRIDE = 132;           // floats per staged row (conflict-free 128-bit stores)
 
 struct FirTcParams {
@@ -53,33 +50,22 @@ struct FirTcParams {
     // optional: BF16 planes of the cleaned channel for the tensor-core CAF (see FirParams in kernels.cuh)
     uint16_t* cafs[3];
     long long caf_off, caf_slen;
-    long long* debug_clk;         // optional phase timestamps of CTA 0
 };
 
-// K-major, SWIZZLE_128B: 8-row groups SBO bytes apart; LBO is not used by the hardware for swizzled
-// K-major layouts (set to one 16-byte unit).  The swizzle is a function of the absolute shared-memory
-// address (bits [7,10) XORed into bits [4,7)), so a matrix may start at ANY row of a 1024-byte-aligned
-// buffer with base_offset = 0 (measured on B200: base_offset = row & 7 gives wrong operands) -- this is
-// what lets the row-shifted A operand below alias one resident copy of the signal.
-__device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t saddr, uint32_t sbo_bytes) {
-    return make_desc(saddr, 16, sbo_bytes) | ((uint64_t)2 << 61);
-}
-// instruction descriptor: D f32, A/B bf16, both K-major
-__host__ __device__ constexpr uint32_t make_idesc_bf16_kmajor(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+__device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], uint32_t saddr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
 }
 
 struct __align__(16) FirShared {
     uint64_t full[FIR_STAGES];
     uint64_t empty[FIR_STAGES];
     uint64_t a_ready;
-    uint64_t tmem_full;
-    uint32_t tmem_base;
-    uint32_t pad;
 };
 
 // dynamic shared memory: [A: plane x half x 136 rows x 128 B] [B stages: 2 x plane x 128 rows x 128 B];
-// the B stages are reused as the epilogue's transpose buffers.
+// the B stages are reused as the epilogue's transpose buffer.  Warps 0-7: two consumer warpgroups
+// (rows [64 wg, 64 wg + 64) of the CTA's row blocks); warps 8-11: loaders.
 __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_constant__ FirTcParams p) {
     extern __shared__ __align__(1024) uint8_t fsm[];
     __shared__ FirShared sh;
@@ -90,27 +76,17 @@ __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_cons
     uint8_t* bbase = fsm + FIR_A_BYTES;
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < FIR_STAGES; ++s) { mbar_init(&sh.full[s], FIR_LOAD_WARPS / FIR_STAGES); mbar_init(&sh.empty[s], 1); }
+        for (int s = 0; s < FIR_STAGES; ++s) { mbar_init(&sh.full[s], FIR_LOAD_WARPS / FIR_STAGES); mbar_init(&sh.empty[s], FIR_MMA_WG); }
         mbar_init(&sh.a_ready, FIR_LOAD_WARPS);
-        mbar_init(&sh.tmem_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == FIR_EPI_WARPS) tmem_alloc(&sh.tmem_base, FIR_TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sh.tmem_base;
-    long long t_begin = 0;
-    if (p.debug_clk && threadIdx.x == 0) {
-        t_begin = clock64();
-        if (blockIdx.x == 0) p.debug_clk[0] = t_begin;
-        unsigned long long gt;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        atomicMax(reinterpret_cast<unsigned long long*>(p.debug_clk + 21), ~gt);      // min start
-    }
 
-    if (warp > FIR_EPI_WARPS) {
-        const int lw = warp - FIR_EPI_WARPS - 1;          // 0..3
+    if (warp >= 4 * FIR_MMA_WG) {
+        // loaders need few registers: hand them to the consumers, whose two 64-register accumulators, A
+        // fragments and descriptors would otherwise not leave room for MMAs in flight
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+        const int lw = warp - 4 * FIR_MMA_WG;             // 0..3
         const int ch = lane & 7, r4 = lane >> 3;
         // ---- resident A: raw signal rows a0 .. a0 + arows - 1, both 64-element halves, three planes
         const int arows = FIR_ROWS + (natoms + 1) / 2;
@@ -128,7 +104,6 @@ __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_cons
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 0;" ::: "memory");
-        fence_proxy_async();
         __syncwarp();
         if (lane == 0) mbar_arrive(&sh.a_ready);
         // ---- streamed B: two warps per stage, each copies half of the stage's rows
@@ -155,75 +130,62 @@ __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_cons
             __syncwarp();
             if (lane == 0) mbar_arrive(&sh.full[st]);
         }
-    } else if (warp == FIR_EPI_WARPS) {
-        // ======================= MMA issuer
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_bf16_kmajor(FIR_ROWS, FIR_N);
-            mbar_wait(&sh.a_ready, 0);
-            for (int kc = 0; kc < natoms; ++kc) {
-                const int st = kc & (FIR_STAGES - 1);
-                mbar_wait(&sh.full[st], (kc / FIR_STAGES) & 1);
-                tc_fence_after();
-                if (p.debug_clk && blockIdx.x == 0 && kc < 12) p.debug_clk[4 + kc] = clock64();
-                const uint32_t sa = smem_u32(abase) + (uint32_t)(kc & 1) * FIR_AHALF_BYTES + (uint32_t)(kc >> 1) * 128;
-                const uint32_t sbm = smem_u32(bbase + st * FIR_BSTAGE_BYTES);
-                const uint32_t accm = tmem + (uint32_t)(kc & 1) * FIR_N;      // main accumulators 0 / 1
-                const uint32_t accs = tmem + 2 * FIR_N;                       // cross terms
-#pragma unroll
-                for (int kk = 0; kk < FIR_KATOM / 16; ++kk) {
-                    uint64_t da[NPLANE], db[NPLANE];
-#pragma unroll
-                    for (int pl = 0; pl < NPLANE; ++pl) {
-                        da[pl] = make_desc_k_sw128(sa + pl * 2 * FIR_AHALF_BYTES + kk * 32, 1024);
-                        db[pl] = make_desc_k_sw128(sbm + pl * FIR_TILE_BYTES + kk * 32, 1024);
-                    }
-                    umma_f16(accm, da[0], db[0], idesc, (kc >= 2) || (kk > 0));
-                    umma_f16(accs, da[0], db[1], idesc, (kc > 0) || (kk > 0));
-                    umma_f16(accs, da[1], db[0], idesc, 1);
-                    umma_f16(accs, da[0], db[2], idesc, 1);
-                    umma_f16(accs, da[2], db[0], idesc, 1);
-                    umma_f16(accs, da[1], db[1], idesc, 1);
-                }
-                umma_commit(&sh.empty[st]);
-            }
-            umma_commit(&sh.tmem_full);
-            if (p.debug_clk && blockIdx.x == 0) p.debug_clk[1] = clock64();
-        }
-        __syncwarp();
     } else {
-        // ======================= epilogue: out = srv - clutter.  TMEM (lane = row block) -> shared-memory
-        // transpose -> the warp's 32 rows x 64 samples are ONE contiguous 16 KB range of srv / out, streamed
-        // with fully coalesced 128-bit accesses (and 64-bit stores per BF16 plane).
-        mbar_wait(&sh.tmem_full, 0);
-        tc_fence_after();
-        if (p.debug_clk && blockIdx.x == 0 && threadIdx.x == 0) p.debug_clk[2] = clock64();
-        float* tile = reinterpret_cast<float*>(bbase) + warp * 32 * FIR_EPI_STRIDE;     // B stages are free now
-        const bool two_main = natoms >= 2;
-        for (int j0 = 0; j0 < FIR_N; j0 += 32) {
-            uint32_t v0[32], v1[32];
-            const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)j0;
-            tmem_ld32(lane_base, v0);
-            tmem_ld32(lane_base + 2 * FIR_N, v1);
+        // ======================= consumers
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
+        const int wg = warp >> 2, wq = warp & 3;
+        const bool leader = (threadIdx.x & 127) == 0;
+        // ldmatrix.x4 row addresses: lanes 8 q .. 8 q + 7 address matrix q = (rows +8 if q odd, K chunk +1 if q >= 2)
+        const int mq = lane >> 3;
+        const int arow = wg * 64 + wq * 16 + (lane & 7) + 8 * (mq & 1);
+        const int achunk = mq >> 1;
+        float accm[64], accs[64];
 #pragma unroll
-            for (int jj = 0; jj < 32; ++jj) v0[jj] = __float_as_uint(__uint_as_float(v0[jj]) + __uint_as_float(v1[jj]));
-            if (two_main) {
-                tmem_ld32(lane_base + FIR_N, v1);
+        for (int i = 0; i < 64; ++i) { accm[i] = 0.f; accs[i] = 0.f; }
+        mbar_wait(&sh.a_ready, 0);
+        for (int kc = 0; kc < natoms; ++kc) {
+            const int st = kc & (FIR_STAGES - 1);
+            mbar_wait(&sh.full[st], (kc / FIR_STAGES) & 1);
+            const int row = arow + (kc >> 1);                  // A of atom kc = signal rows shifted by kc / 2
+            const uint32_t sa = smem_u32(abase) + (uint32_t)(kc & 1) * FIR_AHALF_BYTES + (uint32_t)(row >> 3) * 1024 + (uint32_t)(row & 7) * 128;
+            const uint32_t sbm = smem_u32(bbase + st * FIR_BSTAGE_BYTES);
 #pragma unroll
-                for (int jj = 0; jj < 32; ++jj) v0[jj] = __float_as_uint(__uint_as_float(v0[jj]) + __uint_as_float(v1[jj]));
+            for (int kk = 0; kk < FIR_KATOM / 16; ++kk) {
+                uint32_t fa[NPLANE][4];
+                uint64_t db[NPLANE];
+                const uint32_t chunk = (uint32_t)(((2 * kk + achunk) ^ (row & 7)) << 4);
+#pragma unroll
+                for (int pl = 0; pl < NPLANE; ++pl) {
+                    ldmatrix_x4(fa[pl], sa + pl * 2 * FIR_AHALF_BYTES + chunk);
+                    db[pl] = make_desc_sw128(sbm + pl * FIR_TILE_BYTES + kk * 32, 16, 1024);
+                }
+                wgmma_fence();
+                wgmma_rs(accm, fa[0], db[0]);
+                wgmma_rs(accs, fa[0], db[1]);
+                wgmma_rs(accs, fa[1], db[0]);
+                wgmma_rs(accs, fa[0], db[2]);
+                wgmma_rs(accs, fa[2], db[0]);
+                wgmma_rs(accs, fa[1], db[1]);
+                wgmma_commit();
             }
-            float4* trow = reinterpret_cast<float4*>(tile + lane * FIR_EPI_STRIDE + j0);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-                trow[q] = make_float4(__uint_as_float(v0[4 * q]), __uint_as_float(v0[4 * q + 1]), __uint_as_float(v0[4 * q + 2]), __uint_as_float(v0[4 * q + 3]));
+            wgmma_wait<0>();
+            if (leader) mbar_arrive(&sh.empty[st]);           // this stage's B tiles have been read
         }
-        tc_fence_before();
-    }
-    if (warp != FIR_EPI_WARPS) {
-        // read-out by the four epilogue warps AND the four (now idle) loader warps: 16 rows of a tile each
-        asm volatile("bar.sync 1, %0;" ::"n"(32 * (FIR_EPI_WARPS + FIR_LOAD_WARPS)) : "memory");
-        const int tw = warp < FIR_EPI_WARPS ? warp : warp - FIR_EPI_WARPS - 1;
-        const int rbase = warp < FIR_EPI_WARPS ? 0 : 16;
-        const float* tile = reinterpret_cast<const float*>(bbase) + tw * 32 * FIR_EPI_STRIDE;
+        // ======================= epilogue: out = srv - clutter.  Registers -> shared-memory tile (row = row
+        // block) -> each warp's 16 rows x 64 samples are contiguous ranges of srv / out, streamed with fully
+        // coalesced 128-bit accesses (and 64-bit stores per BF16 plane).
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * 4 * FIR_MMA_WG) : "memory");   // every MMA has read its B stage
+        float* tile = reinterpret_cast<float*>(bbase);                             // [FIR_ROWS][FIR_EPI_STRIDE]
+#pragma unroll
+        for (int i = 0; i < 64; i += 2) {
+            const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int col = (i >> 2) * 8 + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(tile + r * FIR_EPI_STRIDE + col) = make_float2(accm[i] + accs[i], accm[i + 1] + accs[i + 1]);
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * 4 * FIR_MMA_WG) : "memory");
+        const int tw = warp >> 1;                      // 32-row group of the tile
+        const int rbase = (warp & 1) * 16;             // this warp's 16 rows of it
+        const float* trows = tile + tw * 32 * FIR_EPI_STRIDE;
         const long long ibase = (a0 + tw * 32) * 64 + 2 * lane;        // two samples per lane and row
         constexpr int RB = 8;
         for (int r0 = rbase; r0 < rbase + 16; r0 += RB) {
@@ -240,7 +202,7 @@ __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_cons
                 const int r = r0 + u;
                 const long long i = ibase + (long long)r * 64;
                 if (i >= p.n) continue;
-                const float4 cl = *reinterpret_cast<const float4*>(tile + r * FIR_EPI_STRIDE + 4 * lane);
+                const float4 cl = *reinterpret_cast<const float4*>(trows + r * FIR_EPI_STRIDE + 4 * lane);
                 const float4 ov = make_float4(sv[u].x - cl.x, sv[u].y - cl.y, sv[u].z - cl.z, sv[u].w - cl.w);
                 if (i + 1 < p.n) *reinterpret_cast<float4*>(p.out + i) = ov;
                 else p.out[i] = make_float2(ov.x, ov.y);
@@ -273,18 +235,6 @@ __global__ void __launch_bounds__(FIR_THREADS, 1) firtc_kernel(const __grid_cons
         }
     }
     __syncthreads();
-    if (p.debug_clk && threadIdx.x == 0) {
-        const long long t1 = clock64();
-        if (blockIdx.x == 0) p.debug_clk[3] = t1;
-        atomicMax(reinterpret_cast<unsigned long long*>(p.debug_clk + 20), (unsigned long long)(t1 - t_begin));
-        unsigned long long gt;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(gt));
-        atomicMax(reinterpret_cast<unsigned long long*>(p.debug_clk + 22), gt);
-    }
-    if (warp == FIR_EPI_WARPS) {
-        tc_fence_after();
-        tmem_dealloc(tmem, FIR_TMEM_COLS);
-    }
 }
 
 // Wm^T planes: B[u'][v'] for u' = 2 io + ao, v' = 2 iq + bq:  k = io + shift - iq (shift = peek + PRE);

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code of libprcore (passive-radar hot path).
+// kernels.cuh -- sm_90a device code of libprcore (passive-radar hot path).
 //
 // Four kernels carry the frame  LS_Filter -> fast_xambg  (DESIGN.md section 3):
 //
@@ -32,6 +32,12 @@ __host__ __device__ inline int stream_pieces(long long blk, int blk_len, long lo
     const long long a = (blk * (long long)blk_len) / per_cta;
     const long long b = ((blk + 1) * (long long)blk_len - 1) / per_cta;
     return (int)(b - a + 1);
+}
+
+// (a.x * b.x + c.x, a.y * b.y + c.y) with one rounding each.  Hopper has no packed FP32x2 FMA, so this is two
+// scalar fma.rn: the register pairs stay aligned 64-bit operands and the roundings are those of the packed form.
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 
 template <int A, int B> struct Gcd { static constexpr int v = Gcd<B, A % B>::v; };
@@ -97,11 +103,12 @@ __device__ __forceinline__ void slide_mac(float2 (&acc)[TD], const float2* __res
     }
 }
 
-// Packed variant: the same sliding-window MAC issued as FFMA2 (fma.rn.f32x2, sm_100+).  With
+// Packed variant: the same sliding-window MAC on (re, im) register pairs (ffma2_rn).  With
 //   A1[v] += (xr, xr) * (wr, wi)      A2[v] += (xi, xi) * (wr, wi)
-// every operand is an aligned 64-bit register pair, which (i) halves the instruction count and
-// (ii) removes the even/odd register-bank conflicts that cost the scalar FFMA form ~40 % of its
-// issue slots (ncu: dispatch_stall dominant, profiles/r01_lagcorr_v0.md).  The caller combines
+// every operand is an aligned 64-bit register pair.  On sm_90a each pair is two scalar FFMAs, so the
+// instruction count equals the scalar form's; what differs is the operand layout (one broadcast
+// load per sample, accumulators in pairs).  Which form is faster on the H100 has not been measured:
+// PRC_PACKED selects it for A/B runs.  The caller combines
 //   x*conj(w): re = A1.x + A2.y, im = A2.x - A1.y        x*w: re = A1.x - A2.y, im = A1.y + A2.x
 // xs4[i] = (xr, xr, xi, xi) of sample i (one broadcast 128-bit load per sample).
 template <int TI, int TD>
@@ -136,9 +143,9 @@ __device__ __forceinline__ void slide_mac2(float2 (&A1)[TD], float2 (&A2)[TD], c
                     const float2 xr2 = make_float2(xv.x, xv.y);
                     const float2 xi2 = make_float2(xv.z, xv.w);
 #pragma unroll
-                    for (int v = 0; v < TD; ++v) A1[v] = __ffma2_rn(xr2, W[(p * TI + u + v) % RS], A1[v]);
+                    for (int v = 0; v < TD; ++v) A1[v] = ffma2_rn(xr2, W[(p * TI + u + v) % RS], A1[v]);
 #pragma unroll
-                    for (int v = 0; v < TD; ++v) A2[v] = __ffma2_rn(xi2, W[(p * TI + u + v) % RS], A2[v]);
+                    for (int v = 0; v < TD; ++v) A2[v] = ffma2_rn(xi2, W[(p * TI + u + v) % RS], A2[v]);
                 }
             }
         }
@@ -182,9 +189,9 @@ __device__ __forceinline__ void slide_mac2n(float2 (&A1)[TD], float2 (&A2)[TD], 
                         const float2 xr2 = uu ? make_float2(xv.z, xv.z) : make_float2(xv.x, xv.x);
                         const float2 xi2 = uu ? make_float2(xv.w, xv.w) : make_float2(xv.y, xv.y);
 #pragma unroll
-                        for (int v = 0; v < TD; ++v) A1[v] = __ffma2_rn(xr2, W[(p * TI + u + uu + v) % RS], A1[v]);
+                        for (int v = 0; v < TD; ++v) A1[v] = ffma2_rn(xr2, W[(p * TI + u + uu + v) % RS], A1[v]);
 #pragma unroll
-                        for (int v = 0; v < TD; ++v) A2[v] = __ffma2_rn(xi2, W[(p * TI + u + uu + v) % RS], A2[v]);
+                        for (int v = 0; v < TD; ++v) A2[v] = ffma2_rn(xi2, W[(p * TI + u + uu + v) % RS], A2[v]);
                     }
                 }
             }
@@ -239,8 +246,7 @@ __global__ void __launch_bounds__(512) lagcorr_kernel(const __grid_constant__ La
     if (len > p.chunk_len) len = p.chunk_len;
 
     // Staging issues STAGE_BATCH independent global loads per thread before the first store:
-    // a one-load-per-iteration loop serialises ~16 DRAM latencies per CTA (measured: 30 % of the
-    // kernel, profiles/r01_lagcorr_v1.md).
+    // a one-load-per-iteration loop would serialise ~16 DRAM latencies per CTA.
     constexpr int STAGE_BATCH = 8;
     // ---- stage the weighted x chunk (zero outside the block / the signal)
     const float2* __restrict__ x = p.x;

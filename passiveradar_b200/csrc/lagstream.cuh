@@ -1,16 +1,16 @@
-// lagstream.cuh -- persistent, software-pipelined lag-correlation kernel (sm_100a).
+// lagstream.cuh -- persistent, software-pipelined lag-correlation kernel (sm_90a).
 //
 // Same arithmetic as lagcorr_kernel (kernels.cuh):
 //     partial[prob][blk][piece][l] = sum_{i in piece of block blk} x[i] * conj(s[(i + dmin + l) mod n])
 // but organised for the FP32 pipe instead of for simplicity:
 //   * the blocks of one problem are laid end to end as one stream of nblk*blk_len samples and cut
 //     into gridDim.x equal ranges, one per CTA ("stream-K"): every SM gets the same amount of work
-//     whatever F, N and R are (256 Doppler blocks on 148 SMs lose 14 % to wave quantisation when a
+//     whatever F, N and R are (256 Doppler blocks on 132 SMs lose 3 % to wave quantisation when a
 //     CTA is tied to a block); a CTA that crosses a block boundary flushes one partial row per block
 //     it touched ("piece");
 //   * inside its range a CTA walks sub-chunks of <= G*steps*TI samples; sub-chunk k+1 is copied
 //     global -> shared with cp.async (LDGSTS, zero-fill outside the signal) while sub-chunk k is in
-//     the FFMA2 loop: staging never leaves the math pipe idle (it cost 30 % in the one-shot kernel);
+//     the MAC loop: staging never leaves the math pipe idle;
 //   * accumulators stay in registers across sub-chunks; the cross-group reduction and the partial
 //     row are paid once per piece, not once per 1-2k samples.
 // x must already carry its weights (ref, or ref*window written by weight_kernel); the tap-weighted

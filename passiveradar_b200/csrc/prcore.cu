@@ -1,7 +1,7 @@
 // prcore.cu -- host side of libprcore.so: C ABI (include/prcore.h), workspaces, launches.
 //
 // Build (see passiveradar_b200/build.py):
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo \
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo \
 //        -Xcompiler -fPIC -shared -Iinclude -o passiveradar_b200/libprcore.so prcore.cu
 //
 // Threading model: one workspace ("Ctx") per (device, caller stream), or per
@@ -168,18 +168,18 @@ std::vector<Ctx*> g_all_ctx;
 std::atomic<bool> g_attrs_set[64];
 std::atomic<uint64_t> g_epoch{1};                      // bumped by prc_shutdown
 int g_tune_nchunk = -1, g_tune_g = -1;
-int g_tile = 0;          // measured on B200: 10x10 beats 6x18 / 14x14 (109 vs 117 / 115 us, profiles/r01_tuning.md)
+int g_tile = 0;          // register tile of the FP32 lag kernels: 10x10 (PRC_TILE=1: 6x18, 2: 14x14)
 int g_nlms_block = 1;       // block-exact NLMS kernel for NLMS_filter (PRC_NLMS_BLOCK=0: sample-serial kernel)
 int g_tma_l2 = 2;          // CUtensorMapL2promotion: 0 none, 1 64B, 2 128B, 3 256B (PRC_TMA_L2)
-int g_tma = 1;             // TMA (cp.async.bulk.tensor) producers for the tcgen05 kernels (PRC_TMA=0: 16-byte cp.async loaders)
+int g_tma = 1;             // TMA (cp.async.bulk.tensor) producers for the wgmma kernels (PRC_TMA=0: 16-byte cp.async loaders)
 int g_tc_fir = 1;          // tensor-core path for the clutter FIR (PRC_TC_FIR=0: FP32 fir_apply_kernel)
 int g_tc_caf = 1;          // tensor-core path for the CAF block sums as well (PRC_TC_CAF=0: FP32 lagstream)
-int g_tc = 1;              // tcgen05 Toeplitz-GEMM for the LS correlations (PRC_TC=0: FP32 lagstream kernel)
+int g_tc = 1;              // wgmma Toeplitz-GEMM for the LS correlations (PRC_TC=0: FP32 lagstream kernel)
 int g_stream = 1;          // persistent pipelined lag-correlation kernel (PRC_STREAM=0: one-shot kernel)
-int g_packed = 1;          // FFMA2 kernels (PRC_PACKED=0 selects the scalar-FFMA variant for A/B runs)
-std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: tcgen05 / FP32 direct form
+int g_packed = 1;          // paired-FMA kernels (PRC_PACKED=0 selects the scalar-FFMA variant for A/B runs)
+std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: wgmma / FP32 direct form
 std::atomic<int> g_fft_min_n{8192};   // ... for channels of at least this many samples (PRC_FFT_MIN_N)
-std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks (measured 4 % slower than one CTA per block)
+std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks instead of one CTA per block
 std::once_flag g_env_once;
 
 // Workspaces of a thread that called with stream == NULL.  They are released when the thread exits (dask's thread pool
@@ -801,7 +801,6 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
         tp.nk = (int)(ct.nx / 1024); tp.nlag = R + 1; tp.npass = ct.npass; tp.ranges = 0;
         tp.kb = (int)(D / 1024); tp.nblk = F; tp.HT = ct.ht;
         tp.partial = c->partial.as<float2>();
-        tp.debug_tile = nullptr; tp.debug_clk = nullptr;
         static const tc::ToepMaps no_maps{};
         const tc::ToepMaps* mp = &no_maps;
         const bool tma = use_tma();
@@ -1030,7 +1029,6 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
         }
         tp.nk = tc_nk; tp.nlag = M; tp.npass = tc_npass; tp.ranges = tc_ranges; tp.HT = tc_ht;
         tp.partial = c->partial.as<float2>();
-        tp.debug_tile = nullptr; tp.debug_clk = nullptr;
         static const tc::ToepMaps no_maps{};
         const tc::ToepMaps* mp = &no_maps;
         const bool tma = use_tma();
@@ -1134,22 +1132,7 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
                 ft.caf_slen = caf->slen;
                 caf->planes_ready = true;
             }
-            static long long* dbg = nullptr;
-            if (getenv("PRC_FIR_DEBUG")) {
-                if (!dbg) cudaMalloc(&dbg, 256);
-                cudaMemsetAsync(dbg, 0, 256, c->stream);
-                ft.debug_clk = dbg;
-            }
             tc::firtc_kernel<<<fir_nblk, tc::FIR_THREADS, tc::firtc_smem_bytes(), c->stream>>>(ft);
-            if (ft.debug_clk) {
-                long long h[32];
-                cudaMemcpyAsync(h, dbg, 256, cudaMemcpyDeviceToHost, c->stream);
-                cudaStreamSynchronize(c->stream);
-                fprintf(stderr, "[firtc] grid=%d kvp=%d: last MMA commit %lld, tmem_full seen %lld, all done %lld cycles; full[kc] at",
-                        fir_nblk, fir_kv, h[1] - h[0], h[2] - h[0], h[3] - h[0]);
-                for (int k = 0; k < 12; ++k) fprintf(stderr, " %lld", h[4 + k] - h[0]);
-                fprintf(stderr, "; slowest CTA %lld cycles, first start -> last end %lld ns\n", h[20], h[22] - (long long)~(unsigned long long)h[21]);
-            }
         }
         TRY(check_launch("firtc_kernel"));
         if (taps_out)
@@ -1535,7 +1518,7 @@ int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batc
         TRY(taps_spectrum(c, cf.r3, M, bt.nf, &c->wp_caf));
         return xambg_device(c, ref, srv, n, R, F, win32, nullptr, 0, maps, false, false, bt, c->wp_caf.as<float2>(), M, peek);
     }
-    // direct-form kernels (tcgen05 / FP32), frame by frame
+    // direct-form kernels (wgmma / FP32), frame by frame
     TRY(c->clean.ensure((size_t)n * sizeof(float2)));
     TRY(c->status.ensure((size_t)bt.nf * sizeof(int)));
     for (int fr = 0; fr < bt.nf; ++fr) {

@@ -1,4 +1,4 @@
-// toepcorr.cuh -- lag correlations of the LS normal equations on the 5th-gen tensor cores (tcgen05).
+// toepcorr.cuh -- lag correlations of the LS normal equations on the Hopper tensor cores (wgmma).
 //
 // The Gram column c[m] = sum_i conj(ref[i]) ref[i+m] and the right-hand side x[m] = sum_i conj(ref[i])
 // srv[i+m] of LS_Filter (reference clutter_removal.py:39,45) are the one step of the hot path that is
@@ -13,18 +13,15 @@
 //                  im(C[(delta-1)/2]) -= D[u][v]   for even u        (re*im)
 //   with C[l] = sum_i x[i] conj(s[i+l]).
 //
-// M = 128 rows (u) x N = 256 columns (one "pass" of v) x K = 16 (rows a) per tcgen05.mma.kind::f16
-// with BF16 operands, fp32 accumulation in TMEM.  fp32 accuracy comes from a three-way BF16 split
-// z = b0 + b1 + b2 (24 significand bits) and the six products of order <= 2:
+// A CTA tile is M = 128 rows (u) x N = 128 columns (one "pass" of v); two consumer warpgroups each issue
+// wgmma.m64n128k16 (BF16 operands, fp32 accumulators in registers) on 64 of the rows, K = 16 rows a per
+// instruction.  fp32 accuracy comes from a three-way BF16 split z = b0 + b1 + b2 (24 significand bits)
+// and the six products of order <= 2:
 //   D += b0*b0' + b0*b1' + b1*b0' + b0*b2' + b2*b0' + b1*b1'      (dropped terms ~2^-24 relative)
-// -- the same tensor time as 3xTF32 (BF16 runs at twice the TF32 rate) with 25 % fewer operand bytes;
-// kind::tf32 with MN-major operands returns zeros on this part (scripts/tc/mma_probe2.cu), BF16
-// MN-major is exact (scripts/tc/mma_probe3.cu).
-// Operands are MN-major (contiguous along u / v), no swizzle: the canonical core matrix is 8 K-rows x
-// 16 bytes (8 elements); 16-byte MN chunks are SBO = 128 B apart, the two 8-row K groups LBO apart.
-// The overlapping ("im2col") rows of the s operand are materialised by the loader warps' 16-byte
-// cp.async copies straight from the interleaved BF16 planes -- no expanded matrix ever exists in HBM.  One CTA = one (problem, pass, K-range); warps 0-3 epilogue (TMEM -> diagonal sums),
-// warp 4 issues the MMAs, warps 5-8 load.
+// Operands are MN-major (contiguous along u / v) with the 128-byte swizzle; both wgmma operands come from
+// shared memory (transposed-operand form).  The overlapping ("im2col") rows of the s operand are
+// materialised by the producers straight from the interleaved BF16 planes -- no expanded matrix ever
+// exists in HBM.  Warps 0-7: two consumer warpgroups (MMA + diagonal-sum epilogue); warps 8-11: producers.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -35,51 +32,46 @@ namespace tc {
 
 constexpr int ROW = 128;            // elements per K-row (= 64 complex samples)
 constexpr int KSTEP = 16;           // K-rows per MMA (bf16: K = 16)
-constexpr int NPASS = 256;          // columns per pass (UMMA N)
+constexpr int NPASS = 128;          // columns per pass (wgmma N)
 constexpr int STAGES = 4;
 constexpr int NPLANE = 3;           // b0, b1, b2
 constexpr int A_BYTES = ROW * KSTEP * 2;          // 4 KB per plane
-constexpr int B_BYTES = NPASS * KSTEP * 2;        // 8 KB per plane
-constexpr int STAGE_BYTES = NPLANE * (A_BYTES + B_BYTES);   // 36 KB
+constexpr int B_BYTES = NPASS * KSTEP * 2;        // 4 KB per plane
+constexpr int STAGE_BYTES = NPLANE * (A_BYTES + B_BYTES);   // 24 KB
 // 128-byte-swizzled MN-major tiles: atom = 8 K-rows x 128 B (64 elements along MN), the 16-byte chunk
 // index inside a row is XOR-ed with the row index (Swizzle<3,4,3>); atoms ordered [k-group][mn-group].
-// (The unswizzled "interleave" layout works too but the tensor core then runs at ~55 % of its rate.)
 constexpr int ATOM_BYTES = 1024;
 constexpr int A_SBO = (ROW / 64) * ATOM_BYTES;    // stride between the two 8-row K groups of an A tile
 constexpr int B_SBO = (NPASS / 64) * ATOM_BYTES;  // ... of a B tile
 constexpr int MN_LBO = ATOM_BYTES;                // stride between 64-element MN groups
-constexpr int NUM_EPI_WARPS = 4, NUM_LOAD_WARPS = 4;
-constexpr int THREADS = 32 * (NUM_EPI_WARPS + 1 + NUM_LOAD_WARPS + NUM_EPI_WARPS);   // 13 warps
+constexpr int NUM_MMA_WG = 2, NUM_LOAD_WARPS = 4;
+constexpr int THREADS = 32 * (4 * NUM_MMA_WG + NUM_LOAD_WARPS);   // 12 warps
 static_assert(STAGES == NUM_LOAD_WARPS, "loader warp w owns pipeline stage w");
-constexpr int SKEW_FLOATS = 32 * 33 + 32;          // per-warp transpose buffer (row stride 33)
-constexpr int EPI_PARTS = 2 * NUM_EPI_WARPS;       // warps 0-3 take accumulator columns [0,128), warps 9-12 [128,256)
-constexpr int TMEM_COLS = 2 * NPASS;   // [0,256): b0*b0' products, [256,512): the five cross terms
+constexpr int EPI_PARTS = 4 * NUM_MMA_WG;          // one private set of lag sums per consumer warp
+constexpr int TILE_LD = 65;                        // accumulator tile of a warpgroup, column-major, 64 rows + 1 pad
+constexpr int TILE_FLOATS = NPASS * TILE_LD;
 
 struct ToepParams {
     const uint16_t* x[NPLANE];       // interleaved BF16 planes of the x operand, zero beyond the signal
     const uint16_t* s[2][NPLANE];    // per problem: s rotated by dmin and circularly extended
     int nk;                 // K-steps (of 16 rows = 1024 complex samples) in the signal
     int nlag;               // complex lags wanted: 0 .. nlag-1
-    int npass;              // ceil(2*(64+nlag) / 256)
+    int npass;              // ceil(2*(64+nlag) / NPASS)
     int ranges;             // LS mode: CTAs per (problem, pass): gridDim.x = 2 * npass * ranges
     int kb;                 // block mode (> 0): K-steps per block; items = nblk * npass, any gridDim.x
     int nblk;
     int HT;                 // row length of the partial buffer (padded lag count)
     float2* partial;        // LS: [problem][pass*ranges + range][HT];  block mode: [blk][pass][HT]
-    float* debug_tile;      // optional: raw 128x256 accumulator of CTA 0
-    long long* debug_clk;   // optional: phase timestamps of CTA 0
 };
 
 // ---- TMA producer (TMA = true) ------------------------------------------------------------------------------
 // Tensor maps of the BF16 planes: element (c0, c1) = plane[128 * c1 + c0], i.e. K-row c1 of the Toeplitz
-// operand starting at column c0.  Rows are 256 bytes apart but 256 * npass elements wide: they OVERLAP in
-// memory (cuTensorMapEncodeTiled accepts that, scripts/tc/tma_probe.cu), which is what materialises the
-// im2col operand without ever storing it.  Box = 64 elements x 16 K-rows, SWIZZLE_128B: it lands as 16 rows
-// of 128 bytes with the 16-byte chunk index XOR-ed with (row & 7) -- the UMMA operand layout, with the two
-// 8-row K groups of one 64-element MN group contiguous (SBO = 1 KB) and MN groups 2 KB apart (LBO).
-// Measured (profiles/r01_tuning.md): same speed as the cp.async loaders (the kernel is bound by shared-memory
-// bandwidth: 6 MMAs x 12 KB of operand reads + 36 KB of fill per 768-cycle K-step), but one elected thread
-// per stage instead of four full warps of address arithmetic; L2 promotion must be <= 128 B (256 B: 46 us).
+// operand starting at column c0.  Rows are 256 bytes apart but NPASS * npass elements wide: they OVERLAP in
+// memory (cuTensorMapEncodeTiled accepts that), which is what materialises the im2col operand without ever
+// storing it.  Box = 64 elements x 16 K-rows, SWIZZLE_128B: it lands as 16 rows of 128 bytes with the
+// 16-byte chunk index XOR-ed with (row & 7) -- the wgmma operand layout, with the two 8-row K groups of one
+// 64-element MN group contiguous (SBO = 1 KB) and MN groups 2 KB apart (LBO).  One elected thread per
+// stage instead of four full warps of address arithmetic.
 struct ToepMaps {
     CUtensorMap x[NPLANE];
     CUtensorMap s[2][NPLANE];
@@ -113,8 +105,7 @@ __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // TMA: one thread arms the stage's mbarrier with the byte count, then issues 2-D tiled bulk-tensor copies
-// that complete on it.  With SWIZZLE_128B the box lands as rows of 128 bytes whose 16-byte chunk index is
-// XOR-ed with (row & 7) -- exactly the UMMA SWIZZLE_128B operand layout (scripts/tc/tma_probe.cu).
+// that complete on it.
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -125,79 +116,44 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* tm, in
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* tm) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tm)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "r"(cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols));
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc),
-        "r"(accumulate));
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc),
-        "r"(accumulate));
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// wgmma: fence before the first MMA that reads registers written by ordinary instructions (zeroed
+// accumulators, A fragments), commit closes a group, wait<N> leaves at most N groups in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// D[64 x 128] += A[64 x 16] * B[16 x 128], both operands MN-major in shared memory (fp32 accumulators:
+// thread t of the warpgroup holds d[i] at row 16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2), column
+// 8 (i / 4) + 2 (t % 4) + i % 2)
+__device__ __forceinline__ void wgmma_ss(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\nwgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(1));
 }
 
-// shared-memory matrix descriptor, MN-major, no swizzle: core matrix = 8 K-rows x 16 B (128 B
-// contiguous); consecutive 16-byte MN chunks are SBO bytes apart; 8-row K groups LBO bytes apart
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// the same with A from registers (four BF16 pairs per thread, the mma.m16n8k16 A layout per warp) and B
+// K-major in shared memory
+__device__ __forceinline__ void wgmma_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %69, 0;\nwgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(1));
+}
+
+// shared-memory matrix descriptor, SWIZZLE_128B.  MN-major: LBO = stride between 64-element MN groups,
+// SBO = stride between 8-row K groups.  K-major: SBO = stride between 8-row groups, LBO unused.
+__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;          // descriptor version (Blackwell)
-    return d;                        // base_offset 0, layout_type 0 = SWIZZLE_NONE
-}
-// MN-major, SWIZZLE_128B: LBO = stride between 64-element MN groups, SBO = stride between 8-row K groups
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return make_desc(saddr, lbo_bytes, sbo_bytes) | ((uint64_t)2 << 61);
-}
-
-// instruction descriptor: D f32, A/B tf32, both MN-major (kept for the probes)
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
-}
-// instruction descriptor: D f32, A/B bf16, both MN-major
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) |
-           ((uint32_t)(M >> 4) << 24);
+    d |= (uint64_t)1 << 62;          // layout type 1 = SWIZZLE_128B, base offset 0 (operands start on 1 KB boundaries)
+    return d;
 }
 
 struct __align__(16) ToepShared {
     uint64_t full[MAX_SLOTS];
     uint64_t empty[MAX_SLOTS];
-    uint64_t tmem_full[2];
-    uint64_t tmem_empty[2];
-    uint32_t tmem_base;
-    uint32_t pad;
 };
 
 // One unit of work of a CTA: an accumulation over K-steps [kbeg, kbeg + kcount) for one (problem, pass),
@@ -237,41 +193,34 @@ __device__ __forceinline__ ToepItem toep_item(const ToepParams& p, int it) {
     return r;
 }
 
-// DUAL: one item per CTA, the dominant b0*b0' chain and the five cross terms in separate accumulators
-// (long K ranges: LS correlations).  !DUAL: many short items per CTA, one accumulator per item, TMEM double
-// buffered so the diagonal-sum epilogue of item i overlaps the MMAs of item i + 1 (CAF Doppler blocks).
-// Warps 0-3 and 9-12: epilogue; warp 4: MMA issue; warps 5-8: loaders.
-// dynamic shared memory: [stages x {A_b0, A_b1, A_b2, B_b0, B_b1, B_b2}] [8 x skew] [8 x 2 x HT floats]
+// DUAL: the dominant b0*b0' chain and the five 2^-8-smaller cross terms in separate accumulators, so the
+// rounding of the long chain is not mixed into the small terms (long K ranges: LS correlations).  !DUAL:
+// one accumulator (many short items per CTA: CAF Doppler blocks); the producers run ahead into the next
+// item while the consumers sum the diagonals of the current one.
+// dynamic shared memory: [stages x {A_b0, A_b1, A_b2, B_b0, B_b1, B_b2}] [2 x accumulator tile] [8 x 2 x HT floats]
 template <bool DUAL, bool TMA>
 __global__ void __launch_bounds__(THREADS, 1) toepcorr_kernel(const __grid_constant__ ToepParams p, const __grid_constant__ ToepMaps maps) {
     extern __shared__ __align__(1024) uint8_t tsm[];
     __shared__ ToepShared sh;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const bool is_loader = warp > NUM_EPI_WARPS && warp <= NUM_EPI_WARPS + NUM_LOAD_WARPS;
-    const bool is_mma = warp == NUM_EPI_WARPS;
+    const bool is_loader = warp >= 4 * NUM_MMA_WG;
 
     uint8_t* stage_base = tsm;
-    float* skew = reinterpret_cast<float*>(tsm + OPERAND_BYTES);                     // [8][SKEW_FLOATS]
-    float* cacc = skew + EPI_PARTS * SKEW_FLOATS;                                    // [8][2][HT]
+    float* tiles = reinterpret_cast<float*>(tsm + OPERAND_BYTES);                    // [2][TILE_FLOATS]
+    float* cacc = tiles + NUM_MMA_WG * TILE_FLOATS;                                  // [8][2][HT]
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < MAX_SLOTS; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&sh.tmem_full[b], 1); mbar_init(&sh.tmem_empty[b], EPI_PARTS); }
+        for (int s = 0; s < MAX_SLOTS; ++s) { mbar_init(&sh.full[s], 1); mbar_init(&sh.empty[s], NUM_MMA_WG); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (is_mma) tmem_alloc(&sh.tmem_base, TMEM_COLS);
     for (int i = threadIdx.x; i < EPI_PARTS * 2 * p.HT; i += blockDim.x) cacc[i] = 0.f;
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = sh.tmem_base;
-    if (p.debug_clk && blockIdx.x == 0 && threadIdx.x == 0) p.debug_clk[0] = clock64();
 
     if (TMA && is_loader) {
         // ======================= TMA producers: lane 0 of loader warp w owns pipeline stage w.  Per K-step: arm
-        // the stage's mbarrier with 36 KB, then 18 bulk-tensor copies (per plane: 2 boxes of the x rows, 4 boxes
+        // the stage's mbarrier with 24 KB, then 12 bulk-tensor copies (per plane: 2 boxes of the x rows, 2 boxes
         // of the overlapping s rows).
-        const int lw = warp - NUM_EPI_WARPS - 1;
+        const int lw = warp - 4 * NUM_MMA_WG;
         if (lane == 0) {
 #pragma unroll
             for (int pl = 0; pl < NPLANE; ++pl) { tma_prefetch_desc(&maps.x[pl]); tma_prefetch_desc(&maps.s[0][pl]); tma_prefetch_desc(&maps.s[1][pl]); }
@@ -300,11 +249,9 @@ __global__ void __launch_bounds__(THREADS, 1) toepcorr_kernel(const __grid_const
         }
     } else if (is_loader) {
         // ======================= loaders: 16-byte cp.async into 128B-swizzled MN-major tiles.
-        // Loader warp w owns pipeline stage w: it issues the whole 36 KB stage, waits for ITS copies only,
-        // publishes them to the async proxy and arrives.  (A fence after cp.async.wait_group N > 0 also
-        // waits for the younger groups of the same thread and collapses the pipeline: measured 2300
-        // cycles per stage instead of ~600.)
-        const int lw = warp - NUM_EPI_WARPS - 1;                 // 0..3 = stage
+        // Loader warp w owns pipeline stage w: it issues the whole 24 KB stage, waits for ITS copies only,
+        // publishes them to the async proxy and arrives.
+        const int lw = warp - 4 * NUM_MMA_WG;                    // 0..3 = stage
         const int ch = lane & 7;                                 // 16-byte chunk inside a 128-byte row
         const int r4 = lane >> 3;                                // 0..3: row inside a group of four
         int g = 0;                                               // K-steps issued by the CTA so far
@@ -340,103 +287,93 @@ __global__ void __launch_bounds__(THREADS, 1) toepcorr_kernel(const __grid_const
                 if (lane == 0) mbar_arrive(&sh.full[lw]);
             }
         }
-    } else if (is_mma) {
-        // ======================= MMA issuer (one elected lane)
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_bf16(128, NPASS);
-            int g = 0;
-            for (int it = 0;; ++it) {
-                const ToepItem item = toep_item(p, it);
-                if (!item.valid) break;
-                const int buf = DUAL ? 0 : (it & 1);
-                if (!DUAL && it >= 2) mbar_wait(&sh.tmem_empty[buf], ((it >> 1) - 1) & 1);
-                tc_fence_after();
-                const uint32_t acc0 = tmem + (DUAL ? 0 : buf * NPASS);
-                const uint32_t acc1 = DUAL ? tmem + NPASS : acc0;
-                for (int t = 0; t < item.kcount; ++t, ++g) {
-                    const int s = g & (STAGES - 1);
-                    mbar_wait(&sh.full[s], (g / STAGES) & 1);
-                    tc_fence_after();
-                    if (p.debug_clk && blockIdx.x == 0 && g == 0) p.debug_clk[1] = clock64();
-                    const uint32_t a0 = smem_u32(stage_base + s * STAGE_BYTES);
-                    const uint32_t b0 = a0 + NPLANE * A_BYTES;
-                    uint64_t da[NPLANE], db[NPLANE];
-#pragma unroll
-                    for (int pl = 0; pl < NPLANE; ++pl) {
-                        da[pl] = make_desc_sw128(a0 + pl * A_BYTES, TMA ? TMA_LBO : MN_LBO, TMA ? TMA_SBO : A_SBO);
-                        db[pl] = make_desc_sw128(b0 + pl * B_BYTES, TMA ? TMA_LBO : MN_LBO, TMA ? TMA_SBO : B_SBO);
-                    }
-                    // The tensor core truncates once per MMA when it adds into the fp32 accumulator (measured
-                    // bias ~ -steps * 2^-25 relative).  DUAL keeps the dominant b0*b0' chain alone in
-                    // accumulator 0 (one truncation per K-step); the five 2^-8-smaller cross terms go to
-                    // accumulator 1 where their truncations are 256x smaller.
-                    umma_f16(acc0, da[0], db[0], idesc, t > 0);
-                    umma_f16(acc1, da[0], db[1], idesc, DUAL ? (t > 0) : 1);
-                    umma_f16(acc1, da[1], db[0], idesc, 1);
-                    umma_f16(acc1, da[0], db[2], idesc, 1);
-                    umma_f16(acc1, da[2], db[0], idesc, 1);
-                    umma_f16(acc1, da[1], db[1], idesc, 1);
-                    umma_commit(&sh.empty[s]);                   // frees the stage when these MMAs retire
-                }
-                umma_commit(&sh.tmem_full[buf]);
-                if (p.debug_clk && blockIdx.x == 0) { p.debug_clk[2] = clock64(); if (it < 8) p.debug_clk[16 + it] = clock64(); }
-            }
-        }
-        __syncwarp();
     } else {
-        // ======================= epilogue (8 warps): TMEM -> diagonal sums -> one partial row per item
-        const int part = warp < NUM_EPI_WARPS ? warp : NUM_EPI_WARPS + (warp - (NUM_EPI_WARPS + 1 + NUM_LOAD_WARPS));
-        const int quad = warp & 3;                               // TMEM lane quadrant this warp may touch
-        const int jbeg = part < NUM_EPI_WARPS ? 0 : NPASS / 2, jend = jbeg + NPASS / 2;
-        const int etid = part * 32 + lane;                       // 0..255 among the epilogue threads
-        float* sk = skew + part * SKEW_FLOATS;
-        float* cre = cacc + (part * 2 + 0) * p.HT;
-        float* cim = cacc + (part * 2 + 1) * p.HT;
+        // ======================= consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile
+        const int wg = warp >> 2, wq = warp & 3;
+        const bool leader = (threadIdx.x & 127) == 0;
+        const uint32_t lbo = TMA ? TMA_LBO : MN_LBO;
+        const uint32_t sbo_a = TMA ? TMA_SBO : A_SBO, sbo_b = TMA ? TMA_SBO : B_SBO;
+        float* tile = tiles + wg * TILE_FLOATS;                  // [column][row], leading dimension TILE_LD
+        float* cre = cacc + (warp * 2 + 0) * p.HT;
+        float* cim = cacc + (warp * 2 + 1) * p.HT;
+        int g = 0;
         for (int it = 0;; ++it) {
             const ToepItem item = toep_item(p, it);
             if (!item.valid) break;
-            const int buf = DUAL ? 0 : (it & 1);
-            mbar_wait(&sh.tmem_full[buf], DUAL ? 0 : ((it >> 1) & 1));
-            tc_fence_after();
-            if (p.debug_clk && blockIdx.x == 0 && etid == 0 && it == 0) p.debug_clk[3] = clock64();
-            const uint32_t acc0 = tmem + (DUAL ? 0 : buf * NPASS);
-            for (int j0 = jbeg; j0 < jend; j0 += 32) {
+            float acc0[64];
+            float acc1[DUAL ? 64 : 1];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc0[i] = 0.f;
+            if constexpr (DUAL) {
+#pragma unroll
+                for (int i = 0; i < 64; ++i) acc1[i] = 0.f;
+            }
+            for (int t = 0; t < item.kcount; ++t, ++g) {
+                const int s = g & (STAGES - 1);
+                mbar_wait(&sh.full[s], (g / STAGES) & 1);
+                const uint32_t a0 = smem_u32(stage_base + s * STAGE_BYTES) + (uint32_t)wg * lbo;   // MN group wg of A
+                const uint32_t b0 = smem_u32(stage_base + s * STAGE_BYTES) + NPLANE * A_BYTES;
+                uint64_t da[NPLANE], db[NPLANE];
+#pragma unroll
+                for (int pl = 0; pl < NPLANE; ++pl) {
+                    da[pl] = make_desc_sw128(a0 + pl * A_BYTES, lbo, sbo_a);
+                    db[pl] = make_desc_sw128(b0 + pl * B_BYTES, lbo, sbo_b);
+                }
+                wgmma_fence();
+                wgmma_ss(acc0, da[0], db[0]);
+                if constexpr (DUAL) {
+                    wgmma_ss(acc1, da[0], db[1]);
+                    wgmma_ss(acc1, da[1], db[0]);
+                    wgmma_ss(acc1, da[0], db[2]);
+                    wgmma_ss(acc1, da[2], db[0]);
+                    wgmma_ss(acc1, da[1], db[1]);
+                } else {
+                    wgmma_ss(acc0, da[0], db[1]);
+                    wgmma_ss(acc0, da[1], db[0]);
+                    wgmma_ss(acc0, da[0], db[2]);
+                    wgmma_ss(acc0, da[2], db[0]);
+                    wgmma_ss(acc0, da[1], db[1]);
+                }
+                wgmma_commit();
+                if (t > 0) {                                     // the previous K-step's MMAs have read their stage
+                    wgmma_wait<1>();
+                    if (leader) mbar_arrive(&sh.empty[(g - 1) & (STAGES - 1)]);
+                }
+            }
+            wgmma_wait<0>();
+            if (leader) mbar_arrive(&sh.empty[(g - 1) & (STAGES - 1)]);
+            // accumulators -> this warpgroup's tile (column-major: the diagonal walk below is conflict-free)
+#pragma unroll
+            for (int i = 0; i < 64; ++i) {
+                const int r = wq * 16 + (lane >> 2) + 8 * ((i >> 1) & 1);
+                const int col = (i >> 2) * 8 + 2 * (lane & 3) + (i & 1);
+                float v = acc0[i];
+                if constexpr (DUAL) v += acc1[i];
+                tile[col * TILE_LD + r] = v;
+            }
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+            // diagonal sums of 32 x 32 sub-tiles: the warp takes two of its warpgroup's eight
+#pragma unroll 1
+            for (int k = 0; k < 2; ++k) {
+                const int idx = wq + 4 * k;
+                const int rq = idx >> 2, cq = idx & 3;
                 // real diagonal delta = base + dd - 31, dd = jj - l + 31 in [0, 62]; wanted: -1 <= delta <= 2*nlag - 1
-                const int base = item.pass * NPASS + j0 - quad * 32;
+                const int base = item.pass * NPASS + cq * 32 - (wg * 64 + rq * 32);
                 if (base + 31 < -1 || base - 31 > 2 * p.nlag - 1) continue;      // tile entirely outside the lag band
-                const bool dbg = p.debug_clk && blockIdx.x == 0 && etid == 0 && it == 0 && j0 == jbeg + 32;
-                if (dbg) p.debug_clk[8] = clock64();
-                uint32_t v[32];
-                tmem_ld32(acc0 + ((uint32_t)(quad * 32) << 16) + (uint32_t)j0, v);
-                if (dbg) p.debug_clk[9] = clock64();
-                if (DUAL) {
-                    uint32_t v2[32];
-                    tmem_ld32(tmem + ((uint32_t)(quad * 32) << 16) + (uint32_t)(NPASS + j0), v2);
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj) v[jj] = __float_as_uint(__uint_as_float(v[jj]) + __uint_as_float(v2[jj]));
-                }
-                if (p.debug_tile && blockIdx.x == 0 && it == 0) {
-#pragma unroll
-                    for (int jj = 0; jj < 32; ++jj) p.debug_tile[(quad * 32 + lane) * NPASS + j0 + jj] = __uint_as_float(v[jj]);
-                }
-#pragma unroll
-                for (int jj = 0; jj < 32; ++jj) sk[jj * 33 + lane] = __uint_as_float(v[jj]);   // row stride 33: both phases conflict-free
-                __syncwarp();
-                if (dbg) p.debug_clk[10] = clock64();
+                const float* sk = tile + cq * 32 * TILE_LD + rq * 32;            // sk[jj * TILE_LD + l] = D[l][jj]
                 // For row l this lane needs column jj = dd - 31 + l of exactly one of its two diagonals
                 // (dd = lane: valid when l >= 31 - lane; dd = lane + 32: valid when l <= 30 - lane), so one
                 // load per row feeds both sums: 32 pipelined loads instead of 64 half-masked ones.
                 float se[2] = {0.f, 0.f}, so[2] = {0.f, 0.f};
 #pragma unroll
                 for (int l = 0; l < 32; ++l) {
-                    const float val = sk[((lane + l + 1) & 31) * 33 + l];
+                    const float val = sk[((lane + l + 1) & 31) * TILE_LD + l];
                     const bool hi = (l + lane <= 30);            // belongs to dd = lane + 32
                     if (l & 1) { so[1] += hi ? val : 0.f; so[0] += hi ? 0.f : val; }
                     else       { se[1] += hi ? val : 0.f; se[0] += hi ? 0.f : val; }
                 }
-                if (dbg) p.debug_clk[11] = clock64() + (long long)(se[0] + so[0] + se[1] + so[1] == 12345.678f);
-                // Scatter into this warp's private sums, branch-free (divergent read-modify-writes cost ~1000
-                // cycles per tile).  base is even, so delta = base + dd - 31 is even exactly on odd lanes:
+                // Scatter into this warp's private sums, branch-free.  base is even, so delta = base + dd - 31
+                // is even exactly on odd lanes:
                 //   odd lane : re[delta/2] += se + so
                 //   even lane: im[(delta+1)/2] += so   (odd rows)   then   im[(delta-1)/2] -= se   (even rows)
                 // Within a round all target addresses differ (dd and dd + 32 are 16 lags apart).
@@ -471,15 +408,11 @@ __global__ void __launch_bounds__(THREADS, 1) toepcorr_kernel(const __grid_const
                     if (ok[1]) *tgt[1] = e1 - se[1];
                     __syncwarp();
                 }
-                if (dbg) p.debug_clk[12] = clock64();
             }
-            tc_fence_before();
-            __syncwarp();
-            if (!DUAL && lane == 0) mbar_arrive(&sh.tmem_empty[buf]);        // this accumulator may be overwritten
             // combine the eight parts, write the row, clear the sums for the next item
-            asm volatile("bar.sync 2, %0;" ::"n"(EPI_PARTS * 32));
+            asm volatile("bar.sync 3, %0;" ::"n"(EPI_PARTS * 32) : "memory");
             float2* out = p.partial + (size_t)item.row * (size_t)p.HT;
-            for (int l = etid; l < p.HT; l += EPI_PARTS * 32) {
+            for (int l = threadIdx.x; l < p.HT; l += EPI_PARTS * 32) {
                 float re = 0.f, im = 0.f;
 #pragma unroll
                 for (int w = 0; w < EPI_PARTS; ++w) {
@@ -490,16 +423,10 @@ __global__ void __launch_bounds__(THREADS, 1) toepcorr_kernel(const __grid_const
                 }
                 out[l] = make_float2(re, im);
             }
-            asm volatile("bar.sync 2, %0;" ::"n"(EPI_PARTS * 32));
-            if (p.debug_clk && blockIdx.x == 0 && etid == 0) { if (it == 0) p.debug_clk[4] = clock64(); if (it < 8) p.debug_clk[24 + it] = clock64(); }
+            asm volatile("bar.sync 3, %0;" ::"n"(EPI_PARTS * 32) : "memory");
         }
     }
-    tc_fence_before();
     __syncthreads();
-    if (is_mma) {
-        tc_fence_after();
-        tmem_dealloc(tmem, TMEM_COLS);
-    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -639,7 +566,7 @@ __global__ void __launch_bounds__(256) tc_prep_kernel(const __grid_constant__ Pr
 }
 
 inline size_t toep_smem_bytes(int HT) {
-    return (size_t)OPERAND_BYTES + EPI_PARTS * SKEW_FLOATS * sizeof(float) + (size_t)EPI_PARTS * 2 * HT * sizeof(float);
+    return (size_t)OPERAND_BYTES + (size_t)NUM_MMA_WG * TILE_FLOATS * sizeof(float) + (size_t)EPI_PARTS * 2 * HT * sizeof(float);
 }
 
 }  // namespace tc

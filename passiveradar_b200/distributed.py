@@ -237,4 +237,4 @@ def stream_benchmark(pipe, ref_d, srv_d, maps_d, nframes_total, chunk, rank, wor
             "chunk_frames": chunk, "ingest_rank_sent_bytes": sent, "ingest_egress_GBps": round(sent / (ms * 1e-3) / 1e9, 1),
             "staging": "NCCL point-to-point (batch_isend_irecv) from rank 0 on a side stream, two alternating buffers per rank",
             "note": "frame f -> rank f % world; rank 0 holds the stream in HBM and also computes its own share; the limiter is "
-                    "rank 0's NVLink egress when ingest_egress_GBps approaches the ~770 GB/s peer-copy figure"}
+                    "rank 0's NVLink egress when ingest_egress_GBps approaches its peer-copy bandwidth"}

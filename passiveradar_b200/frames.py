@@ -1,4 +1,4 @@
-"""Frame pipeline: streams of CPI frames through  LS_Filter -> fast_xambg  on one B200.
+"""Frame pipeline: streams of CPI frames through  LS_Filter -> fast_xambg  on one H100.
 
 The reference processes one dask chunk (= one CPI frame) per task on a thread pool
 (``main.py:169-194``).  On the GPU the same independence is used differently: a

@@ -1,4 +1,4 @@
-"""Cross-ambiguity function on the B200 -- same call signature as the reference.
+"""Cross-ambiguity function on the H100 -- same call signature as the reference.
 
 Drop-in for ``passiveRadar.range_doppler_processing.fast_xambg``
 (reference ``passiveRadar/range_doppler_processing.py:12-90``).  The host side

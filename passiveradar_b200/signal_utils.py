@@ -1,4 +1,4 @@
-"""Front-end signal utilities on the B200 -- same call signatures as the reference.
+"""Front-end signal utilities on the H100 -- same call signatures as the reference.
 
 Drop-ins for ``passiveRadar.signal_utils.deinterleave_IQ`` (reference
 ``passiveRadar/signal_utils.py:19-22``), ``frequency_shift`` (``:24-27``) and ``resample``

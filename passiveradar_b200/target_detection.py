@@ -1,4 +1,4 @@
-"""Target detection on the B200 -- ``CFAR_2D`` with the reference's call signature
+"""Target detection on the H100 -- ``CFAR_2D`` with the reference's call signature
 (``passiveRadar/target_detection.py:683-703``).  No CPU fallback."""
 from __future__ import annotations
 

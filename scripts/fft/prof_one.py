@@ -1,4 +1,4 @@
-"""One batch of config-2 frames through FramePipeline.run_device (for ncu captures and launch lists).
+"""One batch of config-2 frames through FramePipeline.run_device (for profiler captures and launch lists).
 usage: prof_one.py [batch] [reps] [fft]"""
 import os
 import sys

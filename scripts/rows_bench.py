@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Device-resident timings of the rows either side of the hot path (SURVEY.md 8f), CUDA events on the
-launching stream, inputs already in HBM.  Prints one JSON object; summarised in profiles/r01_rows.md.
+launching stream, inputs already in HBM.  Prints one JSON object.
 
     python scripts/rows_bench.py [--reps 20]
 """

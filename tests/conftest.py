@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     config.addinivalue_line("markers", "slow: takes more than a few seconds on CPU")
 
 
@@ -22,7 +22,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="no CUDA device in this container (run under gpurun)")
+    skip = pytest.mark.skip(reason="no CUDA device on this machine")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)
@@ -31,7 +31,7 @@ def pytest_collection_modifyitems(config, items):
 @pytest.fixture(params=["fft", "direct"])
 def both_paths(request):
     """Run a GPU test once on the FFT-domain kernels (csrc/fftcorr.cuh, forced for every size they accept) and once on
-    the direct-form kernels (tcgen05 / FP32): both are shipped and selectable (include/prcore.h: prc_set_option)."""
+    the direct-form kernels (wgmma / FP32): both are shipped and selectable (include/prcore.h: prc_set_option)."""
     from passiveradar_b200 import _lib
     old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"))
     if request.param == "fft":
@@ -45,11 +45,14 @@ def both_paths(request):
 
 
 def record_parity(name, **values):
-    """Append per-stage parity figures of a GPU test to gpurun_out/r02_parity.json (copied to profiles/ by hand)."""
+    """Append per-stage parity figures of a GPU test to $PRC_PARITY_DIR/parity.json (nothing is written when the
+    variable is unset: the tests never write into the checkout)."""
     import json
-    out_dir = os.path.join(ROOT, "gpurun_out")
+    out_dir = os.environ.get("PRC_PARITY_DIR")
+    if not out_dir:
+        return
     os.makedirs(out_dir, exist_ok=True)
-    path = os.path.join(out_dir, "r02_parity.json")
+    path = os.path.join(out_dir, "parity.json")
     data = {}
     if os.path.exists(path):
         try:

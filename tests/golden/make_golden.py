@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """Generate the golden vectors under tests/golden/ by EXECUTING THE REFERENCE.
 
-Run in the build container (where /root/reference exists):
+Run with a checkout of the reference (Max-Manning/passiveRadar) named by PR_REFERENCE:
 
-    python tests/golden/make_golden.py [--big]
+    PR_REFERENCE=<reference checkout> python tests/golden/make_golden.py [--big]
 
 Every array written here is an output of the reference's own functions
 (``passiveRadar.range_doppler_processing.fast_xambg``,
 ``passiveRadar.clutter_removal.{LS_Filter, NLMS_filter}``) imported from
-``/root/reference`` -- nothing from ``oracle/`` or ``passiveradar_b200/csrc`` is
+the reference checkout -- nothing from ``oracle/`` or ``passiveradar_b200/csrc`` is
 involved, only the seeded input generator ``passiveradar_b200.synth``.
 
 Cases tagged ``literal`` call the reference untouched.  Cases tagged ``shim``
@@ -19,7 +19,8 @@ scipy/signal/_signaltools.py:5344-5347) instead of first running
 (16 s/lag at ndecim=3125, 46 s/lag at 4096).  The case ``xambg_shim_proof``
 stores both outputs for one input so the tests can assert they are identical.
 
-The GPU box has no /root/reference; it only ever reads the .npz files.
+The tests only ever read the .npz files (and tests/golden/reference_digests.json, the sha256 of a few
+cases as this script produced them from the reference).
 """
 from __future__ import annotations
 
@@ -35,7 +36,9 @@ import scipy.signal as signal
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.environ.get("PR_REFERENCE", "/root/reference"))
+if not os.environ.get("PR_REFERENCE"):
+    raise SystemExit("set PR_REFERENCE to a checkout of the reference (Max-Manning/passiveRadar)")
+sys.path.insert(0, os.environ["PR_REFERENCE"])
 
 from passiveRadar.range_doppler_processing import fast_xambg          # noqa: E402  (the reference)
 from passiveRadar.clutter_removal import LS_Filter, NLMS_filter, LS_Filter_Toeplitz, LS_Filter_Multiple   # noqa: E402  (the reference)

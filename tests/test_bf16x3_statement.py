@@ -1,4 +1,4 @@
-"""CPU statement of the two numerical ideas behind the tcgen05 kernels (csrc/toepcorr.cuh, csrc/firtc.cuh):
+"""CPU statement of the two numerical ideas behind the tensor-core (wgmma) kernels (csrc/toepcorr.cuh, csrc/firtc.cuh):
 (1) a float32 value split into three BF16 numbers and the six products of order <= 2 reproduce a float32
 product to ~2^-23; (2) the lag correlation of complex signals is the sum over the real diagonals of a GEMM on
 interleaved real data (the "Toeplitz GEMM").  Pure numpy, no GPU: it documents WHY the kernels can be exact."""

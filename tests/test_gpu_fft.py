@@ -1,7 +1,7 @@
 """GPU parity at the shapes round 1 left untested, on both shipped paths, plus the batched entry points and the
 re-entrancy the boundary promises (include/prcore.h; dask calls the operators from a thread pool, main.py:169-194).
 
-Per-stage figures go to gpurun_out/r02_parity.json (committed copy: profiles/r02_parity.json).
+Per-stage figures go to $PRC_PARITY_DIR/parity.json when that variable is set (tests/conftest.py:record_parity).
 """
 import concurrent.futures as cf
 import ctypes as C
@@ -280,7 +280,7 @@ def test_stream_frames_over_nccl_world2():
     import torch
     import torch.multiprocessing as mp
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         port = s.getsockname()[1]
