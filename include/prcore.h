@@ -187,6 +187,24 @@ int prc_xambg_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
                          int range_bins, int freq_bins, const void* window, prc_c64* out,
                          int mem_kind, int device, void* stream, unsigned flags);
 
+/* ---- gradient-adaptive lattice joint process estimator ------------------------------------------------
+ * prc_gal_jpe_frames_c64 replaces GAL_JPE(), reference passiveRadar/clutter_removal.py:251-364, on nframes
+ * independent frames (frame i at ref/srv/out + i*frame_stride; a single frame is nframes = 1): a lattice of
+ * lattice_len stages (gradient-adaptive reflection coefficients, step mu1, which the recurrence itself adapts
+ * and clamps at 5e-3) feeds an NLMS transversal filter of delay_line_len taps (step mu2).  peek = number of
+ * non-causal taps: sample n uses ref[n + peek].
+ *   out   : n samples per frame; the last peek + 1 are zero                              (:317-359)
+ *   k_out : nframes * delay_line_len final reflection coefficients, or NULL              (:361-362)
+ *   h_out : nframes * delay_line_len final transversal taps, or NULL                     (:361-362)
+ * Requires 1 <= lattice_len <= delay_line_len <= 4096 and peek >= 0 (PRC_E_INVALID otherwise).  The sample
+ * recurrence of a frame is serial: a frame runs on one warp (delay_line_len <= 256) or one CTA, and a batch
+ * of frames fills the GPU.  Arithmetic is complex64 with the reference's rounding points (DESIGN.md).
+ */
+int prc_gal_jpe_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                           int lattice_len, int delay_line_len, double mu1, double mu2, int peek,
+                           prc_c64* out, prc_c64* k_out, prc_c64* h_out,
+                           int mem_kind, int device, void* stream, unsigned flags);
+
 /* ---- run-time switches (also read once from the environment: PRC_FFT, PRC_FFT_MIN_N) ----------------
  *   "fft"        1 (default): LS correlations, clutter FIR and CAF block sums as FFT-domain block correlations
  *                (csrc/fftcorr.cuh);  0: direct form on wgmma / FP32 (csrc/toepcorr.cuh, firtc.cuh, lagstream.cuh)

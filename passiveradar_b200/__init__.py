@@ -2,7 +2,7 @@
 
 Drop-in operators with the reference's call signatures (Max-Manning/passiveRadar):
 
-    from passiveradar_b200 import fast_xambg, LS_Filter, NLMS_filter, block_NLMS
+    from passiveradar_b200 import fast_xambg, LS_Filter, NLMS_filter, block_NLMS, GAL_JPE
 
 and a device-resident frame pipeline for streams of CPI frames
 (``passiveradar_b200.frames.FramePipeline``).  All arithmetic runs in
@@ -11,12 +11,12 @@ this package never imports the CPU oracle and never falls back to the CPU.
 """
 from .range_doppler_processing import fast_xambg, direct_xambg            # noqa: F401
 from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # noqa: F401
-                              LS_Filter_Toeplitz, LS_Filter_Multiple)
+                              LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames)
 from .signal_utils import deinterleave_IQ, frequency_shift, resample, frontend            # noqa: F401
 from .target_detection import CFAR_2D            # noqa: F401
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
-           "LS_Filter_Multiple", "deinterleave_IQ", "frequency_shift", "resample", "frontend", "CFAR_2D"]
+           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend", "CFAR_2D"]
 __version__ = "0.1.0"
 
 

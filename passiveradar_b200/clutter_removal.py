@@ -1,7 +1,8 @@
 """Adaptive clutter cancellers on the H100 -- same call signatures as the reference.
 
 Drop-ins for ``passiveRadar.clutter_removal.LS_Filter`` (reference
-``passiveRadar/clutter_removal.py:6-56``) and ``NLMS_filter`` (``:189-249``), plus
+``passiveRadar/clutter_removal.py:6-56``), ``NLMS_filter`` (``:189-249``) and ``GAL_JPE``
+(``:251-364``; ``gal_jpe_frames`` runs a batch of frames in one call), plus
 ``block_NLMS`` (not in the reference; DESIGN.md defines it so that ``blockLen=1``
 is ``NLMS_filter``).  All arithmetic runs in ``libprcore.so``; no CPU fallback.
 """
@@ -87,6 +88,90 @@ def block_NLMS(refChannel, srvChannel, filterLen, mu, peek=10, blockLen=64, init
     if int(blockLen) < 1:
         raise ValueError("blockLen must be >= 1")
     return _nlms(refChannel, srvChannel, filterLen, mu, peek, blockLen, initialTaps, returnFilter, device)
+
+
+def _gal_args(latticeLen, delayLineLen, peek):
+    latticeLen, delayLineLen, peek = int(latticeLen), int(delayLineLen), int(peek)
+    if latticeLen > delayLineLen:
+        raise ValueError("Delay line order must be greater than or equal to the lattice filter order")
+    if latticeLen < 1:
+        raise ValueError(f"latticeLen must be >= 1, got {latticeLen}")
+    if peek < 0:
+        raise ValueError(f"peek must be >= 0, got {peek}")
+    return latticeLen, delayLineLen, peek
+
+
+def GAL_JPE(refChannel, srvChannel, latticeLen, delayLineLen, mu1, mu2, peek=10, return_filter=False, *, device=None):
+    '''Gradient adaptive lattice joint process estimator -- reference semantics, sample-serial.
+
+    A lattice of ``latticeLen`` stages (gradient-adaptive reflection coefficients, step size ``mu1``,
+    ballpark 1e-3) whitens the reference channel; its ``delayLineLen`` backward prediction errors (the
+    stages beyond ``latticeLen`` are a plain delay line) feed an NLMS transversal filter (step size
+    ``mu2``, ballpark 1e-2).  ``peek`` non-causal taps: sample n uses ``refChannel[n + peek]``.  As in the
+    reference, ``mu1`` adapts itself (``min(0.999 mu1 + 1e-8 e**2, 5e-3)``).
+
+    Returns ``srvChannelFiltered`` (complex64; the last ``peek + 1`` samples are zero) and, with
+    ``return_filter=True``, the final reflection coefficients ``k`` and transversal taps ``h``
+    (``delayLineLen`` complex64 values each).  Raises ``ValueError`` on a shape mismatch, on
+    ``latticeLen > delayLineLen`` and on ``latticeLen < 1``.
+
+    The inputs are rounded to complex64 first; ``mu1`` and ``mu2`` are taken as Python floats.  The reference's
+    arithmetic widens to complex128 part-way through the loop when it is handed complex128 channels; this one stays
+    complex64 with the reference's complex64 rounding points.  Delay lines up to 4096 taps.
+    '''
+    ref, srv = _pair(refChannel, srvChannel)
+    latticeLen, delayLineLen, peek = _gal_args(latticeLen, delayLineLen, peek)
+    n = ref.shape[0]
+    out = np.empty(n, dtype=np.complex64)
+    k = np.empty(delayLineLen, dtype=np.complex64)
+    h = np.empty(delayLineLen, dtype=np.complex64)
+    if n == 0:
+        k[:] = 0
+        h[:] = 0
+    else:
+        lib = _lib.load()
+        dev = _lib.current_device() if device is None else int(device)
+        st = lib.prc_gal_jpe_frames_c64(ref.ctypes.data, srv.ctypes.data, n, 1, n, latticeLen, delayLineLen,
+                                        float(mu1), float(mu2), peek, out.ctypes.data, k.ctypes.data, h.ctypes.data,
+                                        _lib.MEM_HOST, dev, None, 0)
+        _lib.check(st)
+    if return_filter:
+        return out, k, h
+    return out
+
+
+def gal_jpe_frames(ref_frames, srv_frames, latticeLen, delayLineLen, mu1, mu2, peek=10, return_filter=False, *,
+                   device=None):
+    '''``GAL_JPE`` on a batch of independent frames in one library call: row i of the 2-D host arrays
+    ``ref_frames`` / ``srv_frames`` (nframes x n) is one frame.  The recurrence of a frame is serial, so a single
+    frame occupies one warp (delay lines up to 256 taps) or one CTA of the GPU; a batch of frames is what fills it.
+
+    Returns ``out`` (nframes x n complex64) and, with ``return_filter=True``, ``k`` and ``h``
+    (nframes x delayLineLen complex64).  Row i equals ``GAL_JPE(ref_frames[i], srv_frames[i], ...)`` bit for bit.
+    '''
+    ref = np.asarray(ref_frames)
+    srv = np.asarray(srv_frames)
+    if ref.ndim != 2:
+        raise ValueError(f"ref_frames must be two-dimensional (nframes x n), got shape {ref.shape}")
+    if ref.shape != srv.shape:
+        raise ValueError('Input vectors must have the same length')
+    latticeLen, delayLineLen, peek = _gal_args(latticeLen, delayLineLen, peek)
+    ref = np.ascontiguousarray(ref, dtype=np.complex64)
+    srv = np.ascontiguousarray(srv, dtype=np.complex64)
+    nframes, n = ref.shape
+    out = np.zeros((nframes, n), dtype=np.complex64)
+    k = np.zeros((nframes, delayLineLen), dtype=np.complex64)
+    h = np.zeros((nframes, delayLineLen), dtype=np.complex64)
+    if nframes > 0 and n > 0:
+        lib = _lib.load()
+        dev = _lib.current_device() if device is None else int(device)
+        st = lib.prc_gal_jpe_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nframes, n, latticeLen, delayLineLen,
+                                        float(mu1), float(mu2), peek, out.ctypes.data, k.ctypes.data, h.ctypes.data,
+                                        _lib.MEM_HOST, dev, None, 0)
+        _lib.check(st)
+    if return_filter:
+        return out, k, h
+    return out
 
 
 def LS_Filter_Toeplitz(refChannel, srvChannel, filterLen, peek=10, return_filter=False, *, device=None):

@@ -29,6 +29,7 @@
 #include "detect.cuh"
 #include "nlms.cuh"
 #include "nlms_block.cuh"
+#include "gal.cuh"
 #include "fftcorr.cuh"
 
 namespace {
@@ -52,9 +53,9 @@ thread_local std::string g_err;
 std::atomic<uint64_t> g_launches{0};
 
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
-enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_COUNT };
+enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
-                                           "doppler_fft", "nlms", "misc"};
+                                           "doppler_fft", "nlms", "misc", "gal_jpe"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -130,7 +131,7 @@ struct Ctx {
     DBuf cafplane[6];         // bf16 planes of the tensor-core CAF: x[3], s[3]
     DBuf tcplane[9];          // bf16 planes of the tensor-core path: x[3], s0[3], s1[3]
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
-        nl_init, nl_taps;
+        nl_init, nl_taps, gal_k, gal_h;
     int tw_F = 0;
     int status_slot = 0;      // which int of `status` the direct-form Toeplitz solve reports to
     void* pin[2] = {nullptr, nullptr};      // page-locked bounce buffers for pageable host arrays (h2d / d2h below)
@@ -151,7 +152,7 @@ struct Ctx {
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP}) b->release();
         for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
-                        &tw, &pbuf, &status, &nl_init, &nl_taps})
+                        &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h})
             b->release();
         if (pin_ready) {
             for (int k = 0; k < 2; ++k) { cudaFreeHost(pin[k]); cudaEventDestroy(pin_ev[k]); pin[k] = nullptr; pin_ev[k] = nullptr; }
@@ -256,6 +257,7 @@ int set_kernel_attrs(int device) {
     CU(cudaFuncSetAttribute(nlms_block_kernel<1, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<2, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<4, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(gal_jpe_kernel<GAL_CTA_T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
 #define PRC_FFT_ATTRS(R3)                                                                                              \
     CU(cudaFuncSetAttribute(fftc::lscorr_fft_kernel<R3>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));           \
     CU(cudaFuncSetAttribute(fftc::taps_spectrum_kernel<R3>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));        \
@@ -1393,6 +1395,39 @@ int nlms_device(Ctx* c, const float2* ref, const float2* srv, long long n, int f
     return check_launch("nlms_kernel");
 }
 
+// GAL_JPE on bt.nf independent frames (gal.cuh): delay lines up to GAL_WARP_MAX_D taps run one frame per warp
+// (GAL_WARP_FRAMES frames per CTA, shuffles only), longer ones one frame per CTA of ceil(D / 256) warps
+int gal_check(long long n, int L, int D, int peek) {
+    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", n);
+    if (L < 1) return fail(PRC_E_INVALID, "lattice_len=%d invalid (must be >= 1)", L);
+    if (D < L) return fail(PRC_E_INVALID, "delay_line_len=%d must be >= lattice_len=%d", D, L);
+    if (D > GAL_MAX_D)
+        return fail(PRC_E_INVALID, "delay_line_len=%d exceeds the GAL_JPE kernel's maximum of %d", D, GAL_MAX_D);
+    if (peek < 0) return fail(PRC_E_INVALID, "peek=%d invalid", peek);
+    return PRC_OK;
+}
+
+int gal_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt, int L, int D, double mu1, double mu2,
+               int peek, float2* out, float2* k_out, float2* h_out) {
+    TRY(gal_check(n, L, D, peek));
+    GalParams p{};
+    p.ref = ref; p.srv = srv; p.out = out; p.k_out = k_out; p.h_out = h_out;
+    p.n = n; p.stride = bt.stride; p.nframes = bt.nf;
+    p.L = L; p.D = D; p.peek = peek; p.mu1 = mu1; p.mu2 = (float)mu2;
+    ProfScope ps(c, K_GAL);
+    if (D <= GAL_WARP_MAX_D) {
+        const int grid = ceil_div(bt.nf, GAL_WARP_FRAMES), threads = 32 * GAL_WARP_FRAMES;
+        if (D <= 32) gal_jpe_kernel<1, false><<<grid, threads, 0, c->stream>>>(p);
+        else if (D <= 64) gal_jpe_kernel<2, false><<<grid, threads, 0, c->stream>>>(p);
+        else if (D <= 128) gal_jpe_kernel<4, false><<<grid, threads, 0, c->stream>>>(p);
+        else gal_jpe_kernel<8, false><<<grid, threads, 0, c->stream>>>(p);
+        return check_launch("gal_jpe_kernel(warp)");
+    }
+    const int threads = 32 * ceil_div(D, 32 * GAL_CTA_T);
+    gal_jpe_kernel<GAL_CTA_T, true><<<bt.nf, threads, gal_smem(threads), c->stream>>>(p);
+    return check_launch("gal_jpe_kernel(cta)");
+}
+
 // ---- host <-> device copies of caller arrays.  dask hands the operators ordinary (pageable) numpy arrays from several
 // threads at once (main.py:169-194); cudaMemcpyAsync from pageable memory goes through the driver's own staging, one
 // copy at a time for the whole process.  Each workspace therefore owns two page-locked bounce buffers: the calling
@@ -1818,6 +1853,55 @@ int prc_nlms_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int n
         for (int fr = 0; fr < nframes; ++fr)
             TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
         if (taps_out) TRY(d2h(c, taps_out, c->nl_taps.p, mb * nframes, flags));
+    }
+    return finish(c, flags);
+}
+
+int prc_gal_jpe_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                           int lattice_len, int delay_line_len, double mu1, double mu2, int peek,
+                           prc_c64* out, prc_c64* k_out, prc_c64* h_out,
+                           int mem_kind, int device, void* stream, unsigned flags) {
+    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    TRY(gal_check(n, lattice_len, delay_line_len, peek));      // before any CUDA call
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    const size_t nb = (size_t)n * sizeof(float2);
+    const size_t db = (size_t)delay_line_len * sizeof(float2);
+    Batch bt;
+    bt.nf = nframes;
+    bt.stride = nframes > 1 ? frame_stride : n;
+    const float2* dref = reinterpret_cast<const float2*>(ref);
+    const float2* dsrv = reinterpret_cast<const float2*>(srv);
+    float2* dout = reinterpret_cast<float2*>(out);
+    float2* dk = reinterpret_cast<float2*>(k_out);
+    float2* dh = reinterpret_cast<float2*>(h_out);
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->ref.ensure(nb * nframes));
+        TRY(c->srv.ensure(nb * nframes));
+        TRY(c->clean.ensure(nb * nframes));
+        for (int fr = 0; fr < nframes; ++fr) {
+            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
+            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
+        }
+        if (k_out) { TRY(c->gal_k.ensure(db * nframes)); dk = c->gal_k.as<float2>(); }
+        if (h_out) { TRY(c->gal_h.ensure(db * nframes)); dh = c->gal_h.as<float2>(); }
+        dref = c->ref.as<float2>();
+        dsrv = c->srv.as<float2>();
+        dout = c->clean.as<float2>();
+        bt.stride = n;
+    }
+    TRY(gal_device(c, dref, dsrv, n, bt, lattice_len, delay_line_len, mu1, mu2, peek, dout, dk, dh));
+    if (mem_kind == PRC_MEM_HOST) {
+        const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
+        for (int fr = 0; fr < nframes; ++fr)
+            TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
+        if (k_out) TRY(d2h(c, k_out, c->gal_k.p, db * nframes, flags));
+        if (h_out) TRY(d2h(c, h_out, c->gal_h.p, db * nframes, flags));
     }
     return finish(c, flags);
 }
