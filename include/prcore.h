@@ -54,6 +54,7 @@ typedef struct prc_c64 { float re, im; } prc_c64;
 #define PRC_FLAG_ASYNC        1u   /* do not synchronise `stream` before returning */
 #define PRC_FLAG_WINDOW_F32   2u   /* `window` points at float, not double */
 #define PRC_FLAG_ABS_C64      4u   /* prc_cfar2d_f32: `x` is a complex64 map, |x| is used */
+#define PRC_FLAG_MAP_F64      8u   /* tracker entry points: maps are float64, not float32 */
 
 /* ---- lifecycle / diagnostics ------------------------------------------------ */
 int         prc_version(void);
@@ -259,6 +260,61 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
  */
 int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const float* thresh, float* cr_out,
                    uint8_t* det_out, int mem_kind, int device, void* stream, unsigned flags);
+
+/* ---- Kalman target trackers ------------------------------------------------------------------------
+ * Replace get_measurements(), multitarget_tracker() and simple_target_tracker(), reference
+ * passiveRadar/target_detection.py:164-681.  The records below are byte for byte the reference's NumPy
+ * dtypes (packed, every field 8 bytes): prc_kalman = kalman_filter_dtype, prc_track = target_track_dtype,
+ * prc_track_simple = target_track_dtype_simple.
+ *
+ * Maps: nseq sequences of nframes frames; frame i of sequence s is at maps + s*seq_stride + i*frame_stride
+ * (elements), row-major rows x cols like the reference's data[:, :, i] (rows = Doppler bins, cols = range
+ * bins).  float32, or float64 with PRC_FLAG_MAP_F64; arithmetic is float64 either way.  Maps must be finite.
+ * Candidates are ordered by strength, descending; equal strengths in descending position of the transformed
+ * frame (np.flip(np.argsort(s, kind="stable")); the reference's unstable sort leaves that order open).
+ *
+ * prc_get_measurements_frames: counts[s*nframes + i] = the frame's exact candidate count (up to rows*cols);
+ *   its candidates go to meas + (s*nframes + i) * 3 * meas_capacity as three rows of meas_capacity doubles:
+ *   range, Doppler, strength.  Only the first meas_capacity are written; meas_capacity = rows*cols never cuts.
+ * prc_multitarget_track_frames: history[(s*nframes + i)*n_tracks + t] = track t after frame i of sequence s.
+ *   0 <= n_tracks <= 64.
+ * prc_simple_track_frames: history[s*nframes + i] = the tracker state after frame i of sequence s.
+ * rows * cols <= 524288.
+ */
+typedef struct prc_kalman {
+    double x[4], P[16], F1[16], F2[16], Q[16], H[8], R[4], S[4];
+} prc_kalman;
+typedef struct prc_track {
+    int64_t status, lifetime;
+    double measurement[2], estimate[2], measurement_history[20];
+    prc_kalman kalman_state;
+} prc_track;
+typedef struct prc_track_simple {
+    double lock_mode[4], measurement[2];
+    int64_t measurement_idx[2];
+    double estimate[2], range_extent, doppler_extent;
+    prc_kalman kalman_state;
+} prc_track_simple;
+#ifdef __cplusplus
+static_assert(sizeof(prc_kalman) == 672, "prc_kalman must match kalman_filter_dtype");
+static_assert(sizeof(prc_track) == 880, "prc_track must match target_track_dtype");
+static_assert(sizeof(prc_track_simple) == 768, "prc_track_simple must match target_track_dtype_simple");
+#else
+_Static_assert(sizeof(prc_kalman) == 672, "prc_kalman must match kalman_filter_dtype");
+_Static_assert(sizeof(prc_track) == 880, "prc_track must match target_track_dtype");
+_Static_assert(sizeof(prc_track_simple) == 768, "prc_track_simple must match target_track_dtype_simple");
+#endif
+
+int prc_get_measurements_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                                int64_t frame_stride, double doppler_extent, double range_extent,
+                                int64_t meas_capacity, int32_t* counts, double* meas,
+                                int mem_kind, int device, void* stream, unsigned flags);
+int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                                 int64_t frame_stride, double doppler_extent, double range_extent, int n_tracks,
+                                 prc_track* history, int mem_kind, int device, void* stream, unsigned flags);
+int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                            int64_t frame_stride, double range_extent, double doppler_extent,
+                            prc_track_simple* history, int mem_kind, int device, void* stream, unsigned flags);
 
 #ifdef __cplusplus
 }

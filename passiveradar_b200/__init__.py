@@ -13,10 +13,14 @@ from .range_doppler_processing import fast_xambg, direct_xambg            # noqa
 from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # noqa: F401
                               LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames)
 from .signal_utils import deinterleave_IQ, frequency_shift, resample, frontend            # noqa: F401
-from .target_detection import CFAR_2D            # noqa: F401
+from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
+                               multitarget_tracker_frames, simple_tracker_frames, cfar_track,
+                               kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
-           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend", "CFAR_2D"]
+           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend", "CFAR_2D",
+           "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
+           "simple_tracker_frames", "cfar_track"]
 __version__ = "0.1.0"
 
 
@@ -37,7 +41,8 @@ def install(reference_package: str = "passiveRadar"):
     table = {
         "range_doppler_processing": {"fast_xambg": fast_xambg, "direct_xambg": direct_xambg},
         "signal_utils": {"deinterleave_IQ": deinterleave_IQ, "frequency_shift": frequency_shift, "resample": resample},
-        "target_detection": {"CFAR_2D": CFAR_2D},
+        "target_detection": {"CFAR_2D": CFAR_2D, "get_measurements": get_measurements,
+                             "multitarget_tracker": multitarget_tracker, "simple_target_tracker": simple_target_tracker},
         "clutter_removal": {"LS_Filter": LS_Filter, "NLMS_filter": NLMS_filter,
                             "LS_Filter_Toeplitz": LS_Filter_Toeplitz, "LS_Filter_Multiple": LS_Filter_Multiple},
     }

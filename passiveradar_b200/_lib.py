@@ -26,6 +26,7 @@ MEM_DEVICE = 1
 FLAG_ASYNC = 1
 FLAG_WINDOW_F32 = 2
 FLAG_ABS_C64 = 4
+FLAG_MAP_F64 = 8
 IQ_C64, IQ_I8, IQ_I16 = 0, 1, 2
 MIX_NONE, MIX_C64, MIX_C128, MIX_F64, MIX_FS64 = 0, 1, 2, 3, 4
 
@@ -84,7 +85,32 @@ SIGNATURES = {
                                    C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_cfar2d_f32": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_get_measurements_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                              C.c_double, C.c_double, C.c_int64, C.c_void_p, C.c_void_p,
+                                              C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_multitarget_track_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                               C.c_double, C.c_double, C.c_int, C.c_void_p,
+                                               C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_simple_track_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                          C.c_double, C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
 }
+
+
+# the tracker records of include/prcore.h (byte for byte the reference's NumPy dtypes)
+class PrcKalman(C.Structure):
+    _fields_ = [("x", C.c_double * 4), ("P", C.c_double * 16), ("F1", C.c_double * 16), ("F2", C.c_double * 16),
+                ("Q", C.c_double * 16), ("H", C.c_double * 8), ("R", C.c_double * 4), ("S", C.c_double * 4)]
+
+
+class PrcTrack(C.Structure):
+    _fields_ = [("status", C.c_int64), ("lifetime", C.c_int64), ("measurement", C.c_double * 2),
+                ("estimate", C.c_double * 2), ("measurement_history", C.c_double * 20), ("kalman_state", PrcKalman)]
+
+
+class PrcTrackSimple(C.Structure):
+    _fields_ = [("lock_mode", C.c_double * 4), ("measurement", C.c_double * 2), ("measurement_idx", C.c_int64 * 2),
+                ("estimate", C.c_double * 2), ("range_extent", C.c_double), ("doppler_extent", C.c_double),
+                ("kalman_state", PrcKalman)]
 
 _lib = None
 _lock = threading.Lock()

@@ -30,6 +30,7 @@
 #include "nlms.cuh"
 #include "nlms_block.cuh"
 #include "gal.cuh"
+#include "track.cuh"
 #include "fftcorr.cuh"
 
 namespace {
@@ -53,9 +54,11 @@ thread_local std::string g_err;
 std::atomic<uint64_t> g_launches{0};
 
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
-enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_COUNT };
+enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
+                K_TRK_SIMPLE, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
-                                           "doppler_fft", "nlms", "misc", "gal_jpe"};
+                                           "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
+                                           "track_multi", "track_simple"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -132,6 +135,9 @@ struct Ctx {
     DBuf tcplane[9];          // bf16 planes of the tensor-core path: x[3], s0[3], s1[3]
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
         nl_init, nl_taps, gal_k, gal_h;
+    DBuf trk_map, trk_plan, trk_stats, trk_slots, trk_out, trk_cnt;   // trackers: host maps, summation tree, per-frame
+                                                                      // mean / thr / count, candidate slots, results
+    int trk_plan_n = -1, trk_nnodes = 0, trk_nlevels = 0;             // map size trk_plan was built for, its shape
     int tw_F = 0;
     int status_slot = 0;      // which int of `status` the direct-form Toeplitz solve reports to
     void* pin[2] = {nullptr, nullptr};      // page-locked bounce buffers for pageable host arrays (h2d / d2h below)
@@ -152,8 +158,10 @@ struct Ctx {
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP}) b->release();
         for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
-                        &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h})
+                        &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
+                        &trk_slots, &trk_out, &trk_cnt})
             b->release();
+        trk_plan_n = -1;
         if (pin_ready) {
             for (int k = 0; k < 2; ++k) { cudaFreeHost(pin[k]); cudaEventDestroy(pin_ev[k]); pin[k] = nullptr; pin_ev[k] = nullptr; }
             pin_ready = false;
@@ -258,6 +266,12 @@ int set_kernel_attrs(int device) {
     CU(cudaFuncSetAttribute(nlms_block_kernel<2, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<4, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(gal_jpe_kernel<GAL_CTA_T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_MEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_MEAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<double, TRK_MODE_MEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<double, TRK_MODE_SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(track_meas_kernel<double, TRK_MODE_MEAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
 #define PRC_FFT_ATTRS(R3)                                                                                              \
     CU(cudaFuncSetAttribute(fftc::lscorr_fft_kernel<R3>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));           \
     CU(cudaFuncSetAttribute(fftc::taps_spectrum_kernel<R3>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));        \
@@ -1574,6 +1588,139 @@ int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batc
 
 bool bad_mem_kind(int k) { return k != PRC_MEM_HOST && k != PRC_MEM_DEVICE; }
 
+// ---- Kalman trackers (track.cuh) -----------------------------------------------------------------
+constexpr size_t TRK_SLOT_BUDGET = 256u << 20;     // candidate slots of one multi-tracker launch (bytes)
+
+// python slice [start:stop] of an axis of length len
+void py_slice(long long start, long long stop, long long len, int* lo, int* hi) {
+    if (start < 0) { start += len; if (start < 0) start = 0; } else if (start > len) start = len;
+    if (stop < 0) { stop += len; if (stop < 0) stop = 0; } else if (stop > len) stop = len;
+    *lo = (int)start;
+    *hi = (int)std::max(start, stop);
+}
+
+int trk_check(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride, int64_t frame_stride,
+              int mem_kind) {
+    if (!maps) return fail(PRC_E_INVALID, "maps must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
+    if ((long long)rows * cols > TRK_MAX_CELLS)
+        return fail(PRC_E_INVALID, "a %d x %d map exceeds the tracker kernels' maximum of %lld cells", rows, cols,
+                    TRK_MAX_CELLS);
+    if (nseq < 1 || nseq > 65535) return fail(PRC_E_INVALID, "nseq=%d outside [1, 65535]", nseq);
+    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (seq_stride < 0 || frame_stride < 0)
+        return fail(PRC_E_INVALID, "seq_stride=%lld frame_stride=%lld invalid", (long long)seq_stride, (long long)frame_stride);
+    return PRC_OK;
+}
+
+// NumPy's pairwise summation tree of n elements (split at n/2 rounded down to a multiple of 8 until <= 128),
+// breadth-first, followed by the first node of every depth; built once per map size and context
+int trk_plan(Ctx* c, int n) {
+    if (c->trk_plan_n == n) return PRC_OK;
+    std::vector<PwNode> nodes{PwNode{0, n, -1, 0}};
+    std::vector<int> level{0};
+    size_t lo = 0;
+    for (;;) {
+        const size_t hi = nodes.size();
+        for (size_t q = lo; q < hi; ++q) {
+            const PwNode nd = nodes[q];
+            if (nd.len <= 128) continue;
+            const int n2 = nd.len / 2 - (nd.len / 2) % 8;
+            nodes[q].left = (int)nodes.size();
+            nodes.push_back(PwNode{nd.off, n2, -1, 0});
+            nodes.push_back(PwNode{nd.off + n2, nd.len - n2, -1, 0});
+        }
+        if (nodes.size() == hi) break;
+        level.push_back((int)hi);
+        lo = hi;
+    }
+    level.push_back((int)nodes.size());
+    const size_t nb = nodes.size() * sizeof(PwNode), lb = level.size() * sizeof(int);
+    TRY(c->trk_plan.ensure(nb + lb));
+    CU(cudaMemcpyAsync(c->trk_plan.p, nodes.data(), nb, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(static_cast<char*>(c->trk_plan.p) + nb, level.data(), lb, cudaMemcpyHostToDevice, c->stream));
+    c->trk_plan_n = n;
+    c->trk_nnodes = (int)nodes.size();
+    c->trk_nlevels = (int)level.size() - 1;
+    return PRC_OK;
+}
+
+// maps -> device (frame-major, compact) when they are host arrays; fills the map part of mp
+int trk_stage(Ctx* c, const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+              int64_t frame_stride, int mem_kind, unsigned flags, TrkMapParams* mp) {
+    const size_t esz = (flags & PRC_FLAG_MAP_F64) ? 8 : 4;
+    const long long n = (long long)rows * cols;
+    *mp = TrkMapParams{};
+    mp->maps = maps;
+    mp->seq_stride = seq_stride;
+    mp->frame_stride = frame_stride;
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->trk_map.ensure((size_t)nseq * nframes * n * esz));
+        char* d = c->trk_map.as<char>();
+        const char* h = static_cast<const char*>(maps);
+        for (int s = 0; s < nseq; ++s) {
+            if (frame_stride == n) {
+                TRY(h2d(c, d + (size_t)s * nframes * n * esz, h + (size_t)s * seq_stride * esz, (size_t)nframes * n * esz, flags));
+                continue;
+            }
+            for (int f = 0; f < nframes; ++f)
+                TRY(h2d(c, d + ((size_t)s * nframes + f) * n * esz, h + ((size_t)s * seq_stride + (size_t)f * frame_stride) * esz,
+                        n * esz, flags));
+        }
+        mp->maps = d;
+        mp->seq_stride = (long long)nframes * n;
+        mp->frame_stride = n;
+    }
+    TRY(trk_plan(c, (int)n));
+    mp->rows = rows;
+    mp->cols = cols;
+    mp->n = (int)n;
+    mp->nframes = nframes;
+    mp->plan = c->trk_plan.as<PwNode>();
+    mp->level = reinterpret_cast<const int*>(c->trk_plan.as<PwNode>() + c->trk_nnodes);
+    mp->nnodes = c->trk_nnodes;
+    mp->nlevels = c->trk_nlevels;
+    // np.percentile(frame, 99.8), linear method: v = (n - 1) * 0.998, order statistics floor(v) and floor(v) + 1
+    const double v = (double)(n - 1) * (99.8 / 100.0);
+    mp->k = (int)std::floor(v);
+    mp->g = v - (double)mp->k;
+    py_slice(rows / 2 - 4, rows / 2 + 4, rows, &mp->dlo, &mp->dhi);
+    mp->n_unbanded = std::max(0, cols - 16) * (rows - (mp->dhi - mp->dlo));
+    // candidates sorted in shared memory: room for twice the usual count (n - 1 - k)
+    const int want = std::max(256, 2 * ((int)n - 1 - mp->k) + 64);
+    int cap = 256;
+    while (cap < want && cap < TRK_MAX_CAP) cap <<= 1;
+    mp->cap = cap;
+    return PRC_OK;
+}
+
+// bin centres: rpts = linspace(range_extent, 0, cols), dpts = linspace(-1 * doppler_extent, doppler_extent, rows)
+void trk_extent(TrkMapParams* mp, double doppler_extent, double range_extent) {
+    mp->rng_start = range_extent;
+    mp->dop_start = -1.0 * doppler_extent;
+    mp->dop_stop = doppler_extent;
+}
+
+size_t trk_smem(const TrkMapParams& mp, int mode) {
+    const size_t nv = ((size_t)mp.nnodes * 8 + 15) & ~(size_t)15;
+    return mode == TRK_MODE_MEAN ? nv : nv + (size_t)mp.cap * (sizeof(unsigned long long) + sizeof(int));
+}
+
+int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, int nseq) {
+    const size_t smem = trk_smem(mp, mode);
+    if (smem > SMEM_LIMIT) return fail(PRC_E_INVALID, "tracker measurement kernel needs %zu B of shared memory", smem);
+    const dim3 grid(nf, nseq);
+    ProfScope ps(c, K_TRK_MEAS);
+#define PRC_TRK_MEAS(T)                                                                                            \
+    if (mode == TRK_MODE_MEAN) track_meas_kernel<T, TRK_MODE_MEAN><<<grid, TRK_THREADS, smem, c->stream>>>(mp);   \
+    else if (mode == TRK_MODE_SLOTS) track_meas_kernel<T, TRK_MODE_SLOTS><<<grid, TRK_THREADS, smem, c->stream>>>(mp); \
+    else track_meas_kernel<T, TRK_MODE_MEAS><<<grid, TRK_THREADS, smem, c->stream>>>(mp);
+    if (f64) { PRC_TRK_MEAS(double) } else { PRC_TRK_MEAS(float) }
+#undef PRC_TRK_MEAS
+    return check_launch("track_meas_kernel");
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2260,6 +2407,137 @@ int prc_direct_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
     }
     TRY(direct_xambg_device(c, dref, dsrv, n, range_bins, freq_bins, sample_rate, dout));
     if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, ob, flags));
+    return finish(c, flags);
+}
+
+int prc_get_measurements_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                                int64_t frame_stride, double doppler_extent, double range_extent,
+                                int64_t meas_capacity, int32_t* counts, double* meas,
+                                int mem_kind, int device, void* stream, unsigned flags) {
+    TRY(trk_check(maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind));
+    if (!counts) return fail(PRC_E_INVALID, "counts must not be NULL");
+    if (meas_capacity < 0 || (meas_capacity > 0 && !meas))
+        return fail(PRC_E_INVALID, "meas_capacity=%lld needs a meas buffer", (long long)meas_capacity);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    TrkMapParams mp;
+    TRY(trk_stage(c, maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind, flags, &mp));
+    trk_extent(&mp, doppler_extent, range_extent);
+    const size_t nfr = (size_t)nseq * nframes;
+    const size_t ob = nfr * 3 * (size_t)meas_capacity * sizeof(double);
+    TRY(c->trk_stats.ensure(nfr * 2 * sizeof(double)));
+    mp.mean = c->trk_stats.as<double>();
+    mp.thr = mp.mean + nfr;
+    mp.count = counts;
+    mp.out = meas;
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->trk_cnt.ensure(nfr * sizeof(int)));
+        TRY(c->trk_out.ensure(ob));
+        mp.count = c->trk_cnt.as<int>();
+        mp.out = c->trk_out.as<double>();
+    }
+    mp.f0 = 0;
+    mp.out_cap = meas_capacity;
+    mp.out_nf = nframes;
+    TRY(trk_meas_launch(c, mp, (flags & PRC_FLAG_MAP_F64) != 0, TRK_MODE_MEAS, nframes, nseq));
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(d2h(c, counts, mp.count, nfr * sizeof(int), flags));
+        if (ob) TRY(d2h(c, meas, mp.out, ob, flags));
+    }
+    return finish(c, flags);
+}
+
+int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                                 int64_t frame_stride, double doppler_extent, double range_extent, int n_tracks,
+                                 prc_track* history, int mem_kind, int device, void* stream, unsigned flags) {
+    TRY(trk_check(maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind));
+    if (n_tracks < 0 || n_tracks > TRK_MAX_TRACKS)
+        return fail(PRC_E_INVALID, "n_tracks=%d outside [0, %d], the multi-target tracker's maximum", n_tracks,
+                    TRK_MAX_TRACKS);
+    if (n_tracks > 0 && !history) return fail(PRC_E_INVALID, "history must not be NULL");
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (n_tracks == 0) return finish(c, flags);
+    TrkMapParams mp;
+    TRY(trk_stage(c, maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind, flags, &mp));
+    trk_extent(&mp, doppler_extent, range_extent);
+    const bool f64 = (flags & PRC_FLAG_MAP_F64) != 0;
+    const size_t nfr = (size_t)nseq * nframes;
+    const size_t slot = 3 * (size_t)mp.cap * sizeof(double);
+    const int fc = (int)std::max<size_t>(1, std::min<size_t>(nframes, TRK_SLOT_BUDGET / (slot * nseq)));
+    TRY(c->trk_stats.ensure(nfr * (2 * sizeof(double) + sizeof(int))));
+    TRY(c->trk_slots.ensure((size_t)nseq * fc * slot));
+    mp.mean = c->trk_stats.as<double>();
+    mp.thr = mp.mean + nfr;
+    mp.count = reinterpret_cast<int*>(mp.thr + nfr);
+    mp.out = c->trk_slots.as<double>();
+    mp.out_cap = mp.cap;
+    mp.out_nf = fc;
+    const size_t hb = nfr * n_tracks * sizeof(prc_track);
+    prc_track* dh = history;
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->trk_out.ensure(hb));
+        dh = c->trk_out.as<prc_track>();
+    }
+    for (int f0 = 0; f0 < nframes; f0 += fc) {
+        const int nf = std::min(fc, nframes - f0);
+        mp.f0 = f0;
+        TRY(trk_meas_launch(c, mp, f64, TRK_MODE_SLOTS, nf, nseq));
+        TrkMultiParams tp{};
+        tp.m = mp;
+        tp.f64 = f64 ? 1 : 0;
+        tp.hist = dh;
+        tp.n_tracks = n_tracks;
+        tp.f0 = f0;
+        tp.f1 = f0 + nf;
+        tp.slots = mp.out;
+        tp.fc = fc;
+        {
+            ProfScope ps(c, K_TRK_MULTI);
+            track_multi_kernel<<<nseq, 32, 0, c->stream>>>(tp);
+        }
+        TRY(check_launch("track_multi_kernel"));
+    }
+    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, history, dh, hb, flags));
+    return finish(c, flags);
+}
+
+int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int nframes, int64_t seq_stride,
+                            int64_t frame_stride, double range_extent, double doppler_extent,
+                            prc_track_simple* history, int mem_kind, int device, void* stream, unsigned flags) {
+    TRY(trk_check(maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind));
+    if (!history) return fail(PRC_E_INVALID, "history must not be NULL");
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    TrkMapParams mp;
+    TRY(trk_stage(c, maps, rows, cols, nseq, nframes, seq_stride, frame_stride, mem_kind, flags, &mp));
+    const bool f64 = (flags & PRC_FLAG_MAP_F64) != 0;
+    const size_t nfr = (size_t)nseq * nframes;
+    TRY(c->trk_stats.ensure(nfr * sizeof(double)));
+    mp.mean = c->trk_stats.as<double>();
+    TRY(trk_meas_launch(c, mp, f64, TRK_MODE_MEAN, nframes, nseq));
+    const size_t hb = nfr * sizeof(prc_track_simple);
+    prc_track_simple* dh = history;
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->trk_out.ensure(hb));
+        dh = c->trk_out.as<prc_track_simple>();
+    }
+    TrkSimpleParams sp{};
+    sp.m = mp;
+    sp.hist = dh;
+    sp.range_extent = range_extent;
+    sp.doppler_extent = doppler_extent;
+    py_slice(250, 260, rows, &sp.zlo, &sp.zhi);
+    {
+        ProfScope ps(c, K_TRK_SIMPLE);
+        if (f64) track_simple_kernel<double><<<nseq, TRK_SIMPLE_THREADS, 0, c->stream>>>(sp);
+        else track_simple_kernel<float><<<nseq, TRK_SIMPLE_THREADS, 0, c->stream>>>(sp);
+    }
+    TRY(check_launch("track_simple_kernel"));
+    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, history, dh, hb, flags));
     return finish(c, flags);
 }
 

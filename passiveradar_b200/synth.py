@@ -79,3 +79,31 @@ def raw_iq(n, kind="int8", seed=11):
     if kind == "float32":
         return rng.standard_normal(2 * n).astype(np.float32)
     raise ValueError(f"unknown raw IQ kind {kind!r}")
+
+
+def track_maps(seed, rows, cols, T, targets=4):
+    """Seeded (T, rows, cols) float32 maps of the detector-output kind for the trackers: a Rayleigh(1) background
+    plus point targets.  ``targets`` is a count (drawn from the seed) or a sequence of
+    (row0, col0, row_rate, col_rate, amplitude, t_on, t_off): a target at (row0 + row_rate t, col0 + col_rate t)
+    (row = Doppler bin, wrapped; col = range bin, dropped outside the map) with a half-amplitude cross around it,
+    present for t_on <= t < t_off.  Targets move, cross, appear and vanish."""
+    rng = np.random.default_rng(seed)
+    maps = rng.rayleigh(1.0, size=(T, rows, cols)).astype(np.float32)
+    if isinstance(targets, (int, np.integer)):
+        spec = []
+        for _ in range(int(targets)):
+            on = int(rng.integers(0, max(1, T // 3)))
+            spec.append((rng.uniform(0, rows), rng.uniform(10, max(11, cols - 10)), rng.uniform(-0.4, 0.4),
+                         rng.uniform(-0.3, 0.3), rng.uniform(12, 40), on, int(rng.integers(on + 1, T + 1))))
+        targets = spec
+    for r0, c0, vr, vc, amp, on, off in targets:
+        for t in range(int(on), min(int(off), T)):
+            r = int(np.floor(r0 + vr * t + 0.5)) % rows
+            c = int(np.floor(c0 + vc * t + 0.5))
+            if not 0 <= c < cols:
+                continue
+            maps[t, r, c] += np.float32(amp)
+            for dr, dc in ((1, 0), (-1, 0), (0, 1), (0, -1)):
+                if 0 <= c + dc < cols:
+                    maps[t, (r + dr) % rows, c + dc] += np.float32(0.5 * amp)
+    return maps
