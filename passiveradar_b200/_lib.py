@@ -165,7 +165,11 @@ def check(status: int):
 
 
 def set_option(name: str, value: int):
-    """Run-time switch of the library (include/prcore.h: "fft", "fft_min_n")."""
+    """Run-time switch of the library (include/prcore.h: "fft", "fft_min_n", "caf_wave").
+
+    ``get_option`` also reads the environment switches the library latched when it started ("tma", "tma_l2", "tc",
+    "tc_caf", "tc_fir", "stream", "packed", "tile", "nlms_block", "tune_nchunk", "tune_g") and "tma_active" (1 when
+    toepcorr_kernel uses TMA producers).  Those names are read-only: setting one raises PrcoreError."""
     check(load().prc_set_option(name.encode(), int(value)))
 
 

@@ -11,8 +11,11 @@
 //   * inside its range a CTA walks sub-chunks of <= G*steps*TI samples; sub-chunk k+1 is copied
 //     global -> shared with cp.async (LDGSTS, zero-fill outside the signal) while sub-chunk k is in
 //     the MAC loop: staging never leaves the math pipe idle;
-//   * accumulators stay in registers across sub-chunks; the cross-group reduction and the partial
-//     row are paid once per piece, not once per 1-2k samples.
+//   * the register accumulators hold one sub-chunk (<= steps*TI samples per thread); after each
+//     sub-chunk a thread folds them into its own slot of the reduction scratch with a compensated
+//     (Kahan) sum, so the FP32 error does not grow with the length of a piece (one CTA may walk a
+//     whole 2**20-sample channel: PRC_TUNE_NCHUNK=1); the cross-group reduction and the partial row
+//     are paid once per piece, not once per 1-2k samples.
 // x must already carry its weights (ref, or ref*window written by weight_kernel); the tap-weighted
 // decimator of fast_xambg(shortFilt=False) keeps using lagcorr_kernel.
 #pragma once
@@ -87,9 +90,11 @@ __global__ void __launch_bounds__((TI * TD > 100) ? 256 : 512) lagstream_kernel(
     const int prob = blockIdx.y;
     const int HT = p.H * TD;
     const int Lmax = p.G * p.steps * TI;
-    // shared layout: two staging buffers {x[Lmax], s[Lmax + HT]} and the reduction scratch [G][HT]
+    // shared layout: two staging buffers {x[Lmax], s[Lmax + HT]}, the per-thread sums [G][HT] (thread (g, h) owns
+    // entries g*HT + h*TD .. + TD - 1; the flush reduces them over g) and their Kahan compensations [G][HT]
     const int bufsz = 2 * Lmax + HT;
     float2* red = smem + 2 * bufsz;
+    float2* comp = red + p.G * HT;
 
     const long long q0 = (long long)blockIdx.x * p.per_cta;
     long long q1 = q0 + p.per_cta;
@@ -128,6 +133,11 @@ __global__ void __launch_bounds__((TI * TD > 100) ? 256 : 512) lagstream_kernel(
     const int h = tid % p.H;
     const int g = tid / p.H;
     const bool active = g < p.G;
+    const int own = g * HT + h * TD;       // this thread's slots of red / comp
+    if (active) {
+#pragma unroll
+        for (int v = 0; v < TD; ++v) { red[own + v] = make_float2(0.f, 0.f); comp[own + v] = make_float2(0.f, 0.f); }
+    }
 
     long long q = q0;
     SubChunk cur = next_subchunk<TI>(p, q, q1);
@@ -143,29 +153,36 @@ __global__ void __launch_bounds__((TI * TD > 100) ? 256 : 512) lagstream_kernel(
             const float2* buf = smem + b * bufsz;
             const int Sg = cur.steps * TI;
             slide_mac2n<TI, TD>(A1, A2, buf + g * Sg, buf + Lmax + g * Sg + h * TD, cur.steps);
+#pragma unroll
+            for (int v = 0; v < TD; ++v) {      // red += sub-chunk sum, compensated (only this thread touches its slots)
+                const float2 a = make_float2(A1[v].x + A2[v].y, A2[v].x - A1[v].y);
+                const float2 sm = red[own + v], c = comp[own + v];
+                const float2 y = make_float2(a.x - c.x, a.y - c.y);
+                const float2 t = make_float2(sm.x + y.x, sm.y + y.y);
+                comp[own + v] = make_float2((t.x - sm.x) - y.x, (t.y - sm.y) - y.y);
+                red[own + v] = t;
+                A1[v] = make_float2(0.f, 0.f);
+                A2[v] = make_float2(0.f, 0.f);
+            }
         }
         if (cur.flush) {
-            if (active) {
-#pragma unroll
-                for (int v = 0; v < TD; ++v) {
-                    red[g * HT + h * TD + v] = make_float2(A1[v].x + A2[v].y, A2[v].x - A1[v].y);
-                    A1[v] = make_float2(0.f, 0.f);
-                    A2[v] = make_float2(0.f, 0.f);
-                }
-            }
             __syncthreads();
             const long long piece = (long long)blockIdx.x - stream_first_cta(cur.blk, p.blk_len, p.per_cta);
             float2* out = p.partial + (((size_t)prob * p.nblk + cur.blk) * p.maxpieces + piece) * (size_t)HT;
             for (int l = tid; l < HT; l += nthr) {
-                float2 sum = red[l];
+                float2 sum = make_float2(red[l].x - comp[l].x, red[l].y - comp[l].y);
                 for (int gg = 1; gg < p.G; ++gg) {
-                    const float2 t = red[gg * HT + l];
-                    sum.x += t.x;
-                    sum.y += t.y;
+                    const float2 t = red[gg * HT + l], c = comp[gg * HT + l];
+                    sum.x += t.x - c.x;
+                    sum.y += t.y - c.y;
                 }
                 out[l] = sum;
             }
-            __syncthreads();  // red is free again before a later flush writes it
+            __syncthreads();  // every thread has read the piece: the owners restart their sums
+            if (active) {
+#pragma unroll
+                for (int v = 0; v < TD; ++v) { red[own + v] = make_float2(0.f, 0.f); comp[own + v] = make_float2(0.f, 0.f); }
+            }
         }
         cur = nxt;
         b ^= 1;

@@ -426,7 +426,7 @@ int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo
     while (g->steps > 1 && (long long)g->G * g->steps * TI > g->per_cta + g->G * TI) --g->steps;
     for (;;) {
         const size_t Lmax = (size_t)g->G * g->steps * TI;
-        g->smem = (2 * (2 * Lmax + g->HT) + (size_t)g->G * g->HT) * sizeof(float2);
+        g->smem = (2 * (2 * Lmax + g->HT) + 2 * (size_t)g->G * g->HT) * sizeof(float2);   // staging, sums, compensations
         if (g->smem <= 100 * 1024 || g->steps == 1) break;
         --g->steps;
     }
@@ -1721,6 +1721,17 @@ int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, 
     return check_launch("track_meas_kernel");
 }
 
+// switches latched from the environment once per process (read_env): readable by name (prc_get_option), never settable
+const int* env_switch(const std::string& k) {
+    static const std::pair<const char*, const int*> kSwitches[] = {
+        {"tma", &g_tma}, {"tma_l2", &g_tma_l2}, {"tc", &g_tc}, {"tc_caf", &g_tc_caf}, {"tc_fir", &g_tc_fir},
+        {"stream", &g_stream}, {"packed", &g_packed}, {"tile", &g_tile}, {"nlms_block", &g_nlms_block},
+        {"tune_nchunk", &g_tune_nchunk}, {"tune_g", &g_tune_g}};
+    for (const auto& s : kSwitches)
+        if (k == s.first) return s.second;
+    return nullptr;
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2188,6 +2199,8 @@ int prc_set_option(const char* name, int value) {
     if (k == "fft") g_fft.store(value);
     else if (k == "fft_min_n") g_fft_min_n.store(value);
     else if (k == "caf_wave") g_caf_wave.store(value);
+    else if (env_switch(k) || k == "tma_active")
+        return fail(PRC_E_INVALID, "option '%s' is read-only (set from the environment when the library starts)", name);
     else return fail(PRC_E_INVALID, "unknown option '%s'", name);
     return PRC_OK;
 }
@@ -2199,6 +2212,8 @@ int prc_get_option(const char* name, int* value) {
     if (k == "fft") *value = g_fft.load();
     else if (k == "fft_min_n") *value = g_fft_min_n.load();
     else if (k == "caf_wave") *value = g_caf_wave.load();
+    else if (const int* s = env_switch(k)) *value = *s;
+    else if (k == "tma_active") *value = use_tma() ? 1 : 0;
     else return fail(PRC_E_INVALID, "unknown option '%s'", name);
     return PRC_OK;
 }

@@ -1,0 +1,676 @@
+"""Every kernel instantiation prcore.cu can launch, run against the suite's oracles and float64 truths.
+
+Three parts:
+
+* Variant matrix (GPU).  The environment switches of INTEGRATION.md section 6 are latched once per process, so every
+  variant runs in a child process (tests/_variant_child.py) that saves its outputs; this process computes each oracle
+  once and makes every comparison.  A variant's outputs are held to the float64 truth (1e-5) and to the
+  reference-pinned oracle or golden (1e-5 + 1.2 x reference-vs-truth), as in tests/test_gpu_parity.py.  They are also
+  compared with the default child: the loader-only switches (PRC_TMA, PRC_TMA_L2) change how the same bytes reach
+  shared memory and must be bit-identical; the other switches change the arithmetic and are held to 3e-6 on
+  independent channels (P0), the bound tests/test_gpu_fft.py uses between arithmetics.
+* In-process GPU cases for dispatches of the default configuration no other test reaches: NLMS with more than 1024
+  taps, the Doppler stage at F = 4096 .. 16384, the tap-weighted decimator at full size, and caf_wave = 1.
+* A CPU guard: every kernel launch site of prcore.cu must appear in COVERAGE with the GPU tests that reach it.
+
+Per-variant figures go to $PRC_PARITY_DIR/parity.json (tests/conftest.py:record_parity).
+"""
+import json
+import os
+import re
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+import scipy.signal as signal
+
+import _golden as G
+import _variant_child as VC
+from conftest import record_parity
+from passiveradar_b200 import _lib, synth
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+ROOT = os.path.dirname(HERE)
+CHILD = os.path.join(HERE, "_variant_child.py")
+PRCORE = os.path.join(ROOT, "passiveradar_b200", "csrc", "prcore.cu")
+TOL = 1e-5
+XVAR = 3e-6           # between two arithmetics on independent channels (test_random_shapes_fft_path_matches_direct_path_and_oracle)
+
+DIRECT = ["ls_big", "ls_small", "ls_wide", "toep", "caf_big", "caf_small", "frame"]
+# variant -> (environment, cases it runs).  The NLMS switch only changes NLMS; the others only the direct form.
+VARIANTS = {
+    "default": ({}, DIRECT + ["nlms"]),
+    "tma0": ({"PRC_TMA": "0"}, DIRECT),                     # cp.async loader warps of toepcorr_kernel (driver fallback)
+    "tma_l2_0": ({"PRC_TMA_L2": "0"}, DIRECT),              # L2 promotion hint of the tensor maps only
+    "tma_l2_3": ({"PRC_TMA_L2": "3"}, DIRECT),
+    "tc0": ({"PRC_TC": "0"}, DIRECT),                       # lagstream for LS and CAF, fir_apply<10, 10, 2>
+    "tc_caf0": ({"PRC_TC_CAF": "0"}, DIRECT),               # tensor-core LS, lagstream CAF at D % 1024 == 0
+    "tc_fir0": ({"PRC_TC_FIR": "0"}, DIRECT),               # fir_apply writes the tensor-core CAF's s planes
+    "tile1": ({"PRC_TC": "0", "PRC_TILE": "1"}, DIRECT),    # lagstream<6, 18>, fir_apply<6, 18, 2>
+    "tile2": ({"PRC_TC": "0", "PRC_TILE": "2"}, DIRECT),    # lagstream<14, 14>, fir_apply<14, 14, 2>
+    "stream0": ({"PRC_TC": "0", "PRC_STREAM": "0"}, DIRECT),                    # lagcorr<.., true>, fir_apply<10, 10, 1>
+    "scalar": ({"PRC_TC": "0", "PRC_STREAM": "0", "PRC_PACKED": "0"}, DIRECT),  # lagcorr<.., false>, fir_apply<10, 10, 0>
+    "serial_nlms": ({"PRC_NLMS_BLOCK": "0"}, ["nlms"]),     # nlms_kernel<1/2/4>
+    "tune": ({"PRC_TC": "0", "PRC_TUNE_NCHUNK": "1", "PRC_TUNE_G": "1"}, DIRECT),  # one chunk / group per problem
+}
+LOADER_ONLY = ("tma0", "tma_l2_0", "tma_l2_3")
+_ENV_NAMES = {var for var, _ in VC.SWITCHES.values()} | {"PRC_FFT", "PRC_FFT_MIN_N"}
+
+
+def _child_env(extra):
+    env = {k: v for k, v in os.environ.items() if k not in _ENV_NAMES}
+    env.update(extra)
+    env["PYTHONPATH"] = os.pathsep.join([HERE, ROOT] + ([os.environ["PYTHONPATH"]] if os.environ.get("PYTHONPATH") else []))
+    return env
+
+
+def _run_child(args, extra, timeout):
+    res = subprocess.run([sys.executable, CHILD] + args, env=_child_env(extra), capture_output=True, text=True,
+                         timeout=timeout)
+    assert res.returncode == 0, f"child {args} with {extra} failed:\n{res.stdout[-4000:]}\n{res.stderr[-4000:]}"
+    return res.stdout
+
+
+def _rel_columns(got, want_cols, lags, R, peak):
+    """max over the sampled lags d of |got[:, R - d] - want column| / peak."""
+    return max(float(np.abs(got[:, R - d, 0] - want_cols[d]).max()) / peak for d in lags)
+
+
+# ------------------------------------------------------------------ oracles and truths, computed once per session
+class Oracles:
+    """Lazily computed CPU oracles / float64 truths of the cases, cached for the whole module."""
+
+    def __init__(self):
+        self._cache = {}
+
+    def get(self, key, fn):
+        if key not in self._cache:
+            self._cache[key] = fn()
+        return self._cache[key]
+
+    def ls(self, case):
+        """item -> dict(truth=(out, taps), oracle=(out at idx or None, taps) or None, idx, den = max|srv|, profile).
+        The oracle is the item's golden (made by the reference) or, for small synthetic items, the live complex64 oracle."""
+        def make():
+            from oracle import clutter_oracle as co
+            d = {}
+            for item, profile, golden, ref, srv, fl, reg, peek in VC.ls_items(case):
+                t_out, t_taps = co.ls_filter_truth(ref, srv, fl, reg, peek)
+                den = float(np.abs(srv).max())
+                e = dict(truth=(t_out, t_taps), den=den, profile=profile, oracle=None)
+                if golden is not None:
+                    g = G.load(golden)
+                    idx = g["out_idx"] if "out_idx" in g else None
+                    e["oracle"] = (None if idx is None else g["out_sub"], g["taps"])
+                    e["idx"] = idx
+                elif fl + peek <= 64:          # the complex64 oracle forms the n x M data matrix: small problems only
+                    o_out, o_taps = co.ls_filter_oracle(ref, srv, fl, reg, peek, True)
+                    e["oracle"] = (o_out, o_taps)
+                    e["idx"] = np.arange(ref.shape[0])
+                d[item] = e
+            return d
+        return self.get(("ls", case), make)
+
+    def toep(self):
+        def make():
+            from oracle import clutter_oracle as co
+            d = {}
+            for item, profile, g, ref, srv in VC.toep_items():
+                t_out, t_taps = co.ls_filter_toeplitz_oracle(ref, srv, int(g["filter_len"]), int(g["peek"]), True)
+                d[item] = dict(truth=(t_out, t_taps), golden=g, den=float(g["srv_absmax"]))
+            return d
+        return self.get("toep", make)
+
+    def caf(self, case):
+        """item -> dict(lags, oracle columns, truth columns) for caf_big; whole maps for caf_small."""
+        def make():
+            from oracle import xambg_oracle as xo
+            d = {}
+            for item, profile, golden, ref, srv, R, F, input_len, window, short in VC.caf_items(case):
+                if case == "caf_big":
+                    n = ref.shape[0]
+                    lags = sorted({0, 1, R // 3, R // 2, R - 1, R})
+                    oc = {k: xo.fast_xambg_oracle(ref, np.roll(srv, -k), 0, F, n, window)[:, 0, 0] for k in lags}
+                    tc = {k: xo.fast_xambg_truth(ref, np.roll(srv, -k), 0, F, n, window)[:, 0, 0] for k in lags}
+                    d[item] = dict(lags=lags, oracle=oc, truth=tc, R=R, profile=profile)
+                else:
+                    truth = xo.fast_xambg_truth(ref, srv, R, F, input_len, window, short)
+                    oracle = golden["out"] if golden is not None else xo.fast_xambg_oracle(ref, srv, R, F, input_len, window, short)
+                    d[item] = dict(truth=truth, oracle=oracle, profile=profile)
+            return d
+        return self.get(("caf", case), make)
+
+    def frame(self):
+        def make():
+            from oracle import clutter_oracle as co
+            from oracle import xambg_oracle as xo
+            g, ref, srv, n, R, F = VC.frame_inputs()
+            t_clean, t_taps = co.ls_filter_truth(ref, srv, VC.FRAME["filter_len"], VC.FRAME["reg"], VC.FRAME["peek"])
+            t_map = xo.fast_xambg_truth(ref, t_clean, R, F, n, signal.get_window(VC.KAISER, n))
+            return dict(golden=g, t_clean=t_clean, t_taps=t_taps, t_map=t_map, den=float(np.abs(srv).max()))
+        return self.get("frame", make)
+
+    def nlms(self):
+        """key (as the child names it) -> (oracle out, oracle taps, truth out, truth taps) of the C oracle."""
+        def make():
+            from oracle import clutter_oracle as co
+            ref, srv = VC.nlms_inputs()
+            mu, peek = VC.NLMS["mu"], VC.NLMS["peek"]
+            d = {}
+            for fl in VC.NLMS_FILTER_LENS:
+                d[f"M{fl + peek}"] = co.block_nlms_oracle_c(ref, srv, fl, mu, peek, 1) + co.block_nlms_truth_c(ref, srv, fl, mu, peek, 1)
+            fl, B = VC.NLMS_BLOCK["filter_len"], VC.NLMS_BLOCK["block_len"]
+            d[f"M{fl + peek}_B{B}"] = co.block_nlms_oracle_c(ref, srv, fl, mu, peek, B) + co.block_nlms_truth_c(ref, srv, fl, mu, peek, B)
+            return d
+        return self.get("nlms", make)
+
+
+@pytest.fixture(scope="module")
+def oracles():
+    return Oracles()
+
+
+@pytest.fixture(scope="module")
+def variant_outputs(tmp_path_factory):
+    """variant -> its child's outputs; each child runs once per module, the first time a test asks for it."""
+    cache = {}
+
+    def get(name):
+        if name not in cache:
+            env, cases = VARIANTS[name]
+            path = tmp_path_factory.mktemp(f"variant_{name}") / "outputs.npz"
+            _run_child([str(path)] + cases, env, timeout=1200)
+            with np.load(path) as z:
+                cache[name] = {k: z[k] for k in z.files}
+        return cache[name]
+    return get
+
+
+# ------------------------------------------------------------------ per-case checks against truth and oracle
+def _check_ls(case, res, orc, fig):
+    for item, e in orc.ls(case).items():
+        p = f"{case}.{item}.{e['profile']}"
+        out, taps = res[p + ".out"], res[p + ".taps"]
+        t_out, t_taps = e["truth"]
+        fig[f"{item}/taps_vs_truth"] = et = G.rel_inf(taps, t_taps)
+        fig[f"{item}/out_vs_truth"] = eo = G.rel_inf(out, t_out, den=e["den"])
+        assert et <= TOL and eo <= TOL, (case, item, et, eo)
+        if e["oracle"] is not None:
+            o_out, o_taps = e["oracle"]
+            er = G.rel_inf(o_taps, t_taps)
+            fig[f"{item}/taps_vs_reference"] = ed = G.rel_inf(taps, o_taps)
+            assert ed <= TOL + 1.2 * er, (case, item, ed, er)
+            if o_out is not None:
+                idx = e["idx"]
+                er_o = G.rel_inf(o_out, t_out[idx], den=e["den"])
+                fig[f"{item}/out_vs_reference"] = ed = G.rel_inf(out[idx], o_out, den=e["den"])
+                assert ed <= TOL + 1.2 * er_o, (case, item, ed, er_o)
+
+
+def _check_toep(res, orc, fig):
+    for item, e in orc.toep().items():
+        g = e["golden"]
+        p = f"toep.{item}.{g['profile']}"
+        out, taps = res[p + ".out"], res[p + ".taps"]
+        t_out, t_taps = e["truth"]               # the complex128 Levinson solve of the reference's formulation
+        fig[f"{item}/taps_vs_truth"] = et = G.rel_inf(taps, t_taps)
+        fig[f"{item}/out_vs_truth"] = eo = G.rel_inf(out, t_out, den=e["den"])
+        assert et <= TOL and eo <= TOL, (item, et, eo)
+        er = G.rel_inf(g["taps"], t_taps)
+        er_o = G.rel_inf(g["out_sub"], t_out[g["out_idx"]], den=e["den"])
+        assert G.rel_inf(taps, g["taps"]) <= TOL + 1.2 * er, item
+        assert G.rel_inf(out[g["out_idx"]], g["out_sub"], den=e["den"]) <= TOL + 1.2 * er_o, item
+
+
+def _check_caf(case, res, orc, fig):
+    for item, e in orc.caf(case).items():
+        got = res[f"{case}.{item}.{e['profile']}.map"]
+        if case == "caf_big":
+            peak = float(np.abs(got).max())
+            et = _rel_columns(got, e["truth"], e["lags"], e["R"], peak)
+            eo = _rel_columns(got, e["oracle"], e["lags"], e["R"], peak)
+            er = max(float(np.abs(e["oracle"][d] - e["truth"][d]).max()) / peak for d in e["lags"])
+        else:
+            et, eo, er = G.rel_inf(got, e["truth"]), G.rel_inf(got, e["oracle"]), G.rel_inf(e["oracle"], e["truth"])
+        fig[f"{item}/map_vs_truth"], fig[f"{item}/map_vs_reference"] = et, eo
+        assert et <= TOL, (case, item, et)
+        assert eo <= TOL + 1.2 * er, (case, item, eo, er)
+
+
+def _check_frame(res, orc, fig):
+    e = orc.frame()
+    g = e["golden"]
+    p = f"frame.{VC.FRAME['name']}.{g['profile']}"
+    fig["map_vs_truth"] = em = G.rel_inf(res[p + ".map"], e["t_map"])
+    fig["taps_vs_truth"] = et = G.rel_inf(res[p + ".taps"], e["t_taps"])
+    fig["out_vs_truth"] = eo = G.rel_inf(res[p + ".out"], e["t_clean"], den=e["den"])
+    assert em <= TOL and et <= TOL and eo <= TOL, (em, et, eo)
+    er_map, er_taps = G.rel_inf(g["out"], e["t_map"]), G.rel_inf(g["taps"], e["t_taps"])
+    fig["map_vs_reference"] = ed = G.rel_inf(res[p + ".map"], g["out"])
+    assert ed <= TOL + 1.2 * er_map, (ed, er_map)
+    assert G.rel_inf(res[p + ".taps"], g["taps"]) <= TOL + 1.2 * er_taps
+
+
+def _nlms_bounds(out, taps, want, ww, truth, tw, what):
+    """NLMS output against the float64 recurrence (1e-5 of max|truth|) and the reference-pinned C oracle
+    (1e-5 + 1.2 x oracle-vs-truth); taps within 5e-5 of both, as tests/test_gpu_parity.py holds config 4."""
+    den = float(np.abs(truth).max())
+    et, eo, er = G.rel_inf(out, truth, den=den), G.rel_inf(out, want, den=den), G.rel_inf(want, truth, den=den)
+    assert et <= TOL, (what, et)
+    assert eo <= TOL + 1.2 * er, (what, eo, er)
+    assert G.rel_inf(taps, tw) <= 5e-5 and G.rel_inf(taps, ww) <= 5e-5, what
+    return dict(out_vs_truth=et, out_vs_reference=eo, reference_vs_truth=er)
+
+
+def _check_nlms(res, orc, fig):
+    prof = VC.NLMS["profile"]
+    for key, (want, ww, truth, tw) in orc.nlms().items():
+        out, taps = res[f"nlms.{key}.{prof}.out"], res[f"nlms.{key}.{prof}.taps"]
+        for k, v in _nlms_bounds(out, taps, want, ww, truth, tw, key).items():
+            fig[f"{key}/{k}"] = v
+        fl = int(key[1:].split("_")[0]) - VC.NLMS["peek"]
+        assert not out[:fl].any() and not out[-VC.NLMS["peek"]:].any(), key
+
+
+def _check(case, res, orc, fig):
+    if case in ("ls_big", "ls_small", "ls_wide"):
+        _check_ls(case, res, orc, fig)
+    elif case == "toep":
+        _check_toep(res, orc, fig)
+    elif case in ("caf_big", "caf_small"):
+        _check_caf(case, res, orc, fig)
+    elif case == "frame":
+        _check_frame(res, orc, fig)
+    else:
+        _check_nlms(res, orc, fig)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_variant_matches_truth_and_reference(variant, variant_outputs, oracles):
+    env, cases = VARIANTS[variant]
+    res = variant_outputs(variant)
+    assert list(res["cases"]) == cases
+    echo = dict(zip(VC.SWITCHES, res["switches"].tolist()))
+    assert echo == VC.expected_switches(env), echo
+    # the H100's driver has cuTensorMapEncodeTiled: only PRC_TMA=0 selects the cp.async loaders
+    assert int(res["tma_active"]) == (0 if env.get("PRC_TMA") == "0" else 1)
+    for case in cases:
+        fig = {}
+        _check(case, res, oracles, fig)
+        record_parity(f"variants/{variant}/{case}", **fig)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("variant", [v for v in VARIANTS if v != "default"])
+def test_variant_matches_default_child(variant, variant_outputs, oracles):
+    res, base = variant_outputs(variant), variant_outputs("default")
+    keys = [k for k in res if k.count(".") == 3]
+    assert keys and all(k in base for k in keys)
+    worst = 0.0
+    if variant in LOADER_ONLY:
+        # the loaders write the same shared-memory image; the MMA order is unchanged
+        for k in keys:
+            assert np.array_equal(res[k], base[k]), k
+    elif variant == "serial_nlms":
+        # Sample-serial against block-exact NLMS, with the bounds of test_nlms_large_batch_uses_the_half_size_ctas_and_matches.
+        # The serial kernel keeps the reference's rounding order (5e-7 from the C oracle here), the block-exact one lands
+        # nearer the float64 recurrence; so their distance carries the reference's own round-off, which at M = 1110 over
+        # 2**15 samples (2.9e-6 of max|truth|) exceeds the 2e-6 that test sees at M = 410 over 2**13 samples.
+        for key, (want, _, truth, _) in oracles.nlms().items():
+            k = f"nlms.{key}.{VC.NLMS['profile']}"
+            den = float(np.abs(want).max())
+            e = G.rel_inf(res[k + ".out"], base[k + ".out"], den=den)
+            e_ref = G.rel_inf(want, truth, den=den)
+            worst = max(worst, e)
+            assert G.rel_inf(res[k + ".out"], want, den=den) <= TOL, key
+            assert e <= 2e-6 + 1.2 * e_ref, (key, e, e_ref)
+            assert G.rel_inf(res[k + ".taps"], base[k + ".taps"]) <= 5e-5, key
+    else:
+        for k in keys:
+            if k.split(".")[2] != "P0":
+                continue                 # strong clutter: what is left after ~55 dB of cancellation, held to the truth only
+            e = G.rel_inf(res[k], base[k])
+            worst = max(worst, e)
+            assert e <= XVAR, (k, e)
+    record_parity(f"variants/{variant}/vs_default", E=worst)
+
+
+# ------------------------------------------------------------------ switch echo (no GPU needed)
+def test_switch_echo_reports_the_environment():
+    got = json.loads(_run_child(["--switches"], {"PRC_TILE": "2", "PRC_TC": "0", "PRC_TMA": "0"}, timeout=300))
+    assert (got["tile"], got["tc"], got["tma"]) == (2, 0, 0)
+    assert got == VC.expected_switches({"PRC_TILE": "2", "PRC_TC": "0", "PRC_TMA": "0"})
+    defaults = json.loads(_run_child(["--switches"], {}, timeout=300))
+    assert defaults == {"tma": 1, "tma_l2": 2, "tc": 1, "tc_caf": 1, "tc_fir": 1, "stream": 1, "packed": 1, "tile": 0,
+                        "nlms_block": 1, "tune_nchunk": -1, "tune_g": -1}
+
+
+@pytest.mark.parametrize("name", list(VC.SWITCHES) + ["tma_active"])
+def test_environment_switches_are_read_only(name):
+    lib = _lib.load()
+    assert lib.prc_set_option(name.encode(), 1) == _lib.PRC_E_INVALID
+    assert b"read-only" in lib.prc_last_error()
+    if name != "tma_active":             # resolving the TMA encoder needs a driver
+        assert _lib.get_option(name) == VC.expected_switches(os.environ)[name]
+
+
+# ------------------------------------------------------------------ default-configuration dispatches (in process)
+@pytest.mark.gpu
+@pytest.mark.parametrize("fl", [1100, 3000])
+def test_nlms_with_more_than_1024_taps_matches_c_oracle(fl, oracles):
+    """M = 1110 and 3010: nlms_block_kernel<2> and <4> (two and four taps per thread)."""
+    import passiveradar_b200 as prb
+    ref, srv = VC.nlms_inputs()
+    mu, peek = VC.NLMS["mu"], VC.NLMS["peek"]
+    got, gw = prb.NLMS_filter(ref, srv, fl, mu, peek, None, True)
+    fig = _nlms_bounds(got, gw, *oracles.nlms()[f"M{fl + peek}"], fl)
+    record_parity(f"nlms/n32768_M{fl + peek}", **fig)
+    assert not got[:fl].any() and not got[-peek:].any()
+
+
+@pytest.mark.gpu
+def test_nlms_accepts_4096_taps_and_names_the_limit_above():
+    import passiveradar_b200 as prb
+    from oracle import clutter_oracle as co
+    ref, srv = synth.make_frame(6000, "P1", frame=12)
+    got, gw = prb.NLMS_filter(ref, srv, 4086, 0.05, 10, None, True)
+    want = co.block_nlms_oracle_c(ref, srv, 4086, 0.05, 10, 1) + co.block_nlms_truth_c(ref, srv, 4086, 0.05, 10, 1)
+    record_parity("nlms/n6000_M4096", **_nlms_bounds(got, gw, *want, 4086))
+    with pytest.raises(_lib.PrcoreError, match="4096"):
+        prb.NLMS_filter(ref, srv, 4087, 0.05, 10)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("M", [1000, 2000])
+def test_nlms_frames_past_the_sm_count_with_many_taps(M):
+    """More frames than SMs at M = 1000 and 2000: nlms_block_kernel<2, 512> and <4, 512> against single-frame calls and
+    the C oracle (bounds of test_nlms_large_batch_uses_the_half_size_ctas_and_matches)."""
+    import torch
+    import passiveradar_b200 as prb
+    from oracle import clutter_oracle as co
+    nf = torch.cuda.get_device_properties(0).multi_processor_count + 12
+    n, peek, mu = 2 ** 13, 10, 0.05
+    fl = M - peek
+    base = [synth.make_frame(n, "P1", frame=180 + i) for i in range(4)]
+    dev = torch.device("cuda", 0)
+    ref_d = torch.from_numpy(np.stack([base[i % 4][0] for i in range(nf)])).to(dev)
+    srv_d = torch.from_numpy(np.stack([base[i % 4][1] for i in range(nf)])).to(dev)
+    out = torch.empty((nf, n), dtype=torch.complex64, device=dev)
+    taps = torch.empty((nf, M), dtype=torch.complex64, device=dev)
+    lib = _lib.load()
+    st = torch.cuda.Stream(device=dev)
+    _lib.check(lib.prc_nlms_frames_c64(ref_d.data_ptr(), srv_d.data_ptr(), n, nf, n, fl, peek, mu, 1, None, out.data_ptr(),
+                                       taps.data_ptr(), _lib.MEM_DEVICE, 0, st.cuda_stream, 0))
+    got, gt = out.cpu().numpy(), taps.cpu().numpy()
+    for i in (0, 1, 2, 3, nf - 1):
+        ref, srv = base[i % 4]
+        want, _ = co.block_nlms_oracle_c(ref, srv, fl, mu, peek, 1)
+        single, st1 = prb.NLMS_filter(ref, srv, fl, mu, peek, None, True)
+        den = float(np.abs(want).max())
+        assert G.rel_inf(got[i], want, den=den) <= TOL, i
+        assert G.rel_inf(got[i], single, den=den) <= 2e-6, i
+        assert G.rel_inf(gt[i], st1) <= 5e-5, i
+    assert np.array_equal(got[0], got[4])
+
+
+_DOPPLER_SHAPES = [(2 ** 20, 4096), (2 ** 20, 8192), (2 ** 20, 16384), (2 ** 22, 8192), (2 ** 22, 16384)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n,F", _DOPPLER_SHAPES)
+def test_doppler_stage_at_large_F(n, F, both_paths, oracles):
+    """F = 4096: doppler_fft_pow2_kernel<2>; 8192: <1>; 16384: chunk sums + direct DFT.  Sampled range columns against
+    the oracle (columns are independent: lag d of srv is lag 0 of srv rolled by -d)."""
+    import passiveradar_b200 as prb
+    from oracle import xambg_oracle as xo
+    R = 40
+    ref, srv = synth.make_frame(n, "P1", frame=25)
+    w = signal.get_window(VC.KAISER, n)
+    lags = [0, 1, R // 2, R - 1, R]
+    cols = oracles.get(("doppler", n, F), lambda: {d: xo.fast_xambg_oracle(ref, np.roll(srv, -d), 0, F, n, w)[:, 0, 0] for d in lags})
+    got = prb.fast_xambg(ref, srv, R, F, n, w)
+    e = _rel_columns(got, cols, lags, R, float(np.abs(got).max()))
+    record_parity(f"xambg/doppler_n{n}_F{F}/{both_paths}", E_vs_oracle_sampled_columns=e)
+    assert e <= TOL, e
+
+
+@pytest.mark.gpu
+def test_tap_weighted_decimator_at_full_size(both_paths, oracles):
+    """fast_xambg(..., shortFilt=False) at config 2: 40 961 flat-top taps per Doppler block, lagcorr_kernel with taps
+    on either path (the FFT-domain CAF takes the boxcar decimator only)."""
+    import passiveradar_b200 as prb
+    from oracle import xambg_oracle as xo
+    n, F, R = 2 ** 20, 256, 300
+    ref, srv = synth.make_frame(n, "P1", frame=26)
+    lags = sorted({0, 1, R // 3, R // 2, R - 1, R})
+
+    def make():
+        oc = {d: xo.fast_xambg_oracle(ref, np.roll(srv, -d), 0, F, n, None, False)[:, 0, 0] for d in lags}
+        tc = {d: xo.fast_xambg_truth(ref, np.roll(srv, -d), 0, F, n, None, False)[:, 0, 0] for d in lags}
+        return oc, tc
+    oc, tc = oracles.get("longfilt_c2", make)
+    got = prb.fast_xambg(ref, srv, R, F, shortFilt=False)
+    peak = float(np.abs(got).max())
+    eo, et = _rel_columns(got, oc, lags, R, peak), _rel_columns(got, tc, lags, R, peak)
+    record_parity(f"xambg/longfilt_n{n}/{both_paths}", E_vs_oracle_sampled_columns=eo, E_vs_truth_sampled_columns=et)
+    assert eo <= TOL, eo
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("n,F,R", [(2 ** 20, 256, 300), (2 ** 18, 1024, 100)])
+def test_caf_wave_grid_is_bit_identical(n, F, R):
+    """caf_wave = 1 walks the Doppler blocks of the FFT-domain CAF with one wave of CTAs; every block is computed the
+    same way, so single frames, 5-frame CAF batches and 5-frame fused batches are bit-identical to caf_wave = 0.  At
+    (2**20, 256, 300) the 5-frame batch also takes doppler_fft_pow2_kernel<8>, checked against the oracle."""
+    import passiveradar_b200 as prb
+    from oracle import xambg_oracle as xo
+    nf = 5
+    frames = [synth.make_frame(n, "P0", frame=190 + i) for i in range(nf)]
+    ref = np.ascontiguousarray(np.stack([f[0] for f in frames]))
+    srv = np.ascontiguousarray(np.stack([f[1] for f in frames]))
+    w = np.ascontiguousarray(signal.get_window(VC.KAISER, n), dtype=np.float64)
+    lib = _lib.load()
+    old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"), _lib.get_option("caf_wave"))
+    res = {}
+    try:
+        _lib.set_option("fft", 1)
+        _lib.set_option("fft_min_n", 8192)
+        for wave in (0, 1):
+            _lib.set_option("caf_wave", wave)
+            single = prb.fast_xambg(ref[0], srv[0], R, F, n, w)
+            xb = np.empty((nf, F, R + 1), np.complex64)
+            _lib.check(lib.prc_xambg_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nf, n, R, F, w.ctypes.data, xb.ctypes.data,
+                                                _lib.MEM_HOST, 0, None, 0))
+            fb = np.empty((nf, F, R + 1), np.complex64)
+            _lib.check(lib.prc_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nf, n, R, 10, 1.0, R, F, w.ctypes.data,
+                                          fb.ctypes.data, None, None, _lib.MEM_HOST, 0, None, 0))
+            res[wave] = (single, xb, fb)
+    finally:
+        _lib.set_option("fft", old[0])
+        _lib.set_option("fft_min_n", old[1])
+        _lib.set_option("caf_wave", old[2])
+    for a, b, what in zip(res[0], res[1], ("fast_xambg", "prc_xambg_frames_c64", "prc_frames_c64")):
+        assert np.array_equal(a, b), what
+    xb = res[1][1]
+    lags = sorted({0, 1, R // 2, R - 1, R})
+    worst = 0.0
+    for i in (0, nf - 1):
+        cols = {d: xo.fast_xambg_oracle(ref[i], np.roll(srv[i], -d), 0, F, n, w)[:, 0, 0] for d in lags}
+        worst = max(worst, _rel_columns(xb[i][:, :, None], cols, lags, R, float(np.abs(xb[i]).max())))
+    record_parity(f"xambg/caf_wave_n{n}_F{F}_R{R}", E_vs_oracle_sampled_columns=worst)
+    assert worst <= TOL, worst
+
+
+# ------------------------------------------------------------------ CPU guard: every launch site is covered
+# (host function, kernel<template arguments>) of every launch in prcore.cu -> [(test id, variant, what it reaches)].
+# Variant: "default" (shipped configuration), "fft" / "direct" (the both_paths fixture), or a VARIANTS child.
+# A row is checked against the source, not the other way round: read the dispatch code before adding one.
+PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/test_kernel_variants.py::"
+FE, GAL, TRK = "tests/test_gpu_frontend.py::", "tests/test_gal_jpe.py::", "tests/test_tracking.py::"
+VARIANT_TEST = KV + "test_variant_matches_truth_and_reference"
+COVERAGE = {
+    "launch_lagstream: lagstream_kernel<10, 10>": [(PAR + "test_ls_matches_live_oracle", "direct", "LS, n <= 20000"),
+                                                   (VARIANT_TEST, "tc0", "LS and CAF at config 2")],
+    "launch_lagstream: lagstream_kernel<6, 18>": [(VARIANT_TEST, "tile1", "LS, Toeplitz LS, CAF")],
+    "launch_lagstream: lagstream_kernel<14, 14>": [(VARIANT_TEST, "tile2", "LS, Toeplitz LS, CAF")],
+    "fft_twiddles: fft::fft_twiddle_kernel<R3>": [
+        (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 (n = 200000) and 8 (n = 10**6)"),
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
+    "ls_fft_corr: fftc::lscorr_fft_kernel<R3>": [
+        (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8 (M <= 1024)"),
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; ls_fft_plan never picks R3 = 4")],
+    "levinson_launch: levinson_kernel<1>": [(PAR + "test_ls_matches_live_oracle", "fft", "M <= 1024, batched solve")],
+    "levinson_launch: levinson_kernel<4>": [(PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "M = 1110")],
+    "taps_spectrum: fftc::taps_spectrum_kernel<R3>": [
+        (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8 (CAF transform)"),
+        (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8 (FIR transform)"),
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
+    "fir_fft: fftc::fir_fft_kernel<R3>": [
+        (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8"),
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; the LS transform is never R3 = 4")],
+    "caf_fft: fftc::caf_fft_kernel<R3, true>": [
+        (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8"),
+        (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16"),
+        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
+    "caf_fft: fftc::caf_fft_kernel<R3, false>": [
+        (PAR + "test_xambg_matches_live_oracle", "fft", "R3 = 4"),
+        (FFT + "test_xambg_large_shapes_sampled_columns", "fft", "R3 = 8 (F = 64, D >= 16384)"),
+        (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16 (R = 1200)"),
+        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
+    "xambg_device: weight_kernel": [(VARIANT_TEST, "default", "tensor-core CAF, caf_big"),
+                                    (PAR + "test_xambg_matches_live_oracle", "direct", "lagstream CAF with a window")],
+    "xambg_device: tc::tc_prep_kernel": [(VARIANT_TEST, "default", "caf_big"),
+                                         (FFT + "test_xambg_large_shapes_sampled_columns", "direct", "D = 1024 .. 65536")],
+    "xambg_device: tc::toepcorr_kernel<false, true>": [(VARIANT_TEST, "default", "caf_big, frame"),
+                                                       (FFT + "test_xambg_large_shapes_sampled_columns", "direct", "")],
+    "xambg_device: tc::toepcorr_kernel<false, false>": [(VARIANT_TEST, "tma0", "caf_big, frame: cp.async loaders")],
+    "xambg_device: lagcorr_kernel<LC_TI, LC_TD, true>": [
+        (VARIANT_TEST, "default", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
+        (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps")],
+    "xambg_device: lagcorr_kernel<LC_TI, LC_TD, false>": [(VARIANT_TEST, "scalar", "caf_small, caf_big, frame")],
+    "xambg_device: twiddle_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "every fast_xambg")],
+    "xambg_device: doppler_fft_pow2_kernel<8>": [
+        (KV + "test_caf_wave_grid_is_bit_identical", "default", "5 frames x 38 column groups >= SM count"),
+        (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "direct", "R = 1200, F = 64")],
+    "xambg_device: doppler_fft_pow2_kernel<2>": [(PAR + "test_xambg_matches_live_oracle", "direct", "F <= 4096"),
+                                                 (KV + "test_doppler_stage_at_large_F", "fft", "F = 4096")],
+    "xambg_device: doppler_fft_pow2_kernel<1>": [(KV + "test_doppler_stage_at_large_F", "fft", "F = 8192")],
+    "xambg_device: chunk_sum_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
+                                       (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
+    "xambg_device: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
+                                         (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
+    "ls_device: tc::bf16_split_kernel": [(FFT + "test_ls_config4_size_and_readme_shape", "direct", "n = 10**6, not a multiple of 1024")],
+    "ls_device: tc::tc_prep_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
+    "ls_device: tc::toepcorr_kernel<true, true>": [(VARIANT_TEST, "default", "ls_big, frame"),
+                                                   (PAR + "test_ls_matches_reference_golden", "direct", "ls_c2_p1")],
+    "ls_device: tc::toepcorr_kernel<true, false>": [(VARIANT_TEST, "tma0", "ls_big, frame: cp.async loaders")],
+    "ls_device: lagcorr_kernel<LC_TI, LC_TD, true>": [(VARIANT_TEST, "stream0", "ls_big, ls_small, ls_wide")],
+    "ls_device: lagcorr_kernel<LC_TI, LC_TD, false>": [(VARIANT_TEST, "scalar", "ls_big, ls_small, ls_wide")],
+    "ls_device: levinson_kernel<1>": [(VARIANT_TEST, "default", "ls_big, ls_small"),
+                                      (PAR + "test_ls_matches_live_oracle", "direct", "")],
+    "ls_device: levinson_kernel<4>": [(VARIANT_TEST, "default", "ls_wide"),
+                                      (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", "")],
+    "ls_device: tc::fir_bmat_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
+    "ls_device: tc::firtc_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
+    "ls_device: fir_apply_kernel<FIR_TK, FIR_TO, 0>": [(VARIANT_TEST, "scalar", "")],
+    "ls_device: fir_apply_kernel<FIR_TK, FIR_TO, 1>": [(VARIANT_TEST, "stream0", "")],
+    "ls_device: fir_apply_kernel<10, 10, 2>": [(VARIANT_TEST, "default", "ls_small, ls_wide, toep"),
+                                               (VARIANT_TEST, "tc_fir0", "frame: writes the tensor-core CAF's s planes")],
+    "ls_device: fir_apply_kernel<6, 18, 2>": [(VARIANT_TEST, "tile1", "")],
+    "ls_device: fir_apply_kernel<14, 14, 2>": [(VARIANT_TEST, "tile2", "")],
+    "ls_toeplitz_device: shift_roll_kernel": [(VARIANT_TEST, "default", "toep"),
+                                              (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins")],
+    "mix_device: iq_mix_kernel": [(FE + "test_frequency_shift_follows_numpy_promotion", "default", "")],
+    "resample_device: resample_ends_kernel": [(FE + "test_resample_matches_reference_golden", "default", "")],
+    "resample_device: resample_kernel": [(FE + "test_resample_matches_reference_golden", "default", "")],
+    "cfar_device: cfar_abssum_kernel": [(FE + "test_cfar_matches_reference_golden", "default", "")],
+    "cfar_device: cfar2d_kernel": [(FE + "test_cfar_matches_reference_golden", "default", "")],
+    "direct_xambg_device: piece_sum_kernel": [(FE + "test_direct_xambg_matches_reference_golden", "default", "")],
+    "nlms_device: nlms_block_kernel<1, 512>": [(FFT + "test_nlms_large_batch_uses_the_half_size_ctas_and_matches", "default", "M = 410")],
+    "nlms_device: nlms_block_kernel<2, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 1000")],
+    "nlms_device: nlms_block_kernel<4, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 2000")],
+    "nlms_device: nlms_block_kernel<1>": [(PAR + "test_nlms_matches_reference_golden", "default", ""),
+                                          (VARIANT_TEST, "default", "nlms M = 410")],
+    "nlms_device: nlms_block_kernel<2>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 1110")],
+    "nlms_device: nlms_block_kernel<4>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 3010"),
+                                          (KV + "test_nlms_accepts_4096_taps_and_names_the_limit_above", "default", "M = 4096")],
+    "nlms_device: nlms_kernel<1>": [(VARIANT_TEST, "serial_nlms", "M = 410")],
+    "nlms_device: nlms_kernel<2>": [(VARIANT_TEST, "serial_nlms", "M = 1110")],
+    "nlms_device: nlms_kernel<4>": [(VARIANT_TEST, "serial_nlms", "M = 3010")],
+    "gal_device: gal_jpe_kernel<1, false>": [(GAL + "test_gal_edge_cases", "default", "D = 1")],
+    "gal_device: gal_jpe_kernel<2, false>": [(GAL + "test_gal_edge_cases", "default", "D = 40")],
+    "gal_device: gal_jpe_kernel<4, false>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 77")],
+    "gal_device: gal_jpe_kernel<8, false>": [(GAL + "test_gal_long_run_matches_c_oracle_and_truth", "default", "D = 185")],
+    "gal_device: gal_jpe_kernel<GAL_CTA_T, true>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 300, 4096")],
+    "stage_window: f64_to_f32_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "float64 window")],
+    "prc_xambg_c64: f64_to_f32_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_longfilt taps")],
+    "trk_meas_launch: track_meas_kernel<T, TRK_MODE_MEAN>": [
+        (TRK + "test_float32_equals_float64_and_frame_layouts_agree", "default", "T = float, double (simple tracker)")],
+    "trk_meas_launch: track_meas_kernel<T, TRK_MODE_SLOTS>": [
+        (TRK + "test_float32_equals_float64_and_frame_layouts_agree", "default", "T = float, double (multi-target tracker)")],
+    "trk_meas_launch: track_meas_kernel<T, TRK_MODE_MEAS>": [
+        (TRK + "test_float32_equals_float64_and_frame_layouts_agree", "default", "T = float, double (get_measurements)")],
+    "prc_multitarget_track_frames: track_multi_kernel": [(TRK + "test_multitarget_tracker_matches_golden", "default", "")],
+    "prc_simple_track_frames: track_simple_kernel<double>": [(TRK + "test_simple_target_tracker_matches_golden", "default", "")],
+    "prc_simple_track_frames: track_simple_kernel<float>": [(TRK + "test_float32_equals_float64_and_frame_layouts_agree", "default", "")],
+}
+
+_FUNC_DEF = re.compile(r"^(?!(?:return|typedef|using|namespace|struct|enum|extern|template|#))[A-Za-z_][\w:<>*&\s]*?\b([A-Za-z_]\w*)\s*\(")
+_LAUNCH = re.compile(r"([A-Za-z_][\w:]*)\s*(<[^<>;()]*>)?\s*<<<")
+
+
+def launch_sites(path=PRCORE):
+    """{'host function: kernel<template arguments>': [line numbers]} of every kernel launch in the file, including
+    the ones inside macros (PRC_R3_SWITCH, PRC_TRK_MEAS)."""
+    sites = {}
+    func = None
+    with open(path) as f:
+        for no, line in enumerate(f, 1):
+            m = _FUNC_DEF.match(line)
+            if m:
+                func = m.group(1)
+            code = line.split("//", 1)[0]
+            for k in _LAUNCH.finditer(code):
+                targs = ""
+                if k.group(2):
+                    targs = "<" + ", ".join(a.strip() for a in k.group(2)[1:-1].split(",")) + ">"
+                sites.setdefault(f"{func}: {k.group(1)}{targs}", []).append(no)
+    return sites
+
+
+def _is_gpu_test(test_id):
+    path, name = test_id.split("::")
+    with open(os.path.join(ROOT, path)) as f:
+        src = f.read()
+    m = re.search(rf"^def {re.escape(name)}\(", src, re.M)
+    assert m, f"{test_id} does not exist"
+    decorators = src[:m.start()].rstrip("\n").rsplit("\n\n", 1)[-1]       # the block right above the def
+    return re.search(r"^pytestmark = pytest\.mark\.gpu$", src, re.M) is not None or "@pytest.mark.gpu" in decorators
+
+
+def test_every_launch_site_has_a_covering_gpu_test():
+    sites = launch_sites()
+    assert len(sites) >= 60
+    missing = sorted(set(sites) - set(COVERAGE))
+    stale = sorted(set(COVERAGE) - set(sites))
+    assert not missing, "launch sites of prcore.cu without a covering test in COVERAGE: " + \
+        "; ".join(f"{s} (line {sites[s][0]})" for s in missing)
+    assert not stale, f"COVERAGE rows that are no launch site of prcore.cu: {stale}"
+    for site, reached in COVERAGE.items():
+        assert reached, f"{site}: no test"
+        for test_id, variant, _ in reached:
+            assert _is_gpu_test(test_id), f"{site}: {test_id} is not a GPU test"
+            assert variant in ("default", "fft", "direct") or variant in VARIANTS, f"{site}: unknown variant {variant}"
+            if test_id == VARIANT_TEST:
+                assert variant in VARIANTS
+
+
+def test_coverage_guard_sees_a_new_launch(tmp_path):
+    """The guard fails for a launch it has not been told about."""
+    src = open(PRCORE).read()
+    scratch = tmp_path / "prcore.cu"
+    scratch.write_text(src + "\nint new_entry(Ctx* c) {\n    new_kernel<3><<<1, 32, 0, c->stream>>>();\n    return 0;\n}\n")
+    extra = set(launch_sites(str(scratch))) - set(COVERAGE)
+    assert extra == {"new_entry: new_kernel<3>"}
