@@ -218,6 +218,9 @@ int prc_gal_jpe_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, in
  *   "tune_nchunk" (PRC_TUNE_NCHUNK, -1 = automatic), "tune_g" (PRC_TUNE_G, -1 = automatic);
  *   "tma_active"  1 when toepcorr_kernel uses TMA producers: "tma" is 1 and the driver has cuTensorMapEncodeTiled
  *                 (0: the cp.async loader warps)
+ *   "fft_ctas_ls", "fft_ctas_fir", "fft_ctas_caf"  CTAs per SM of lscorr_fft_kernel, fir_fft_kernel and the fused
+ *                 caf_fft_kernel at L = 2048 on the calling thread's current device, as the runtime's occupancy
+ *                 calculator gives it for the launch configuration: the number their one-wave grids are sized from
  */
 int prc_set_option(const char* name, int value);
 int prc_get_option(const char* name, int* value);

@@ -117,10 +117,19 @@ struct LsCorrParams {
 // shared memory: [fft::Smem (2 exchange buffers, twiddles) | staging L float2]
 template <int R3> constexpr int lscorr_smem_float2() { return fft::Geo<R3>::SMEM_FLOAT2 + fft::Geo<R3>::L; }
 
+// CTAs per SM the register allocation of lscorr_fft_kernel is held to.  R3 = 8: 68.6 KB of shared memory fits three
+// times in an SM, and an allocation of 175 registers x 128 threads would let only two in -- at <= 168 registers,
+// without spills, three fit.  R3 = 16 is held to one CTA per SM by its shared memory; 0 leaves the
+// allocation of the other instantiations to ptxas as before.
+template <int R3> constexpr int lscorr_min_ctas() { return R3 == 8 ? 3 : 0; }
+
 // CTA c of a frame takes segments c, c + gridDim.x, ...; items per segment: 0 = zero-padded reference segment (X),
 // 1 = L reference samples from the segment start (Yr), 2 = L surveillance samples from start - peek (Ys).
+// X is the first len samples of Yr, and a thread stages the same elements for both: the L reference samples are
+// staged once, for item 0, which zeroes the elements from len on in its registers, and item 1 reads the same slots
+// again (a third fewer copies from L2 and shared-memory stores; the transforms see the same inputs).
 template <int R3>
-__global__ void __launch_bounds__(16 * R3) lscorr_fft_kernel(const __grid_constant__ LsCorrParams p) {
+__global__ void __launch_bounds__(16 * R3, lscorr_min_ctas<R3>()) lscorr_fft_kernel(const __grid_constant__ LsCorrParams p) {
     using G = fft::Geo<R3>;
     extern __shared__ __align__(16) float2 sm[];
     const int t = threadIdx.x;
@@ -133,10 +142,10 @@ __global__ void __launch_bounds__(16 * R3) lscorr_fft_kernel(const __grid_consta
 
     auto issue = [&](int it) {
         const int q = it / 3, kind = it - 3 * q;
+        if (kind == 1) return;                      // Yr: still in the slots item 0 read
         const int sgm = blockIdx.x + q * gridDim.x;
         const long long i0 = (long long)sgm * p.Bs;
-        if (kind == 0) stage_sig<G::T, false>(stg, t, ref, i0, min(p.Bs, p.n - sgm * p.Bs), p.n, p.linear);
-        else if (kind == 1) stage_sig<G::T, true>(stg, t, ref, i0, G::L, p.n, p.linear);
+        if (kind == 0) stage_sig<G::T, true>(stg, t, ref, i0, G::L, p.n, p.linear);
         else stage_sig<G::T, true>(stg, t, srv, i0 - p.peek, G::L, p.n, p.linear);
         cp_async_commit();
     };
@@ -151,8 +160,13 @@ __global__ void __launch_bounds__(16 * R3) lscorr_fft_kernel(const __grid_consta
 #pragma unroll 1
     for (int it = 0; it < nitems; ++it) {
         const int kind = it % 3;
-        if (kind == 0) fetch_staged<G::T, false>(v, stg, t, min(p.Bs, p.n - ((int)blockIdx.x + (it / 3) * (int)gridDim.x) * p.Bs));
-        else fetch_staged<G::T, true>(v, stg, t, G::L);
+        fetch_staged<G::T, true>(v, stg, t, G::L);
+        if (kind == 0) {                            // X: the segment's len samples, zero padded
+            const int len = min(p.Bs, p.n - ((int)blockIdx.x + (it / 3) * (int)gridDim.x) * p.Bs);
+#pragma unroll
+            for (int n1 = 0; n1 < 16; ++n1)
+                if (n1 * G::T + t >= len) v[n1] = make_float2(0.f, 0.f);
+        }
         fft::fft_n2p<R3>(v, t, S, [&] { if (it + 1 < nitems) issue(it + 1); });
         if (kind == 0) {
 #pragma unroll
@@ -292,6 +306,11 @@ template <int R3> constexpr int caf_smem_float2() { return fft::Geo<R3>::SMEM_FL
 
 // Items of a Doppler block: per segment the surveillance samples (kind 0), with FUSED the reference samples the
 // clutter filter needs (kind 1), and the windowed reference (kind 2); one transform call site for all of them.
+// With FUSED, kind 1 stages ref[i0 - off ..] with off = M - 1 - peek, and the ln <= Bmax reference samples of kind 2
+// lie inside that window (off + Bmax <= L): kind 2 reads them from the slots kind 1 staged, shifted by off, and
+// stages only the window.  The slots are written by other threads, so this relies on the barriers of kind 1's
+// transform (every thread waited for its own copies before it); the next segment's copies are issued after the
+// first barrier of kind 2's transform, when every thread has read them.
 template <int R3, bool FUSED>
 __global__ void __launch_bounds__(16 * R3) caf_fft_kernel(const __grid_constant__ CafFftParams p) {
     using G = fft::Geo<R3>;
@@ -305,6 +324,8 @@ __global__ void __launch_bounds__(16 * R3) caf_fft_kernel(const __grid_constant_
     const float2* srv = p.srv + (size_t)blockIdx.y * p.frame_stride;
     const float2* wp = FUSED ? p.wp + (size_t)blockIdx.y * G::L : nullptr;
     const float inv = 1.0f / (float)G::L;
+    const int off = p.M - 1 - p.peek;
+    const bool reuse = FUSED && off >= 0 && off + p.Bmax <= G::L;      // kind 2 reads kind 1's slots
     bool tw_staged = false;
 #pragma unroll 1
     for (int j = blockIdx.x; j < p.F; j += gridDim.x) {
@@ -326,7 +347,7 @@ __global__ void __launch_bounds__(16 * R3) caf_fft_kernel(const __grid_constant_
             } else if (kind == 1) {
                 stage_sig<G::T, true>(stg, t, ref, i0 + p.peek - (p.M - 1), G::L, p.n, 0);
             } else {
-                stage_sig<G::T, false>(stg, t, ref, i0, ln, p.n, 0);
+                if (!reuse) stage_sig<G::T, false>(stg, t, ref, i0, ln, p.n, 0);
                 if (p.win) {
                     const float* w0 = p.win + i0 + t;
 #pragma unroll
@@ -350,7 +371,16 @@ __global__ void __launch_bounds__(16 * R3) caf_fft_kernel(const __grid_constant_
             const int q = it / NK, kind = FUSED ? it - q * NK : 2 * (it - q * NK);
             if (kind == 2) {
                 const int ln = (int)min((long long)Bs, hi - (lo + (long long)q * Bs));
-                fetch_staged<G::T, false>(v, stg, t, ln);
+                if (reuse) {
+                    cp_async_wait_all();                            // the window
+#pragma unroll
+                    for (int n1 = 0; n1 < 16; ++n1) {
+                        const int i = n1 * G::T + t;
+                        v[n1] = i < ln ? stg[i + off] : make_float2(0.f, 0.f);
+                    }
+                } else {
+                    fetch_staged<G::T, false>(v, stg, t, ln);
+                }
                 if (p.win) {
 #pragma unroll
                     for (int n1 = 0; n1 < 16; ++n1) {

@@ -145,6 +145,7 @@ struct Ctx {
     bool pin_ready = false;
     DBuf fft_tw[3], wp_fir, wp_caf, fftP;     // FFT-domain path: twiddle tables (L = 1024 / 2048 / 4096), taps spectra, CAF block sums
     bool fft_tw_ready[3] = {false, false, false};
+    int fft_ctas[4][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
     std::vector<ProfRec> recs;
     void release() {
         cudaSetDevice(device);
@@ -570,13 +571,46 @@ int fft_twiddles(Ctx* c, int r3, const float2** tw) {
     return PRC_OK;
 }
 
+// FFT-domain kernels whose grids are sized to one wave of CTAs for the whole batch
+enum FftKern { FK_LS = 0, FK_FIR = 1, FK_CAF = 2, FK_CAF_FUSED = 3 };
+
+// CTAs of one instantiation an SM holds at once, at the block size and dynamic shared memory it is launched with:
+// registers (and the launch bounds that cap them) and shared memory decide it, so the grids follow the build rather
+// than a number written next to them.  Asked once per context.  1 if the runtime cannot answer (the grid stays
+// correct, only smaller; the launch itself then reports what is wrong).
+int fft_ctas_per_sm(Ctx* c, FftKern k, int r3) {
+    int& cached = c->fft_ctas[k][r3_index(r3)];
+    if (cached > 0) return cached;
+    int v = 0;
+    cudaError_t e = cudaSuccess;
+    if (k == FK_LS) {
+        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::lscorr_fft_kernel<R3>, 16 * R3,
+                                                                           fftc::lscorr_smem_float2<R3>() * sizeof(float2))));
+    } else if (k == FK_FIR) {
+        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::fir_fft_kernel<R3>, 16 * R3,
+                                                                           fftc::fir_smem_float2<R3>() * sizeof(float2))));
+    } else if (k == FK_CAF) {
+        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, false>, 16 * R3,
+                                                                           fftc::caf_smem_float2<R3>() * sizeof(float2))));
+    } else {
+        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, true>, 16 * R3,
+                                                                           fftc::caf_smem_float2<R3>() * sizeof(float2))));
+    }
+    if (e != cudaSuccess || v < 1) {
+        cudaGetLastError();
+        return 1;
+    }
+    cached = v;
+    return v;
+}
+
 // ---- LS correlations: segments of the channel
 struct LsFftPlan {
     bool on = false;
     int r3 = 8, nseg = 0, Bs = 0, ncta = 0, HT = 0;
 };
 
-LsFftPlan ls_fft_plan(const Ctx* c, long long n, int M, int nf) {
+LsFftPlan ls_fft_plan(Ctx* c, long long n, int M, int nf) {
     LsFftPlan pl;
     if (!g_fft.load() || n < g_fft_min_n.load() || M < 1 || M > 2048) return pl;
     pl.r3 = M <= 1024 ? 8 : 16;
@@ -586,9 +620,10 @@ LsFftPlan ls_fft_plan(const Ctx* c, long long n, int M, int nf) {
     pl.nseg = (int)((n + bmax - 1) / bmax);
     pl.Bs = (int)((n + pl.nseg - 1) / pl.nseg);
     pl.nseg = (int)((n + pl.Bs - 1) / pl.Bs);
-    // CTAs of one transform group (16 R3 threads), 3 resident per SM: the whole batch is ONE wave of CTAs, every CTA
-    // walks its share of a frame's segments (any split works: segments are independent)
-    const long long slots = 3ll * c->nsm;
+    // CTAs of one transform group (16 R3 threads), as many per SM as are resident at once (R3 = 8: 3, R3 = 16: 1): the
+    // whole batch is ONE wave of CTAs, every CTA walks its share of a frame's segments (any split works: segments are
+    // independent)
+    const long long slots = (long long)fft_ctas_per_sm(c, FK_LS, pl.r3) * c->nsm;
     pl.ncta = (int)std::max<long long>(1, std::min<long long>(pl.nseg, slots / nf));
     pl.HT = (M + 1) & ~1;
     pl.on = true;
@@ -659,8 +694,9 @@ int fir_fft(Ctx* c, int r3, const float2* ref, const float2* srv, float2* out, l
     p.n = (int)n; p.M = M; p.peek = peek; p.linear = linear ? 1 : 0;
     p.nseg = ceil_div(n, L - M + 1);
     p.tw = tw;
-    // one wave of CTAs for the whole batch (3 resident per SM: 68 KB of shared memory each)
-    const int per_frame = (int)std::max<long long>(1, std::min<long long>(p.nseg, 3ll * c->nsm / bt.nf));
+    // one wave of CTAs for the whole batch (R3 = 8: 3 resident per SM, 68 KB of shared memory each)
+    const long long slots = (long long)fft_ctas_per_sm(c, FK_FIR, r3) * c->nsm;
+    const int per_frame = (int)std::max<long long>(1, std::min<long long>(p.nseg, slots / bt.nf));
     {
         ProfScope ps(c, K_FIR);
         PRC_R3_SWITCH(r3, (fftc::fir_fft_kernel<R3><<<dim3(per_frame, bt.nf), 16 * R3, fftc::fir_smem_float2<R3>() * sizeof(float2), c->stream>>>(p)));
@@ -705,10 +741,14 @@ int caf_fft(Ctx* c, const CafFftPlan& pl, const float2* ref, const float2* srv, 
     p.n = (int)n; p.R = R; p.F = F; p.M = M; p.peek = peek;
     p.D = D; p.c0 = c0; p.ntaps = (int)ntaps; p.Bmax = pl.Bmax;
     p.P = c->fftP.as<float2>(); p.HT = pl.HT; p.tw = tw;
-    // one wave of CTAs for the whole batch (3 resident per SM): a CTA walks several Doppler blocks of its frame, so the
-    // twiddle tables are staged once per CTA and there is no partially filled last wave
+    // caf_wave: one wave of CTAs for the whole batch (R3 = 8: 3 resident per SM, shared memory bound): a CTA walks
+    // several Doppler blocks of its frame, so the twiddle tables are staged once per CTA and there is no partially
+    // filled last wave
     int gx = F;
-    if (g_caf_wave.load()) gx = (int)std::max<long long>(1, std::min<long long>(F, 3ll * c->nsm / bt.nf));
+    if (g_caf_wave.load()) {
+        const long long slots = (long long)fft_ctas_per_sm(c, wp ? FK_CAF_FUSED : FK_CAF, pl.r3) * c->nsm;
+        gx = (int)std::max<long long>(1, std::min<long long>(F, slots / bt.nf));
+    }
     const dim3 grid(gx, bt.nf);
     {
         ProfScope ps(c, K_LAGCORR_CAF);
@@ -1732,6 +1772,15 @@ const int* env_switch(const std::string& k) {
     return nullptr;
 }
 
+// read-only names of the residency the one-wave grids are sized from (fft_ctas_per_sm, R3 = 8 -- the transform
+// length of up to 1024 LS taps and of the CAF at config 2): the FftKern they report, -1 for any other name
+int fft_ctas_option(const std::string& k) {
+    if (k == "fft_ctas_ls") return FK_LS;
+    if (k == "fft_ctas_fir") return FK_FIR;
+    if (k == "fft_ctas_caf") return FK_CAF_FUSED;
+    return -1;
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2201,6 +2250,8 @@ int prc_set_option(const char* name, int value) {
     else if (k == "caf_wave") g_caf_wave.store(value);
     else if (env_switch(k) || k == "tma_active")
         return fail(PRC_E_INVALID, "option '%s' is read-only (set from the environment when the library starts)", name);
+    else if (fft_ctas_option(k) >= 0)
+        return fail(PRC_E_INVALID, "option '%s' is read-only (CTAs per SM of the build's kernels on this device)", name);
     else return fail(PRC_E_INVALID, "unknown option '%s'", name);
     return PRC_OK;
 }
@@ -2214,6 +2265,14 @@ int prc_get_option(const char* name, int* value) {
     else if (k == "caf_wave") *value = g_caf_wave.load();
     else if (const int* s = env_switch(k)) *value = *s;
     else if (k == "tma_active") *value = use_tma() ? 1 : 0;
+    else if (fft_ctas_option(k) >= 0) {
+        int dev = 0;
+        CU(cudaGetDevice(&dev));
+        Ctx* c;
+        TRY(get_ctx(dev, nullptr, &c));
+        std::lock_guard<std::mutex> lk(c->mu);
+        *value = fft_ctas_per_sm(c, (FftKern)fft_ctas_option(k), 8);
+    }
     else return fail(PRC_E_INVALID, "unknown option '%s'", name);
     return PRC_OK;
 }
