@@ -327,6 +327,37 @@ int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int 
                             int64_t frame_stride, double range_extent, double doppler_extent,
                             prc_track_simple* history, int mem_kind, int device, void* stream, unsigned flags);
 
+/* ---- channel offset estimator ---------------------------------------------------------------------
+ * prc_channel_offset replaces find_channel_offset(s1, s2, nd, nl), reference passiveRadar/signal_utils.py:73-78:
+ *   B1 = decimate(s1, nd), B2 = pad(decimate(s2, nd), (nl, nl)), xc = |correlate(B1, B2, 'valid')|,
+ *   *offset = (argmax(xc) - nl) * nd   (the first maximum on ties).
+ * decimate is scipy.signal.decimate's default: sosfiltfilt with the order-8 Chebyshev sections
+ * cheby1(8, 0.05, 0.8 / nd, output='sos') (odd extension of 27 samples, computed in the input's own dtype as NumPy
+ * does, so integer inputs wrap), then every nd-th sample.  sos: 2 x 4 x 6 doubles and zi: 2 x 4 x 2 doubles
+ * (= sosfilt_zi(sos)), one block per signal, designed by the caller as decimate does for that signal's dtype (float32-
+ * rounded for float32 / complex64 inputs).  All arithmetic is float64 / complex128 whatever the dtypes.
+ *   offset : one int64 (host or device, as mem_kind says)
+ *   xc_abs : NULL, or the |n1d - (n2d + 2 nl)| + 1 values of |xc| as doubles, n_d = ceil(n / nd)
+ * Limits (PRC_E_INVALID): n1, n2 > 27; 1 <= nd <= 64; nl >= 0; a circular transform of at most 2^26 points.
+ *
+ * prc_xcorr replaces xcorr(s1, s2, nlead, nlag) = correlate(s1, pad(s2, (nlag, nlead)), 'valid') (:29-32): out
+ * receives the |n1 - (n2 + nlag + nlead)| + 1 valid lags, complex128 when either input is complex, else float64.
+ *
+ * Scratch memory is allocated stream-ordered on the call's stream and released before the call returns it.
+ */
+#define PRC_DT_I8    0
+#define PRC_DT_U8    1
+#define PRC_DT_I16   2
+#define PRC_DT_F32   3
+#define PRC_DT_F64   4
+#define PRC_DT_C64   5
+#define PRC_DT_C128  6
+int prc_channel_offset(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2, int64_t n2, int nd, int64_t nl,
+                       const double* sos, const double* zi, int64_t* offset, double* xc_abs,
+                       int mem_kind, int device, void* stream, unsigned flags);
+int prc_xcorr(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2, int64_t n2, int64_t nlead, int64_t nlag,
+              void* out, int mem_kind, int device, void* stream, unsigned flags);
+
 #ifdef __cplusplus
 }
 #endif

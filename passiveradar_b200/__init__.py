@@ -12,13 +12,15 @@ this package never imports the CPU oracle and never falls back to the CPU.
 from .range_doppler_processing import fast_xambg, direct_xambg            # noqa: F401
 from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # noqa: F401
                               LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames)
-from .signal_utils import deinterleave_IQ, frequency_shift, resample, frontend            # noqa: F401
+from .signal_utils import (deinterleave_IQ, frequency_shift, resample, frontend,            # noqa: F401
+                           find_channel_offset, offset_compensation, shift, xcorr)
 from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
                                multitarget_tracker_frames, simple_tracker_frames, cfar_track,
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
-           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend", "CFAR_2D",
+           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
+           "find_channel_offset", "offset_compensation", "shift", "xcorr", "CFAR_2D",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
            "simple_tracker_frames", "cfar_track"]
 __version__ = "0.1.0"
@@ -27,7 +29,7 @@ __version__ = "0.1.0"
 def install(reference_package: str = "passiveRadar"):
     """Swap the hot-path functions of an importable copy of the reference for the GPU ones.
 
-    ``main.py`` binds ``fast_xambg``, ``LS_Filter_Multiple`` and ``NLMS_filter`` with
+    ``main.py`` binds ``fast_xambg``, ``LS_Filter_Multiple``, ``NLMS_filter`` and ``find_channel_offset`` with
     ``from passiveRadar... import ...`` (main.py:10-14); calling ``install()`` before ``main.py`` is
     imported/run makes those names resolve to this package while config, I/O and the dask graph stay
     the reference's own code::
@@ -40,7 +42,9 @@ def install(reference_package: str = "passiveRadar"):
     replaced = []
     table = {
         "range_doppler_processing": {"fast_xambg": fast_xambg, "direct_xambg": direct_xambg},
-        "signal_utils": {"deinterleave_IQ": deinterleave_IQ, "frequency_shift": frequency_shift, "resample": resample},
+        # xcorr stays the reference's: only its LS_Filter_Toeplitz and direct_xambg call it, and both are replaced
+        "signal_utils": {"deinterleave_IQ": deinterleave_IQ, "frequency_shift": frequency_shift, "resample": resample,
+                         "find_channel_offset": find_channel_offset, "offset_compensation": offset_compensation},
         "target_detection": {"CFAR_2D": CFAR_2D, "get_measurements": get_measurements,
                              "multitarget_tracker": multitarget_tracker, "simple_target_tracker": simple_target_tracker},
         "clutter_removal": {"LS_Filter": LS_Filter, "NLMS_filter": NLMS_filter,

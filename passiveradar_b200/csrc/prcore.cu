@@ -32,6 +32,7 @@
 #include "gal.cuh"
 #include "track.cuh"
 #include "fftcorr.cuh"
+#include "chanoff.cuh"
 
 namespace {
 
@@ -55,10 +56,11 @@ std::atomic<uint64_t> g_launches{0};
 
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
-                K_TRK_SIMPLE, K_COUNT };
+                K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
-                                           "track_multi", "track_simple"};
+                                           "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
+                                           "chanoff_fft", "chanoff_argmax"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -1781,6 +1783,168 @@ int fft_ctas_option(const std::string& k) {
     return -1;
 }
 
+// ---- channel offset / xcorr (chanoff.cuh) ---------------------------------------------------------------------------
+constexpr int CHANOFF_MAX_ND = 64;          // largest decimation factor (its pole radius 0.9971 sets W ~ 14k samples)
+constexpr int CHANOFF_MAX_LOG2 = 26;        // largest transform: 2^26 complex128 = 1 GiB per buffer
+
+// Stream-ordered scratch of one call: once per run, and ~0.5 GB at main.py's shapes, so it is not kept in the Ctx
+struct AsyncScratch {
+    cudaStream_t st;
+    std::vector<void*> ptrs;
+    explicit AsyncScratch(cudaStream_t s) : st(s) {}
+    ~AsyncScratch() { for (void* p : ptrs) cudaFreeAsync(p, st); }
+    template <class T> int get(T** out, size_t bytes) {
+        void* p = nullptr;
+        cudaError_t e = cudaMallocAsync(&p, bytes ? bytes : 16, st);
+        if (e != cudaSuccess) { cudaGetLastError(); return fail(PRC_E_NOMEM, "cudaMallocAsync(%zu): %s", bytes, cudaGetErrorString(e)); }
+        ptrs.push_back(p);
+        *out = static_cast<T*>(p);
+        return PRC_OK;
+    }
+};
+
+bool chanoff_bad_dtype(int dt) { return dt < chanoff::DT_I8 || dt > chanoff::DT_C128; }
+
+// W: samples after which a zero-state start of the cascade agrees with the exact state below float64 round-off
+// (DESIGN.md section 11): the transient decays as r^k for the largest pole radius r, times a polynomial in k for the
+// four nearly repeated pole pairs, which the 256-sample margin covers
+int chanoff_warmup(const chanoff::Sos& f, long long* warm) {
+    double r = 0.0;
+    for (int s = 0; s < chanoff::NSEC; ++s) {
+        if (f.s[s][3] != 1.0) return fail(PRC_E_INVALID, "sos section %d: a0 = %g, must be 1", s, f.s[s][3]);
+        const double a1 = f.s[s][4], a2 = f.s[s][5], disc = a1 * a1 - 4.0 * a2;
+        const double rs = disc < 0.0 ? std::sqrt(a2) : std::max(std::fabs(-a1 + std::sqrt(disc)), std::fabs(-a1 - std::sqrt(disc))) / 2.0;
+        r = std::max(r, rs);
+    }
+    if (!(r < 1.0)) return fail(PRC_E_INVALID, "the decimation filter is not stable (pole radius %g)", r);
+    *warm = (long long)std::ceil(std::log(1e-18) / std::log(r)) + 256;
+    return PRC_OK;
+}
+
+// xc[k] = sum_i a[i + k + p0] conj(b[i]) over the nvalid valid lags of correlate(A, pad(B, (pad_l, pad_r)), 'valid'),
+// A, B = the inputs, decimated (f != nullptr: sosfiltfilt + [::nd]) or as they are.  mode ARG_ABS: |xc| -> out
+// (optional) and res[0..1] = argmax, (argmax - nl) * nd; ARG_COMPLEX / ARG_REAL: the lags -> out.
+int chanoff_device(Ctx* c, AsyncScratch& ws, const void* s1, int dt1, long long n1, const void* s2, int dt2, long long n2,
+                   const chanoff::Sos* f, int nd, long long pad_l, long long pad_r, int mode, void* out, long long* res) {
+    using namespace chanoff;
+    const long long n1d = f ? (n1 + nd - 1) / nd : n1, n2d = f ? (n2 + nd - 1) / nd : n2;
+    const long long lenb = n2d + pad_l + pad_r;
+    const long long nvalid = (n1d >= lenb ? n1d - lenb : lenb - n1d) + 1;
+    const long long p0 = (n1d >= lenb ? 0 : n1d - lenb) + pad_l;
+    // circular length with no valid lag aliased: p + L beyond the support's top n1d - 1, p - L below -(n2d - 1)
+    const long long need = std::max(std::max(std::max(n1d, n2d), std::max(p0 + nvalid - 1 + n2d, n1d - p0)), 2ll);
+    int m = 1;
+    while (m <= CHANOFF_MAX_LOG2 && (1ll << m) < need) ++m;
+    if (m > CHANOFF_MAX_LOG2)
+        return fail(PRC_E_INVALID, "the correlation needs a transform of %lld points; the maximum is 2^%d = %lld", need,
+                    CHANOFF_MAX_LOG2, 1ll << CHANOFF_MAX_LOG2);
+    const long long L = 1ll << m;
+    double2 *X, *Y, *tlo, *thi;
+    const int nhi = (int)std::max(1ll, (L / 2) >> TW_LO_BITS);
+    TRY(ws.get(&X, (size_t)L * sizeof(double2)));
+    TRY(ws.get(&Y, (size_t)L * sizeof(double2)));
+    TRY(ws.get(&tlo, ((size_t)1 << TW_LO_BITS) * sizeof(double2)));
+    TRY(ws.get(&thi, (size_t)nhi * sizeof(double2)));
+    CU(cudaMemsetAsync(X + n1d, 0, (size_t)(L - n1d) * sizeof(double2), c->stream));
+    CU(cudaMemsetAsync(Y + n2d, 0, (size_t)(L - n2d) * sizeof(double2), c->stream));
+    if (f) {
+        const long long nmax = std::max(n1, n2) + 2 * PADLEN;
+        double* F;
+        TRY(ws.get(&F, (size_t)nmax * sizeof(double2)));
+        const void* src[2] = {s1, s2};
+        const int dts[2] = {dt1, dt2};
+        const long long ns[2] = {n1, n2};
+        double2* dst[2] = {X, Y};
+        for (int q = 0; q < 2; ++q) {
+            IirParams ip{};
+            ip.f = f[q];
+            TRY(chanoff_warmup(f[q], &ip.warm));
+            ip.dt = dts[q];
+            ip.n = ns[q];
+            ip.next = ns[q] + 2 * PADLEN;
+            ip.chunk = std::max(256ll, (ip.next + 16383) / 16384);
+            ip.nd = nd;
+            const bool cplx = dt_complex(dts[q]);
+            ProfScope ps(c, K_CHANOFF_IIR);
+            ip.x = src[q];
+            ip.y = F;
+            launch_iir(ip, cplx, false, c->stream);
+            TRY(check_launch("chanoff_iir_kernel(forward)"));
+            ip.x = F;
+            ip.y = dst[q];
+            launch_iir(ip, cplx, true, c->stream);
+            TRY(check_launch("chanoff_iir_kernel(backward)"));
+        }
+    } else {
+        ProfScope ps(c, K_CHANOFF_LOAD);
+        launch_load(s1, dt1, n1, X, c->nsm, c->stream);
+        launch_load(s2, dt2, n2, Y, c->nsm, c->stream);
+        TRY(check_launch("chanoff_load_kernel"));
+    }
+    // passes from the top index bits down: 8 bits (x 8 consecutive columns) while more than 11 remain, then the rest
+    struct Pass { int lo, nb, c, s0; };
+    std::vector<Pass> passes;
+    for (int top = m; top > 0;) {
+        const int nb = top <= FFT_TILE_BITS ? top : 8, lo = top - nb;
+        passes.push_back(Pass{lo, nb, std::min(3, lo), m - top});
+        top = lo;
+    }
+    {
+        ProfScope ps(c, K_CHANOFF_FFT);
+        launch_twiddle(tlo, thi, nhi, m, c->stream);
+        TRY(check_launch("chanoff_twiddle_kernel"));
+        FftParams fp{};
+        fp.buf[0] = X; fp.buf[1] = Y;
+        fp.tw_lo = tlo; fp.tw_hi = thi;
+        fp.m = m;
+        for (int k = 0; k < 2 * (int)passes.size(); ++k) {      // forward passes of X and Y, then the inverse of X conj(Y)
+            const bool inverse = k >= (int)passes.size();
+            const Pass& ps_ = inverse ? passes[2 * passes.size() - 1 - k] : passes[k];
+            fp.lo = ps_.lo; fp.nb = ps_.nb; fp.c = ps_.c; fp.s0 = ps_.s0;
+            fp.product = k == (int)passes.size();
+            launch_fft_pass(fp, inverse, c->stream);
+            TRY(check_launch("chanoff_fft_kernel"));
+        }
+    }
+    ArgParams ap{};
+    ap.cc = X; ap.L = L; ap.nvalid = nvalid; ap.p0 = p0;
+    ap.scale = 1.0 / (double)L;
+    ap.mode = mode;
+    ap.out = out;
+    const int nb = argmax_blocks(nvalid);
+    ProfScope ps(c, K_CHANOFF_ARGMAX);
+    if (mode == ARG_ABS) {
+        TRY(ws.get(&ap.part_v, (size_t)nb * sizeof(double)));
+        TRY(ws.get(&ap.part_k, (size_t)nb * sizeof(long long)));
+    }
+    launch_argmax(ap, nb, c->stream);
+    TRY(check_launch("chanoff_argmax_kernel"));
+    if (mode == ARG_ABS) {
+        launch_argmax_final(ap.part_v, ap.part_k, nb, pad_l, nd, res, c->stream);
+        TRY(check_launch("chanoff_argmax_final_kernel"));
+    }
+    return PRC_OK;
+}
+
+int chanoff_inputs(const void* s1, int dt1, int64_t n1, const void* s2, int dt2, int64_t n2, int mem_kind) {
+    if (!s1 || !s2) return fail(PRC_E_INVALID, "s1/s2 must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (chanoff_bad_dtype(dt1) || chanoff_bad_dtype(dt2)) return fail(PRC_E_INVALID, "dtype %d / %d invalid", dt1, dt2);
+    if (n1 < 1 || n2 < 1) return fail(PRC_E_INVALID, "n1=%lld n2=%lld invalid", (long long)n1, (long long)n2);
+    return PRC_OK;
+}
+
+// host inputs -> stream-ordered device copies of their raw bytes (int8 stays one byte per sample over PCIe)
+int chanoff_stage(Ctx* c, AsyncScratch& ws, const void** s, int dt, int64_t n, int mem_kind, unsigned flags) {
+    if (mem_kind == PRC_MEM_DEVICE) return PRC_OK;
+    const size_t b = (size_t)n * chanoff::dt_size(dt);
+    void* d;
+    TRY(ws.get(&d, b));
+    TRY(h2d(c, d, *s, b, flags));
+    *s = d;
+    return PRC_OK;
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2612,6 +2776,66 @@ int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int 
     }
     TRY(check_launch("track_simple_kernel"));
     if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, history, dh, hb, flags));
+    return finish(c, flags);
+}
+
+int prc_channel_offset(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2, int64_t n2, int nd, int64_t nl,
+                       const double* sos, const double* zi, int64_t* offset, double* xc_abs,
+                       int mem_kind, int device, void* stream, unsigned flags) {
+    TRY(chanoff_inputs(s1, dtype1, n1, s2, dtype2, n2, mem_kind));
+    if (!sos || !zi || !offset) return fail(PRC_E_INVALID, "sos/zi/offset must not be NULL");
+    if (nd < 1 || nd > CHANOFF_MAX_ND) return fail(PRC_E_INVALID, "nd=%d outside [1, %d]", nd, CHANOFF_MAX_ND);
+    if (nl < 0) return fail(PRC_E_INVALID, "nl=%lld invalid", (long long)nl);
+    if (n1 <= chanoff::PADLEN || n2 <= chanoff::PADLEN)
+        return fail(PRC_E_INVALID, "The length of the input vector x must be greater than padlen, which is %d.", chanoff::PADLEN);
+    chanoff::Sos f[2];
+    for (int q = 0; q < 2; ++q) {
+        memcpy(f[q].s, sos + 24 * q, sizeof f[q].s);
+        memcpy(f[q].zi, zi + 8 * q, sizeof f[q].zi);
+        long long w;
+        TRY(chanoff_warmup(f[q], &w));               // before any CUDA call
+    }
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    AsyncScratch ws(c->stream);
+    TRY(chanoff_stage(c, ws, &s1, dtype1, n1, mem_kind, flags));
+    TRY(chanoff_stage(c, ws, &s2, dtype2, n2, mem_kind, flags));
+    long long* res;
+    TRY(ws.get(&res, 2 * sizeof(long long)));
+    const long long n1d = (n1 + nd - 1) / nd, n2d = (n2 + nd - 1) / nd, lenb = n2d + 2 * nl;
+    const long long nvalid = (n1d >= lenb ? n1d - lenb : lenb - n1d) + 1;
+    double* xc = xc_abs;
+    if (xc_abs && mem_kind == PRC_MEM_HOST) TRY(ws.get(&xc, (size_t)nvalid * sizeof(double)));
+    TRY(chanoff_device(c, ws, s1, dtype1, n1, s2, dtype2, n2, f, nd, nl, nl, chanoff::ARG_ABS, xc, res));
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(d2h(c, offset, res + 1, sizeof(long long), flags));
+        if (xc_abs) TRY(d2h(c, xc_abs, xc, (size_t)nvalid * sizeof(double), flags));
+    } else {
+        CU(cudaMemcpyAsync(offset, res + 1, sizeof(long long), cudaMemcpyDeviceToDevice, c->stream));
+    }
+    return finish(c, flags);
+}
+
+int prc_xcorr(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2, int64_t n2, int64_t nlead, int64_t nlag,
+              void* out, int mem_kind, int device, void* stream, unsigned flags) {
+    TRY(chanoff_inputs(s1, dtype1, n1, s2, dtype2, n2, mem_kind));
+    if (!out) return fail(PRC_E_INVALID, "out must not be NULL");
+    if (nlead < 0 || nlag < 0) return fail(PRC_E_INVALID, "nlead=%lld nlag=%lld invalid", (long long)nlead, (long long)nlag);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    AsyncScratch ws(c->stream);
+    TRY(chanoff_stage(c, ws, &s1, dtype1, n1, mem_kind, flags));
+    TRY(chanoff_stage(c, ws, &s2, dtype2, n2, mem_kind, flags));
+    const bool cplx = chanoff::dt_complex(dtype1) || chanoff::dt_complex(dtype2);
+    const long long lenb = n2 + nlag + nlead;
+    const size_t ob = (size_t)((n1 >= lenb ? n1 - lenb : lenb - n1) + 1) * (cplx ? sizeof(double2) : sizeof(double));
+    void* dout = out;
+    if (mem_kind == PRC_MEM_HOST) TRY(ws.get(&dout, ob));
+    TRY(chanoff_device(c, ws, s1, dtype1, n1, s2, dtype2, n2, nullptr, 1, nlag, nlead,
+                       cplx ? chanoff::ARG_COMPLEX : chanoff::ARG_REAL, dout, nullptr));
+    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, ob, flags));
     return finish(c, flags);
 }
 

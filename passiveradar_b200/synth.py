@@ -107,3 +107,25 @@ def track_maps(seed, rows, cols, T, targets=4):
                 if 0 <= c + dc < cols:
                     maps[t, (r + dr) % rows, c + dc] += np.float32(0.5 * amp)
     return maps
+
+
+def offset_pair(n1, n2, kind="int8", delay=0, seed=5):
+    """Seeded two-channel capture of one illuminator for the channel-offset estimator: s2[j] = s1[j + delay] (same
+    source, ``delay`` samples apart; independent receiver noise on each channel), as ``int8`` raw samples, ``uint8``
+    offset-binary samples or ``complex64`` IQ, of n1 and n2 samples."""
+    rng = np.random.default_rng(seed)
+    a = max(0, -delay)
+    total = a + max(n1, delay + n2) + 1
+    if kind == "complex64":
+        u = white_iq(rng, total)
+        s1 = u[a:a + n1] + np.complex64(0.1) * white_iq(rng, n1)
+        s2 = u[a + delay:a + delay + n2] + np.complex64(0.1) * white_iq(rng, n2)
+        return s1.astype(np.complex64), s2.astype(np.complex64)
+    u = rng.integers(-96, 96, size=total)
+    s1 = u[a:a + n1] + rng.integers(-16, 17, size=n1)
+    s2 = u[a + delay:a + delay + n2] + rng.integers(-16, 17, size=n2)
+    if kind == "int8":
+        return s1.astype(np.int8), s2.astype(np.int8)
+    if kind == "uint8":
+        return (s1 + 128).astype(np.uint8), (s2 + 128).astype(np.uint8)
+    raise ValueError(f"unknown offset-pair kind {kind!r}")
