@@ -246,6 +246,9 @@ int prc_direct_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
  * padtype='line') (signal_utils.py:15-17) in the same pass: h = the nh = 2*half_len+1 low-pass taps
  * ALREADY multiplied by up (what resample_poly hands to upfirdn; host doubles, designed by the caller
  * with scipy.signal.firwin exactly as resample_poly does).  out receives prc_resample_out_len() samples.
+ * With n = 1 the line extension's slope is 0/0 and every output is NaN, as resample_poly gives.  One CTA
+ * stages its taps and input window in at most 200 KB of shared memory: at up = 1 the largest down is 89, at
+ * up = 2 it is 171; a ratio beyond returns PRC_E_INVALID with the bytes it needs.
  */
 #define PRC_IQ_C64   0
 #define PRC_IQ_I8    1
@@ -267,7 +270,10 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
  * divided by the wrapped 2-D box average (fw x fw window minus the guard hole) + 1e-10.
  * x: rows x cols float32 (or complex64 with PRC_FLAG_ABS_C64: the magnitude is taken on the device, so
  * a map can go from prc_xambg_c64 to the detector without leaving HBM).  cr_out (float32) and/or
- * det_out (uint8, cr > *thresh) are written; thresh may be NULL when det_out is NULL.
+ * det_out (uint8, cr > *thresh) are written; thresh may be NULL when det_out is NULL.  The window sum and
+ * the division are evaluated in float64, as the reference's float64 Tfilt makes convolve2d do, so signed
+ * real maps are held to the reference too.  Limits: 1 <= fw <= 64, rows <= 524 280 (65 535 CTA rows of 8);
+ * beyond either the call returns PRC_E_INVALID naming the limit.
  */
 int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const float* thresh, float* cr_out,
                    uint8_t* det_out, int mem_kind, int device, void* stream, unsigned flags);

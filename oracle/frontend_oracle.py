@@ -29,9 +29,10 @@ def frontend_oracle(interleavedIQ, fc, Fs, phase_offset, up, dn):
     return resample_oracle(frequency_shift_oracle(deinterleave_iq_oracle(interleavedIQ), fc, Fs, phase_offset), up, dn)
 
 
-def resample_truth(x, up, dn):
+def resample_truth(x, up, dn, ms=None):
     """float64 statement of resample_poly(padtype='line') written out as the polyphase sum the device
-    kernel evaluates (independent of SciPy's upfirdn): used to check the index arithmetic."""
+    kernel evaluates (independent of SciPy's upfirdn): used to check the index arithmetic.  ``ms``: only
+    these output indices (the loop is per output sample), returned in that order."""
     import math
     x = np.asarray(x, dtype=np.complex128)
     g = math.gcd(up, dn)
@@ -46,14 +47,15 @@ def resample_truth(x, up, dn):
     n_out = n * up // dn + bool(n * up % dn)
     hpad = np.concatenate((np.zeros(n_pre_pad), h))
     slope = (x[-1] - x[0]) / (n - 1)
-    out = np.zeros(n_out, dtype=np.complex128)
-    for m in range(n_out):
+    ms = range(n_out) if ms is None else ms
+    out = np.zeros(len(ms), dtype=np.complex128)
+    for q, m in enumerate(ms):
         T = (m + n_pre_remove) * dn
         ih, ph = divmod(T, up)
         k = np.arange(ph, hpad.shape[0], up)
         i = ih - np.arange(k.shape[0])
         xe = np.where(i < 0, x[0] + i * slope, np.where(i >= n, x[-1] + (i - n + 1) * slope, x[np.clip(i, 0, n - 1)]))
-        out[m] = np.dot(hpad[k], xe)
+        out[q] = np.dot(hpad[k], xe)
     return out
 
 

@@ -110,8 +110,8 @@ __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_const
     const long long i_lo = i_hi0 - (p.tpp - 1);              // smallest index any output of the CTA needs
     for (int q = threadIdx.x; q < p.up * p.tpp; q += RS_THREADS) hp[q] = p.hp[q];
     const float2 x0 = p.ends[0], x1 = p.ends[1];
-    float2 slope = make_float2(0.f, 0.f);
-    if (n > 1) slope = make_float2((x1.x - x0.x) / (float)(n - 1), (x1.y - x0.y) / (float)(n - 1));
+    // n == 1 gives 0/0 = NaN, and every output NaN, as scipy's padtype='line' does
+    const float2 slope = make_float2((x1.x - x0.x) / (float)(n - 1), (x1.y - x0.y) / (float)(n - 1));
     for (int q = threadIdx.x; q < p.span; q += RS_THREADS) {
         const long long i = i_lo + q;
         float2 v;

@@ -1350,6 +1350,8 @@ int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const 
 int cfar_device(Ctx* c, const void* x, bool is_complex, int rows, int cols, int fw, int gw, const float* thresh,
                 float* cr, uint8_t* det) {
     if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
+    if (rows > CFAR_MAX_ROWS)          // one CTA row of tiles per gridDim.y index
+        return fail(PRC_E_INVALID, "rows=%d exceed the CFAR maximum of %d rows", rows, CFAR_MAX_ROWS);
     if (fw < 1 || fw > CFAR_MAX_FW) return fail(PRC_E_INVALID, "fw=%d outside [1, %d]", fw, CFAR_MAX_FW);
     if (gw < 0 || fw * fw - gw * gw == 0) return fail(PRC_E_INVALID, "fw=%d gw=%d: fw^2 - gw^2 must not be 0", fw, gw);
     TRY(c->cf_part.ensure(CFAR_MEAN_CTAS * sizeof(double)));
@@ -1362,14 +1364,23 @@ int cfar_device(Ctx* c, const void* x, bool is_complex, int rows, int cols, int 
     if (e1 < 0) e1 = std::max(0, e1 + fw);     // negative slice start counts from the end
     p.e1 = std::min(e1, fw); p.e2 = std::min(std::max(e2, 0), fw);
     p.c = (fw - 1) / 2;
-    p.scale = (float)(1.0 / ((double)fw * fw - (double)gw * gw));
+    p.scale = 1.0 / ((double)fw * fw - (double)gw * gw);
     p.has_thresh = thresh ? 1 : 0;
     p.thresh = thresh ? *thresh : 0.f;
     p.partial = c->cf_part.as<double>();
     p.cr = cr; p.det = det;
     ProfScope ps(c, K_MISC);
     cfar_abssum_kernel<<<CFAR_MEAN_CTAS, 256, 0, c->stream>>>(p, c->cf_part.as<double>());
-    const size_t smem = (size_t)(CFAR_TX + fw - 1) * (CFAR_TY + fw - 1) * sizeof(float);
+    const size_t smem = (size_t)(CFAR_TX + fw - 1) * (CFAR_TY + fw - 1) * sizeof(double);   // 53 960 B at fw = 64
+    {   // under a lock: a concurrent first call must not launch before the attribute is set
+        static std::mutex attr_mu;
+        static bool attr_set[64];
+        std::lock_guard<std::mutex> g(attr_mu);
+        if (!attr_set[c->device]) {
+            CU(cudaFuncSetAttribute(cfar2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT));
+            attr_set[c->device] = true;
+        }
+    }
     cfar2d_kernel<<<dim3(ceil_div(cols, CFAR_TX), ceil_div(rows, CFAR_TY)), dim3(CFAR_TX, CFAR_TY), smem, c->stream>>>(p);
     return check_launch("cfar2d_kernel");
 }
