@@ -206,6 +206,24 @@ int prc_gal_jpe_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, in
                            prc_c64* out, prc_c64* k_out, prc_c64* h_out,
                            int mem_kind, int device, void* stream, unsigned flags);
 
+/* ---- SVD least-squares clutter filter ------------------------------------------------------------------
+ * prc_ls_svd_frames_c64 replaces LS_Filter_SVD(), reference passiveRadar/clutter_removal.py:58-107, on nframes
+ * independent frames (frame i at ref/srv/out + i*frame_stride; a single frame is nframes = 1).  With the data
+ * matrix A[:, k] = roll(ref, k - peek), M = filter_len + peek columns, the taps are the minimum-norm least-squares
+ * solution of A taps = srv, computed from the Hermitian Toeplitz Gram matrix A^H A (A itself is never formed):
+ * its eigenvalues below max(1e-20, 1e-10 * largest) -- singular values of A below max(1e-10, 1e-5 * largest) --
+ * are dropped (DESIGN.md section 13).  All arithmetic is float64; out is rounded to complex64 once.
+ *   out      : n samples per frame, srv - A taps                                           (:102)
+ *   taps_out : nframes * M taps rounded to complex64, or NULL                              (:99)
+ *   rank_out : nframes ints, or NULL: the number of kept singular values; -1 when the input is not finite or the
+ *              eigensolver does not converge, and that frame's out and taps are NaN
+ * Requires n >= 1, filter_len >= 0, peek >= 0 and 1 <= M <= 1024 (PRC_E_INVALID naming the limit otherwise).
+ * One CTA per frame runs the eigensolver, so a batch of frames is what fills the GPU.
+ */
+int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                          int filter_len, int peek, prc_c64* out, prc_c64* taps_out, int* rank_out,
+                          int mem_kind, int device, void* stream, unsigned flags);
+
 /* ---- run-time switches (also read once from the environment: PRC_FFT, PRC_FFT_MIN_N) ----------------
  *   "fft"        1 (default): LS correlations, clutter FIR and CAF block sums as FFT-domain block correlations
  *                (csrc/fftcorr.cuh);  0: direct form on wgmma / FP32 (csrc/toepcorr.cuh, firtc.cuh, lagstream.cuh)

@@ -2,7 +2,7 @@
 
 Drop-in operators with the reference's call signatures (Max-Manning/passiveRadar):
 
-    from passiveradar_b200 import fast_xambg, LS_Filter, NLMS_filter, block_NLMS, GAL_JPE
+    from passiveradar_b200 import fast_xambg, LS_Filter, NLMS_filter, block_NLMS, GAL_JPE, LS_Filter_SVD
 
 and a device-resident frame pipeline for streams of CPI frames
 (``passiveradar_b200.frames.FramePipeline``).  All arithmetic runs in
@@ -11,7 +11,8 @@ this package never imports the CPU oracle and never falls back to the CPU.
 """
 from .range_doppler_processing import fast_xambg, direct_xambg            # noqa: F401
 from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # noqa: F401
-                              LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames)
+                              LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames,
+                              LS_Filter_SVD, ls_filter_svd_frames)
 from .signal_utils import (deinterleave_IQ, frequency_shift, resample, frontend,            # noqa: F401
                            find_channel_offset, offset_compensation, shift, xcorr)
 from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
@@ -19,7 +20,7 @@ from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, s
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
-           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
+           "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
            "find_channel_offset", "offset_compensation", "shift", "xcorr", "CFAR_2D",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
            "simple_tracker_frames", "cfar_track"]

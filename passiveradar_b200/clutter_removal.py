@@ -2,7 +2,8 @@
 
 Drop-ins for ``passiveRadar.clutter_removal.LS_Filter`` (reference
 ``passiveRadar/clutter_removal.py:6-56``), ``NLMS_filter`` (``:189-249``) and ``GAL_JPE``
-(``:251-364``; ``gal_jpe_frames`` runs a batch of frames in one call), plus
+(``:251-364``; ``gal_jpe_frames`` runs a batch of frames in one call), ``LS_Filter_SVD`` (``:58-107``;
+``ls_filter_svd_frames`` likewise), plus
 ``block_NLMS`` (not in the reference; DESIGN.md defines it so that ``blockLen=1``
 is ``NLMS_filter``).  All arithmetic runs in ``libprcore.so``; no CPU fallback.
 """
@@ -219,3 +220,107 @@ def LS_Filter_Multiple(refChannel, srvChannel, filterLen, sampleRate, dopplerBin
                                  bins.ctypes.data, bins.shape[0], out.ctypes.data, None, _lib.MEM_HOST, dev, None, 0)
     _lib.check(st)
     return out.astype(np.complex128)
+
+
+def _svd_args(filterLen, peek):
+    filterLen, peek = int(filterLen), int(peek)
+    if filterLen < 0:
+        raise ValueError(f"filterLen must be >= 0, got {filterLen}")
+    if peek < 0:
+        raise ValueError(f"peek must be >= 0, got {peek}")
+    return filterLen, peek
+
+
+def _ls_svd(ref, srv, filterLen, peek, device):
+    """2-D complex64 (nframes x n) -> out (nframes x n), taps (nframes x M) complex64 and ranks (int32)."""
+    nframes, n = ref.shape
+    ntaps = filterLen + peek
+    out = np.empty((nframes, n), dtype=np.complex64)
+    taps = np.zeros((nframes, ntaps), dtype=np.complex64)
+    rank = np.zeros(nframes, dtype=np.int32)
+    if ntaps == 0 or nframes == 0:
+        out[...] = srv
+        return out, taps, rank
+    if n == 0:
+        return out, taps, rank
+    lib = _lib.load()
+    dev = _lib.current_device() if device is None else int(device)
+    st = lib.prc_ls_svd_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nframes, n, filterLen, peek, out.ctypes.data,
+                                   taps.ctypes.data, rank.ctypes.data, _lib.MEM_HOST, dev, None, 0)
+    _lib.check(st)
+    return out, taps, rank
+
+
+def LS_Filter_SVD(refChannel, srvChannel, filterLen, peek=10, return_filter=False, *, device=None):
+    '''Block least squares adaptive filter through the singular value decomposition -- the reference's
+    ``LS_Filter_SVD`` (``clutter_removal.py:58-107``), which "doesn't get upset if the data matrix is close to
+    singular": a silent, single-carrier or periodic reference channel, where ``LS_Filter(reg=0)`` raises
+    ``LinAlgError`` and ``LS_Filter_Toeplitz`` fails.
+
+    The taps are the minimum-norm least-squares solution of ``A taps = srv``, ``A[:, k] = roll(ref, k - peek)``
+    (``filterLen + peek`` columns, at most 1024).  The GPU never forms ``A``: it decomposes the Hermitian Toeplitz
+    Gram matrix ``A^H A`` in float64 (Householder tridiagonalisation and implicit-shift QL) and drops singular value
+    ``S_k`` when ``S_k < max(1e-10, 1e-5 * S_max)``.  The reference drops ``S_k < 1e-10`` only; going through the
+    Gram matrix squares the condition number, so a null direction of ``A`` shows up at ~1e-8 ``S_max`` even in
+    float64, and the relative floor is what separates it (DESIGN.md section 13).  The residual
+    ``srv - A @ taps`` is accumulated in float64 and rounded once.
+
+    ``refChannel`` is rounded to complex64, as the reference's ``A`` is, and ``srvChannel`` is sent to the GPU as
+    complex64.  ``srvChannelFiltered`` and, with ``return_filter=True``, the taps come back in
+    ``np.result_type(np.complex64, srvChannel.dtype)`` as the reference's do; for complex128 / float64 inputs the
+    result is widened, so the complex64 rounding of ``srvChannel`` is the only extra error.
+
+    Raises ``ValueError`` on a shape mismatch or a negative ``filterLen`` / ``peek``, and
+    ``np.linalg.LinAlgError("SVD did not converge")`` on non-finite input, as NumPy does.
+    '''
+    refChannel = np.asarray(refChannel)
+    srvChannel = np.asarray(srvChannel)
+    if refChannel.shape != srvChannel.shape:
+        raise ValueError('Input vectors must have the same length')
+    filterLen, peek = _svd_args(filterLen, peek)
+    rt = np.result_type(np.complex64, srvChannel.dtype)
+    if filterLen + peek == 0:                  # no columns: the reference subtracts nothing
+        out, taps = srvChannel.astype(rt), np.zeros(0, dtype=rt)
+    else:
+        ref = _lib.as_c64(refChannel, "refChannel")
+        srv = _lib.as_c64(srvChannel, "srvChannel")
+        o, t, rank = _ls_svd(ref[None], srv[None], filterLen, peek, device)
+        if rank[0] < 0:
+            raise np.linalg.LinAlgError("SVD did not converge")
+        out, taps = o[0].astype(rt, copy=False), t[0].astype(rt, copy=False)
+    if return_filter:
+        return out, taps
+    return out
+
+
+def ls_filter_svd_frames(ref_frames, srv_frames, filterLen, peek=10, return_filter=False, *, return_rank=False,
+                         device=None):
+    '''``LS_Filter_SVD`` on a batch of independent frames in one library call: row i of the 2-D host arrays
+    ``ref_frames`` / ``srv_frames`` (nframes x n) is one frame.  One CTA decomposes each frame's Gram matrix, so a
+    batch of frames is what fills the GPU.
+
+    Returns ``out`` (nframes x n) and, with ``return_filter=True``, the taps (nframes x (filterLen + peek)), in
+    ``np.result_type(np.complex64, srv_frames.dtype)``; row i equals ``LS_Filter_SVD(ref_frames[i], srv_frames[i],
+    ...)`` bit for bit.  With ``return_rank=True`` the number of kept singular values of every frame comes last; a
+    frame with non-finite input then reports -1 (its row is NaN) instead of raising ``LinAlgError``.
+    '''
+    ref = np.asarray(ref_frames)
+    srv = np.asarray(srv_frames)
+    if ref.ndim != 2:
+        raise ValueError(f"ref_frames must be two-dimensional (nframes x n), got shape {ref.shape}")
+    if ref.shape != srv.shape:
+        raise ValueError('Input vectors must have the same length')
+    filterLen, peek = _svd_args(filterLen, peek)
+    rt = np.result_type(np.complex64, srv.dtype)
+    out, taps, rank = _ls_svd(np.ascontiguousarray(ref, dtype=np.complex64), np.ascontiguousarray(srv, dtype=np.complex64),
+                              filterLen, peek, device)
+    if filterLen + peek == 0:
+        out = srv.astype(rt)
+    if not return_rank and (rank < 0).any():
+        raise np.linalg.LinAlgError("SVD did not converge")
+    res = (out.astype(rt, copy=False),)
+    if return_filter:
+        res += (taps.astype(rt, copy=False),)
+    if return_rank:
+        res += (rank,)
+    return res[0] if len(res) == 1 else res

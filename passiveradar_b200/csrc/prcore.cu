@@ -33,6 +33,7 @@
 #include "track.cuh"
 #include "fftcorr.cuh"
 #include "chanoff.cuh"
+#include "lssvd.cuh"
 
 namespace {
 
@@ -56,11 +57,12 @@ std::atomic<uint64_t> g_launches{0};
 
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
-                K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_COUNT };
+                K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
+                K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
-                                           "chanoff_fft", "chanoff_argmax"};
+                                           "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -137,6 +139,8 @@ struct Ctx {
     DBuf tcplane[9];          // bf16 planes of the tensor-core path: x[3], s0[3], s1[3]
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
         nl_init, nl_taps, gal_k, gal_h;
+    DBuf svd_part, svd_cr, svd_ws, svd_taps, svd_rank;   // LS_Filter_SVD: lag-sum partials, c / rhs, A and Z
+                                                         // of frames that exceed shared memory, float64 taps, ranks
     DBuf trk_map, trk_plan, trk_stats, trk_slots, trk_out, trk_cnt;   // trackers: host maps, summation tree, per-frame
                                                                       // mean / thr / count, candidate slots, results
     int trk_plan_n = -1, trk_nnodes = 0, trk_nlevels = 0;             // map size trk_plan was built for, its shape
@@ -162,7 +166,7 @@ struct Ctx {
         for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
-                        &trk_slots, &trk_out, &trk_cnt})
+                        &trk_slots, &trk_out, &trk_cnt, &svd_part, &svd_cr, &svd_ws, &svd_taps, &svd_rank})
             b->release();
         trk_plan_n = -1;
         if (pin_ready) {
@@ -269,6 +273,7 @@ int set_kernel_attrs(int device) {
     CU(cudaFuncSetAttribute(nlms_block_kernel<2, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<4, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(gal_jpe_kernel<GAL_CTA_T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(lssvd::svd_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_MEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(track_meas_kernel<float, TRK_MODE_MEAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
@@ -1956,6 +1961,67 @@ int chanoff_stage(Ctx* c, AsyncScratch& ws, const void** s, int dt, int64_t n, i
     return PRC_OK;
 }
 
+// ---- LS_Filter_SVD (lssvd.cuh) ----------------------------------------------------------------------------------------
+constexpr size_t SVD_WS_BUDGET = 4ull << 30;     // A and Z of frames whose matrices exceed shared memory, per launch
+
+int ls_svd_check(long long n, int filter_len, int peek) {
+    if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
+    if (filter_len < 0 || peek < 0) return fail(PRC_E_INVALID, "filter_len=%d peek=%d invalid", filter_len, peek);
+    const long long M = (long long)filter_len + peek;
+    if (M < 1) return fail(PRC_E_INVALID, "filter_len + peek = 0: no taps");
+    if (M > lssvd::MAX_M)
+        return fail(PRC_E_INVALID, "%lld taps exceed the SVD filter's maximum of %d", M, lssvd::MAX_M);
+    return PRC_OK;
+}
+
+// bt.nf frames: lag sums -> eigendecomposition and pseudo-inverse per frame -> residual; ranks to rank (device)
+int ls_svd_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len, int peek,
+                  float2* out, float2* taps_out, int* rank) {
+    const int M = filter_len + peek;
+    const lssvd::CorrGeo cg = lssvd::corr_geo(n, M);
+    TRY(c->svd_part.ensure((size_t)bt.nf * 2 * M * cg.nparts * sizeof(double2)));
+    TRY(c->svd_cr.ensure((size_t)bt.nf * 2 * M * sizeof(double2)));
+    TRY(c->svd_taps.ensure((size_t)bt.nf * M * sizeof(double2)));
+    {
+        ProfScope ps(c, K_SVD_CORR);
+        lssvd::CorrParams p{};
+        p.ref = ref; p.srv = srv; p.n = n; p.stride = bt.stride; p.M = M; p.peek = peek;
+        p.span = cg.span; p.nparts = cg.nparts; p.ntiles = cg.ntiles;
+        p.part = c->svd_part.as<double2>();
+        lssvd::launch_corr(p, bt.nf, c->stream);
+        TRY(check_launch("svd_corr_kernel"));
+        lssvd::launch_reduce(p.part, cg.nparts, (long long)bt.nf * 2 * M, c->svd_cr.as<double2>(), c->stream);
+        TRY(check_launch("svd_reduce_kernel"));
+    }
+    {
+        ProfScope ps(c, K_SVD_EIG);
+        const lssvd::EigGeo eg = lssvd::eig_geo(M, SMEM_LIMIT - 2 * lssvd::MAX_M * sizeof(double) - 64);      // s_rot and flags are static
+        const size_t per = (eg.a_smem ? 0 : (size_t)M * M * sizeof(double2)) + (eg.z_smem ? 0 : (size_t)M * M * sizeof(double));
+        const int group = per ? (int)std::max<size_t>(1, std::min<size_t>(bt.nf, SVD_WS_BUDGET / per)) : bt.nf;
+        if (per) TRY(c->svd_ws.ensure((size_t)group * per));
+        for (int f0 = 0; f0 < bt.nf; f0 += group) {
+            lssvd::EigParams p{};
+            p.cr = c->svd_cr.as<double2>() + (size_t)f0 * 2 * M;
+            p.M = M;
+            p.nframes = std::min(group, bt.nf - f0);
+            p.a_smem = eg.a_smem; p.z_smem = eg.z_smem;
+            p.gA = eg.a_smem ? nullptr : c->svd_ws.as<double2>();
+            p.gZ = eg.z_smem ? nullptr : reinterpret_cast<double*>(c->svd_ws.as<char>() + (eg.a_smem ? 0 : (size_t)group * M * M * sizeof(double2)));
+            p.taps = c->svd_taps.as<double2>() + (size_t)f0 * M;
+            p.taps_out = taps_out ? taps_out + (size_t)f0 * M : nullptr;
+            p.rank = rank + f0;
+            lssvd::launch_eig(p, eg, c->stream);
+            TRY(check_launch("svd_eig_kernel"));
+        }
+    }
+    ProfScope ps(c, K_SVD_FIR);
+    lssvd::FirParams p{};
+    p.ref = ref; p.srv = srv; p.out = out; p.n = n; p.stride = bt.stride; p.M = M; p.peek = peek;
+    p.taps = c->svd_taps.as<double2>();
+    lssvd::launch_fir(p, bt.nf, c->stream);
+    return check_launch("svd_fir_kernel");
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2847,6 +2913,56 @@ int prc_xcorr(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2
     TRY(chanoff_device(c, ws, s1, dtype1, n1, s2, dtype2, n2, nullptr, 1, nlag, nlead,
                        cplx ? chanoff::ARG_COMPLEX : chanoff::ARG_REAL, dout, nullptr));
     if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, ob, flags));
+    return finish(c, flags);
+}
+
+int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                          int filter_len, int peek, prc_c64* out, prc_c64* taps_out, int* rank_out,
+                          int mem_kind, int device, void* stream, unsigned flags) {
+    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    TRY(ls_svd_check(n, filter_len, peek));             // before any CUDA call
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    const int M = filter_len + peek;
+    const size_t nb = (size_t)n * sizeof(float2), mb = (size_t)M * sizeof(float2) * nframes;
+    Batch bt;
+    bt.nf = nframes;
+    bt.stride = nframes > 1 ? frame_stride : n;
+    const float2* dref = reinterpret_cast<const float2*>(ref);
+    const float2* dsrv = reinterpret_cast<const float2*>(srv);
+    float2* dout = reinterpret_cast<float2*>(out);
+    float2* dtaps = reinterpret_cast<float2*>(taps_out);
+    int* drank = rank_out;
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->ref.ensure(nb * nframes));
+        TRY(c->srv.ensure(nb * nframes));
+        TRY(c->clean.ensure(nb * nframes));
+        for (int fr = 0; fr < nframes; ++fr) {
+            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
+            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
+        }
+        if (taps_out) { TRY(c->lstaps.ensure(mb)); dtaps = c->lstaps.as<float2>(); }
+        dref = c->ref.as<float2>();
+        dsrv = c->srv.as<float2>();
+        dout = c->clean.as<float2>();
+        bt.stride = n;
+    }
+    if (mem_kind == PRC_MEM_HOST || !rank_out) {
+        TRY(c->svd_rank.ensure((size_t)nframes * sizeof(int)));
+        drank = c->svd_rank.as<int>();
+    }
+    TRY(ls_svd_device(c, dref, dsrv, n, bt, filter_len, peek, dout, dtaps, drank));
+    if (mem_kind == PRC_MEM_HOST) {
+        const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
+        for (int fr = 0; fr < nframes; ++fr)
+            TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
+        if (taps_out) TRY(d2h(c, taps_out, c->lstaps.p, mb, flags));
+        if (rank_out) TRY(d2h(c, rank_out, drank, (size_t)nframes * sizeof(int), flags));
+    }
     return finish(c, flags);
 }
 
