@@ -248,6 +248,47 @@ def ls_filter_multiple_oracle(refChannel, srvChannel, filterLen, sampleRate, dop
     return cleaned
 
 
+def _lin_xcorr_truth(a, b, nlag):
+    """float64 ``xcorr_oracle(a, b, 0, nlag)``: out[k] = sum_{i >= k} a[i] conj(b[i - k]), k = 0 .. nlag."""
+    import scipy.fft as sfft
+    n = a.shape[0]
+    nfft = sfft.next_fast_len(n + nlag + 1)
+    return sfft.ifft(sfft.fft(a, nfft) * np.conj(sfft.fft(b, nfft)))[:nlag + 1]
+
+
+def ls_filter_toeplitz_truth(ref, srv, filter_len, peek=10):
+    """float64 ``LS_Filter_Toeplitz``: the reference rolled by -peek, its linear auto-correlation and its linear
+    cross-correlation with srv over lags 0 .. M-1 (M = filter_len + peek), a dense solve of the Hermitian Toeplitz
+    system, and the linear FIR clutter[i] = sum_k taps[k] shifted[i - k].  Returns (cleaned, taps) in complex128."""
+    import scipy.fft as sfft
+    import scipy.linalg as sla
+    ref = np.asarray(ref, dtype=np.complex128)
+    srv = np.asarray(srv, dtype=np.complex128)
+    if ref.shape != srv.shape:
+        raise ValueError(f"Input vectors must have the same length - got {ref.shape} and {srv.shape}")
+    n = ref.shape[0]
+    m = filter_len + peek
+    shifted = np.roll(ref, -peek)
+    acorr = _lin_xcorr_truth(shifted, shifted, m - 1)
+    xc = _lin_xcorr_truth(srv, shifted, m - 1)
+    taps = np.linalg.solve(sla.toeplitz(acorr, np.conj(acorr)), xc)
+    nfft = sfft.next_fast_len(n + m)
+    clutter = sfft.ifft(sfft.fft(shifted, nfft) * sfft.fft(taps, nfft))[:n]
+    return srv - clutter, taps
+
+
+def ls_filter_multiple_truth(ref, srv, filter_len, sample_rate, doppler_bins=(0,), peek=10):
+    """float64 ``LS_Filter_Multiple``: ``ls_filter_toeplitz_truth`` on the running residual, once per Doppler bin.  The
+    shifted reference of a bin is ``frequency_shift_oracle`` of the complex64 reference, rounded as the reference rounds
+    it (float32 phase ramp); only what follows is float64.  Returns the cleaned channel in complex128."""
+    ref64 = np.asarray(ref).astype(np.complex64)
+    cleaned = np.asarray(srv, dtype=np.complex128)
+    for doppler in doppler_bins:
+        ref_k = ref64 if doppler == 0 else frequency_shift_oracle(ref64, doppler, sample_rate)
+        cleaned, _ = ls_filter_toeplitz_truth(ref_k, cleaned, filter_len, peek)
+    return cleaned
+
+
 def nlms_block_exact(refChannel, srvChannel, filterLen, mu, peek=10, L=32, dtype=np.complex64):
     """The NLMS recurrence of the reference evaluated L samples at a time WITHOUT changing its values
     (the statement ``nlms_block_kernel`` implements; not ``block_NLMS``, whose taps are frozen in a block).

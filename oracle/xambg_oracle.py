@@ -150,15 +150,61 @@ def block_sums_truth(ref, srv, range_bins, freq_bins, window=None, short_filt=Tr
     return P
 
 
-def fast_xambg_truth(ref, srv, range_bins, freq_bins, input_len=None, window=None, short_filt=True):
-    """float64 truth for the whole map, same output convention as ``fast_xambg``."""
+def block_sums_truth_fft(ref, srv, range_bins, freq_bins, window=None, short_filt=True, max_points=1 << 22):
+    """``block_sums_truth`` evaluated with float64 FFTs, so that thousands of lags at millions of samples are affordable
+    on the host.  Block j holds the nt product indices i = hi - nt + 1 .. hi (hi = j*D + c), tap taps[hi - i], and
+    P[j, R - d] = sum_i taps[hi - i] x[i] conj(srv[(i + d) mod N]) for d = 0 .. R: a linear correlation of the
+    weighted block (zero outside [0, N)) with the nt + R surveillance samples from its first index on, one transform of
+    at least nt + R points per block (no circular alias reaches lags 0 .. R).  Blocks go ``max_points`` at a time."""
+    import scipy.fft as sfft
+    ref = np.asarray(ref, dtype=np.complex128)
+    srv = np.asarray(srv, dtype=np.complex128)
+    n = ref.shape[0]
+    d = decimation_factor(n, freq_bins)
+    if d == 1:
+        taps, c = np.ones(1), 0
+    else:
+        taps = np.asarray(decimator_taps(d, short_filt), dtype=np.float64)
+        c = decimator_alignment(taps.shape[0], d)
+    x = ref if window is None else ref * np.asarray(window, dtype=np.float64)
+    nt = taps.shape[0]
+    R = range_bins
+    nfft = sfft.next_fast_len(nt + R)
+    t = np.arange(nt)
+    ts = np.arange(nt + R)
+    P = np.empty((freq_bins, R + 1), dtype=np.complex128)
+    step = max(1, max_points // nfft)
+    for j0 in range(0, freq_bins, step):
+        js = np.arange(j0, min(freq_bins, j0 + step))
+        lo = js[:, None] * d + c - (nt - 1)
+        idx = lo + t[None, :]
+        inside = (idx >= 0) & (idx < n)
+        xb = np.where(inside, x[np.clip(idx, 0, n - 1)], 0) * taps[::-1][None, :]
+        sb = srv[(lo + ts[None, :]) % n]
+        corr = np.conj(sfft.ifft(np.conj(sfft.fft(xb, nfft, axis=1)) * sfft.fft(sb, nfft, axis=1), axis=1))
+        P[js] = corr[:, R::-1]
+    return P
+
+
+def fast_xambg_truth(ref, srv, range_bins, freq_bins, input_len=None, window=None, short_filt=True, fast=False):
+    """float64 truth for the whole map, same output convention as ``fast_xambg``; ``fast``: block sums by
+    ``block_sums_truth_fft`` rather than the definition's loop."""
     ref = _pad_to(np.asarray(ref), input_len)
     srv = _pad_to(np.asarray(srv), input_len)
     if isinstance(window, (tuple, str)):
         window = signal.get_window(window, input_len)
-    P = block_sums_truth(ref, srv, range_bins, freq_bins, window, short_filt)
+    P = (block_sums_truth_fft if fast else block_sums_truth)(ref, srv, range_bins, freq_bins, window, short_filt)
     X = np.fft.fftshift(np.fft.fft(P, axis=0), axes=0)
     return X[:, :, None]
+
+
+def frame_truth(ref, srv, filter_len, reg, peek, range_bins, freq_bins, window=None):
+    """float64 frame: ``ls_filter_truth`` (circular LS filter), then the map of the float64 cleaned channel.  Returns
+    (map [F, R+1], taps, cleaned) in complex128."""
+    from .clutter_oracle import ls_filter_truth
+    cleaned, taps = ls_filter_truth(ref, srv, filter_len, reg, peek)
+    amb = fast_xambg_truth(np.asarray(ref, dtype=np.complex128), cleaned, range_bins, freq_bins, None, window, fast=True)
+    return amb[:, :, 0], taps, cleaned
 
 
 def rel_inf(a, b):

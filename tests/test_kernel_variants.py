@@ -510,6 +510,7 @@ def test_caf_wave_grid_is_bit_identical(n, F, R):
 PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/test_kernel_variants.py::"
 FE, GAL, TRK = "tests/test_gpu_frontend.py::", "tests/test_gal_jpe.py::", "tests/test_tracking.py::"
 RS = "tests/test_rows_sweep.py::"
+PS = "tests/test_path_sweep.py::"
 VARIANT_TEST = KV + "test_variant_matches_truth_and_reference"
 COVERAGE = {
     "launch_lagstream: lagstream_kernel<10, 10>": [(PAR + "test_ls_matches_live_oracle", "direct", "LS, n <= 20000"),
@@ -521,21 +522,29 @@ COVERAGE = {
         (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
     "ls_fft_corr: fftc::lscorr_fft_kernel<R3>": [
         (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8 (M <= 1024)"),
-        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; ls_fft_plan never picks R3 = 4")],
-    "levinson_launch: levinson_kernel<1>": [(PAR + "test_ls_matches_live_oracle", "fft", "M <= 1024, batched solve")],
-    "levinson_launch: levinson_kernel<4>": [(PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "M = 1110")],
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; ls_fft_plan never picks R3 = 4"),
+        (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1 .. 2048 at n = 2L and a one-sample last segment"),
+        (PS + "test_frames_batch_sizes_hold_every_row_to_its_truth", "default", "one CTA per frame (nf > slots / 2)")],
+    "levinson_launch: levinson_kernel<1>": [(PAR + "test_ls_matches_live_oracle", "fft", "M <= 1024, batched solve"),
+                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1, 2, 1023, 1024")],
+    "levinson_launch: levinson_kernel<4>": [(PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "M = 1110"),
+                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1025 .. 2048 against the truth")],
     "taps_spectrum: fftc::taps_spectrum_kernel<R3>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8 (CAF transform)"),
         (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8 (FIR transform)"),
         (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
     "fir_fft: fftc::fir_fft_kernel<R3>": [
         (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8"),
-        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; the LS transform is never R3 = 4")],
+        (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16; the LS transform is never R3 = 4"),
+        (PS + "test_toeplitz_and_multiple_at_the_planner_edges", "default", "linear mode, M = 1 .. 2048")],
     "caf_fft: fftc::caf_fft_kernel<R3, true>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16"),
-        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
+        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid"),
+        (PS + "test_fused_frame_at_the_planner_edges", "default",
+         "R3 = 16 against the frame truth (R + M - 1 = 3072); filterLen = 0: the staging without reuse; peek = 0")],
     "caf_fft: fftc::caf_fft_kernel<R3, false>": [
+        (PS + "test_xambg_at_the_planner_edges", "fft", "R = 3L/4 at L = 1024, 2048, 4096; D = 32; F = 1; f32 window"),
         (PAR + "test_xambg_matches_live_oracle", "fft", "R3 = 4"),
         (FFT + "test_xambg_large_shapes_sampled_columns", "fft", "R3 = 8 (F = 64, D >= 16384)"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16 (R = 1200)"),
