@@ -34,6 +34,7 @@
 #include "fftcorr.cuh"
 #include "chanoff.cuh"
 #include "lssvd.cuh"
+#include "framepass.cuh"
 
 namespace {
 
@@ -58,11 +59,12 @@ std::atomic<uint64_t> g_launches{0};
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
-                K_COUNT };
+                K_CAF_COMBINE, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
-                                           "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir"};
+                                           "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
+                                           "caf_combine"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -150,8 +152,9 @@ struct Ctx {
     cudaEvent_t pin_ev[2] = {nullptr, nullptr};
     bool pin_ready = false;
     DBuf fft_tw[3], wp_fir, wp_caf, fftP;     // FFT-domain path: twiddle tables (L = 1024 / 2048 / 4096), taps spectra, CAF block sums
+    DBuf fpacc;                               // one-pass frame: AccP / AccQ spectra per Doppler block [nf][F][2][L]
     bool fft_tw_ready[3] = {false, false, false};
-    int fft_ctas[4][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
+    int fft_ctas[6][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
     std::vector<ProfRec> recs;
     void release() {
         cudaSetDevice(device);
@@ -162,7 +165,7 @@ struct Ctx {
         clean2.release();
         for (DBuf& b : fft_tw) b.release();
         for (bool& r : fft_tw_ready) r = false;
-        for (DBuf* b : {&wp_fir, &wp_caf, &fftP}) b->release();
+        for (DBuf* b : {&wp_fir, &wp_caf, &fftP, &fpacc}) b->release();
         for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
@@ -196,6 +199,7 @@ int g_packed = 1;          // paired-FMA kernels (PRC_PACKED=0 selects the scala
 std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: wgmma / FP32 direct form
 std::atomic<int> g_fft_min_n{8192};   // ... for channels of at least this many samples (PRC_FFT_MIN_N)
 std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks instead of one CTA per block
+std::atomic<int> g_frame_onepass{1};  // FFT-domain frame: LS lag sums and CAF block spectra in one pass (framepass.cuh); 0: two passes
 std::once_flag g_env_once;
 
 // Workspaces of a thread that called with stream == NULL.  They are released when the thread exits (dask's thread pool
@@ -290,6 +294,7 @@ int set_kernel_attrs(int device) {
     PRC_FFT_ATTRS(8)
     PRC_FFT_ATTRS(16)
 #undef PRC_FFT_ATTRS
+    CU(fftc::framepass_set_attrs(lim));
     g_attrs_set[device].store(true);
     return PRC_OK;
 }
@@ -579,7 +584,7 @@ int fft_twiddles(Ctx* c, int r3, const float2** tw) {
 }
 
 // FFT-domain kernels whose grids are sized to one wave of CTAs for the whole batch
-enum FftKern { FK_LS = 0, FK_FIR = 1, FK_CAF = 2, FK_CAF_FUSED = 3 };
+enum FftKern { FK_LS = 0, FK_FIR = 1, FK_CAF = 2, FK_CAF_FUSED = 3, FK_FRAME = 4, FK_COMBINE = 5 };   // FRAME, COMBINE: R3 = 8 only
 
 // CTAs of one instantiation an SM holds at once, at the block size and dynamic shared memory it is launched with:
 // registers (and the launch bounds that cap them) and shared memory decide it, so the grids follow the build rather
@@ -599,9 +604,11 @@ int fft_ctas_per_sm(Ctx* c, FftKern k, int r3) {
     } else if (k == FK_CAF) {
         PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, false>, 16 * R3,
                                                                            fftc::caf_smem_float2<R3>() * sizeof(float2))));
-    } else {
+    } else if (k == FK_CAF_FUSED) {
         PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, true>, 16 * R3,
                                                                            fftc::caf_smem_float2<R3>() * sizeof(float2))));
+    } else {
+        v = k == FK_FRAME ? fftc::frame_pass_ctas_per_sm() : fftc::caf_combine_ctas_per_sm();
     }
     if (e != cudaSuccess || v < 1) {
         cudaGetLastError();
@@ -654,15 +661,15 @@ int ls_fft_corr(Ctx* c, const LsFftPlan& pl, const float2* ref, const float2* sr
     return check_launch("lscorr_fft_kernel");
 }
 
-// (T + reg I) w = rhs for nf frames: taps -> c->lstaps [nf][M], status -> c->status [nf]
-int levinson_launch(Ctx* c, int nchunk, int HT, int M, double reg, int nf) {
-    TRY(c->lstaps.ensure((size_t)nf * M * sizeof(float2)));
-    TRY(c->status.ensure((size_t)nf * sizeof(int)));
+// (T + reg I) w = rhs for nf frames: taps -> c->lstaps [f0 + nf][M], status -> c->status [f0 + nf], from frame f0 on
+int levinson_launch(Ctx* c, int nchunk, int HT, int M, double reg, int nf, int f0 = 0) {
+    TRY(c->lstaps.ensure((size_t)(f0 + nf) * M * sizeof(float2)));
+    TRY(c->status.ensure((size_t)(f0 + nf) * sizeof(int)));
     LevinsonParams lp{};
     lp.partial = c->partial.as<float2>();
     lp.nchunk = nchunk; lp.HT = HT; lp.M = M; lp.reg = reg;
-    lp.taps = c->lstaps.as<float2>();
-    lp.status = c->status.as<int>();
+    lp.taps = c->lstaps.as<float2>() + (size_t)f0 * M;
+    lp.status = c->status.as<int>() + f0;
     {
         ProfScope ps(c, K_LEVINSON);
         // one thread per unknown (a CTA of 1024 threads would own a whole SM's registers and could not share it
@@ -674,13 +681,13 @@ int levinson_launch(Ctx* c, int nchunk, int HT, int M, double reg, int nf) {
     return check_launch("levinson_kernel");
 }
 
-// W' of c->lstaps for transform length 256 r3 -> wp [nf][L]
-int taps_spectrum(Ctx* c, int r3, int M, int nf, DBuf* wp) {
+// W' of c->lstaps (from frame f0 on) for transform length 256 r3 -> wp [nf][L]
+int taps_spectrum(Ctx* c, int r3, int M, int nf, DBuf* wp, int f0 = 0) {
     const float2* tw;
     TRY(fft_twiddles(c, r3, &tw));
     TRY(wp->ensure((size_t)nf * 256 * r3 * sizeof(float2)));
     fftc::TapSpecParams p{};
-    p.taps = c->lstaps.as<float2>(); p.M = M; p.wp = wp->as<float2>(); p.tw = tw;
+    p.taps = c->lstaps.as<float2>() + (size_t)f0 * M; p.M = M; p.wp = wp->as<float2>(); p.tw = tw;
     {
         ProfScope ps(c, K_MISC);
         PRC_R3_SWITCH(r3, (fftc::taps_spectrum_kernel<R3><<<nf, 16 * R3, fft_smem(R3), c->stream>>>(p)));
@@ -688,12 +695,12 @@ int taps_spectrum(Ctx* c, int r3, int M, int nf, DBuf* wp) {
     return check_launch("taps_spectrum_kernel");
 }
 
-// out = srv - FIR(ref, c->lstaps) by overlap-save (circular, or zero-extended when linear)
+// out = srv - FIR(ref, c->lstaps from frame f0 on) by overlap-save (circular, or zero-extended when linear)
 int fir_fft(Ctx* c, int r3, const float2* ref, const float2* srv, float2* out, long long n, Batch bt, int M, int peek,
-            bool linear) {
+            bool linear, int f0 = 0) {
     const float2* tw;
     TRY(fft_twiddles(c, r3, &tw));
-    TRY(taps_spectrum(c, r3, M, bt.nf, &c->wp_fir));
+    TRY(taps_spectrum(c, r3, M, bt.nf, &c->wp_fir, f0));
     const int L = 256 * r3;
     fftc::FirFftParams p{};
     p.ref = ref; p.srv = srv; p.out = out; p.frame_stride = bt.stride;
@@ -776,11 +783,12 @@ int decimator_offset(long long ntaps, long long D) {   // resample_poly alignmen
 }
 
 // bt.nf > 1 (a batch of frames) and fuse_wp != nullptr (clutter filter applied inside the CAF kernel, taps spectrum
-// [nf][L] for the transform length of caf_fft_plan(..., fuse_M)) exist on the FFT-domain path only
+// [nf][L] for the transform length of caf_fft_plan(..., fuse_M)) exist on the FFT-domain path only; p_ready: the block
+// sums are already in c->fftP (one-pass frame), only the Doppler stage runs
 int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int R, int F,
                  const float* win32, const float* dtaps32, long long ndtaps, float2* out,
                  bool refw_ready = false, bool caf_planes_ready = false, Batch bt = Batch{},
-                 const float2* fuse_wp = nullptr, int fuse_M = 0, int fuse_peek = 0) {
+                 const float2* fuse_wp = nullptr, int fuse_M = 0, int fuse_peek = 0, bool p_ready = false) {
     if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
     if (F < 1 || R < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", F, R);
     const long long D = n / F;
@@ -806,10 +814,15 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
     const float* bnd_w_all = nullptr;               // ... window to apply to bnd_x on the fly (bnd_x unweighted)
     const float2* dop_src = nullptr;                // Doppler-stage input when it is not c->partial
     const CafFftPlan fp = caf_fft_plan(n, R, F, ntaps, D, taps == nullptr && ntaps == D + 1, fuse_wp ? fuse_M : 0);
-    if ((bt.nf > 1 || fuse_wp) && !fp.on)
+    if ((bt.nf > 1 || fuse_wp) && !fp.on && !p_ready)
         return fail(PRC_E_INVALID, "batched / fused CAF needs the FFT-domain path (n=%lld, F=%d, R=%d not eligible)", n, F, R);
-    const CafTc ct = (!fp.on && ntaps == D + 1 && c0 == D / 2) ? caf_tc_plan(c, n, R, F, taps != nullptr) : CafTc{};
-    if (fp.on) {
+    const CafTc ct = (!p_ready && !fp.on && ntaps == D + 1 && c0 == D / 2) ? caf_tc_plan(c, n, R, F, taps != nullptr) : CafTc{};
+    if (p_ready) {
+        // ---- block sums already in c->fftP ([nf][F][HT], the one-pass frame's caf_combine_kernel): Doppler stage only
+        g.nchunk = 1;
+        g.HT = (R + 2) & ~1;
+        dop_src = c->fftP.as<float2>();
+    } else if (fp.on) {
         // ---- FFT-domain block correlations (fftcorr.cuh): one CTA per Doppler block, P[j][d] straight from the channels
         TRY(caf_fft(c, fp, ref, srv, n, bt, R, F, win32, D, c0, ntaps, fuse_wp, fuse_M, fuse_peek));
         g.nchunk = 1;
@@ -1610,6 +1623,113 @@ int check_ls_status(Ctx* c, unsigned flags, int nf = 1) {
     return PRC_OK;
 }
 
+// ---- one-pass FFT-domain frame (framepass.cuh): LS lag sums and the CAF's per-block spectra AccP, AccQ from one set
+// of window transforms, then the Toeplitz solve, W', and AccP - AccQ conj(W') per block
+struct OnePassPlan {
+    bool on = false;
+    int Bmax = 0, ntail = 0, Bt = 0, c0 = 0;
+    long long D = 0, tail_lo = 0;
+};
+
+// AccP / AccQ spectra of one chunk of frames: 2 L complex64 per Doppler block and frame (8 MiB per frame at 256 blocks
+// of L = 2048); larger batches run in chunks of frames that fit
+constexpr size_t FP_ACC_CAP = 256u << 20;
+
+// Taken when both FFT-domain plans are on, the clutter filter has at least one tap before peek (so Yr' starts at or
+// before Ys'), the segment limit of both the LS lags and the CAF lags at L = 2048 is at least L / 4, and the transform
+// count x L log L is below that of the two passes (lscorr_fft_kernel + caf_fft_kernel<FUSED>).  Otherwise off, and the
+// frame runs exactly as before.
+OnePassPlan onepass_plan(const LsFftPlan& lf, const CafFftPlan& cf, long long n, int filter_len, int peek, int R, int F,
+                         long long D) {
+    OnePassPlan op;
+    if (!g_frame_onepass.load() || !lf.on || !cf.on || filter_len < 1) return op;
+    const int M = filter_len + peek;
+    const long long L = 256 * fftc::FP_R3;
+    const long long bls = L - 2ll * M + 2;                       // lags M-1 .. 2M-2 of X_ls conj(Yr')
+    const long long bmax = std::min(bls, L - M - R - peek + 1);  // CAF lags peek .. R + peek of the cleaned window
+    if (bmax < L / 4 || n < L) return op;
+    const long long ntaps = D + 1;
+    const int c0 = decimator_offset(ntaps, D);
+    if (c0 - (ntaps - 1) > 0) return op;                         // samples before the first block: not a layout we run
+    op.tail_lo = std::min((long long)(F - 1) * D + c0 + 1, n);
+    const long long tail = n - op.tail_lo;
+    op.ntail = (int)((tail + bls - 1) / bls);
+    op.Bt = op.ntail ? (int)((tail + op.ntail - 1) / op.ntail) : 0;
+    double one = 3.0 * op.ntail, two_caf = 0.0;
+    for (int j = 0; j < F; ++j) {
+        const long long lo = std::max((long long)j * D + c0 - (ntaps - 1), 0ll), hi = std::min((long long)j * D + c0 + 1, n);
+        const long long len = std::max(hi - lo, 0ll);
+        one += 4.0 * ((len + bmax - 1) / bmax) + 1.0;            // + the combine's transform
+        two_caf += 3.0 * ((len + cf.Bmax - 1) / cf.Bmax) + 1.0;
+    }
+    const double one_cost = one * L * ilog2((int)L);
+    const double two_cost = 3.0 * lf.nseg * (256.0 * lf.r3) * ilog2(256 * lf.r3) + two_caf * (256.0 * cf.r3) * ilog2(256 * cf.r3);
+    if (one_cost >= two_cost) return op;
+    op.on = true;
+    op.Bmax = (int)bmax;
+    op.c0 = c0;
+    op.D = D;
+    return op;
+}
+
+int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len,
+                  int peek, double reg, int R, int F, const float* win32, float2* maps, float2* taps_out, float2* cleaned_out) {
+    if (n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
+    constexpr int R3 = fftc::FP_R3;
+    constexpr int L = 256 * R3;
+    const int M = filter_len + peek;
+    const float2* tw;
+    TRY(fft_twiddles(c, R3, &tw));
+    const size_t per_frame = (size_t)F * 2 * L * sizeof(float2);
+    const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)bt.nf, FP_ACC_CAP / per_frame));
+    const int HT = (M + 1) & ~1, HTc = (R + 2) & ~1;
+    TRY(c->fpacc.ensure(per_frame * chunk));
+    TRY(c->lstaps.ensure((size_t)bt.nf * M * sizeof(float2)));
+    TRY(c->status.ensure((size_t)bt.nf * sizeof(int)));
+    TRY(c->fftP.ensure((size_t)chunk * F * HTc * sizeof(float2)));
+    const int units = F + op.ntail;
+    for (int f0 = 0; f0 < bt.nf; f0 += chunk) {
+        const int nf = std::min(chunk, bt.nf - f0);
+        const Batch b{nf, bt.stride};
+        const float2* r = ref + (size_t)f0 * bt.stride;
+        const float2* s = srv + (size_t)f0 * bt.stride;
+        // one wave of CTAs (two per SM), each walking a run of Doppler blocks (and tail segments) of its frame
+        const long long slots = (long long)fft_ctas_per_sm(c, FK_FRAME, R3) * c->nsm;
+        const int ncta = (int)std::max<long long>(1, std::min<long long>(units, slots / nf));
+        TRY(c->partial.ensure((size_t)nf * 2 * ncta * HT * sizeof(float2)));
+        fftc::FramePassParams p{};
+        p.ref = r; p.srv = s; p.frame_stride = bt.stride; p.win = win32;
+        p.n = (int)n; p.M = M; p.peek = peek; p.F = F;
+        p.D = op.D; p.c0 = op.c0; p.ntaps = (int)(op.D + 1); p.Bmax = op.Bmax;
+        p.tail_lo = (int)op.tail_lo; p.ntail = op.ntail; p.Bt = op.Bt;
+        p.acc = c->fpacc.as<float2>(); p.partial = c->partial.as<float2>(); p.HT = HT; p.tw = tw;
+        {
+            ProfScope ps(c, K_LAGCORR_CAF);
+            fftc::launch_frame_pass(p, ncta, nf, c->stream);
+        }
+        TRY(check_launch("frame_pass_kernel"));
+        TRY(levinson_launch(c, ncta, HT, M, reg, nf, f0));
+        TRY(taps_spectrum(c, R3, M, nf, &c->wp_caf, f0));
+        if (cleaned_out) TRY(fir_fft(c, R3, r, s, cleaned_out + (size_t)f0 * bt.stride, n, b, M, peek, false, f0));
+        fftc::CafCombineParams q{};
+        q.acc = c->fpacc.as<float2>(); q.wp = c->wp_caf.as<float2>();
+        q.F = F; q.R = R; q.peek = peek;
+        q.P = c->fftP.as<float2>(); q.HT = HTc; q.tw = tw;
+        const long long cslots = (long long)fft_ctas_per_sm(c, FK_COMBINE, R3) * c->nsm;
+        const int gc = (int)std::max<long long>(1, std::min<long long>(F, cslots / nf));
+        {
+            ProfScope ps(c, K_CAF_COMBINE);
+            fftc::launch_caf_combine(q, gc, nf, c->stream);
+        }
+        TRY(check_launch("caf_combine_kernel"));
+        TRY(xambg_device(c, r, s, n, R, F, win32, nullptr, 0, maps + (size_t)f0 * F * (R + 1), false, false, b, nullptr, 0, 0,
+                         true));
+    }
+    if (taps_out)
+        CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)bt.nf * M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
+    return PRC_OK;
+}
+
 // one frame (or, on the FFT-domain path, a batch of frames) of  LS_Filter -> fast_xambg  on device pointers
 int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len, int peek, double reg,
                  int R, int F, const float* win32, float2* maps, float2* taps_out, float2* cleaned_out) {
@@ -1617,6 +1737,9 @@ int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batc
     const long long D = n / F;
     const LsFftPlan lf = (M >= 1 && M <= 2048) ? ls_fft_plan(c, n, M, bt.nf) : LsFftPlan{};
     const CafFftPlan cf = (D >= 2) ? caf_fft_plan(n, R, F, D + 1, D, true, M) : CafFftPlan{};
+    const OnePassPlan op = onepass_plan(lf, cf, n, filter_len, peek, R, F, D);
+    if (op.on)
+        return frame_onepass(c, op, ref, srv, n, bt, filter_len, peek, reg, R, F, win32, maps, taps_out, cleaned_out);
     if (lf.on && cf.on) {
         // FFT-domain frame: lag sums -> Toeplitz solve -> taps spectrum -> CAF with the clutter filter applied to the
         // surveillance spectrum inside the kernel (the cleaned channel exists only if the caller asks for it)
@@ -1796,6 +1919,7 @@ int fft_ctas_option(const std::string& k) {
     if (k == "fft_ctas_ls") return FK_LS;
     if (k == "fft_ctas_fir") return FK_FIR;
     if (k == "fft_ctas_caf") return FK_CAF_FUSED;
+    if (k == "fft_ctas_frame") return FK_FRAME;
     return -1;
 }
 
@@ -2489,6 +2613,7 @@ int prc_set_option(const char* name, int value) {
     if (k == "fft") g_fft.store(value);
     else if (k == "fft_min_n") g_fft_min_n.store(value);
     else if (k == "caf_wave") g_caf_wave.store(value);
+    else if (k == "frame_onepass") g_frame_onepass.store(value);
     else if (env_switch(k) || k == "tma_active")
         return fail(PRC_E_INVALID, "option '%s' is read-only (set from the environment when the library starts)", name);
     else if (fft_ctas_option(k) >= 0)
@@ -2504,6 +2629,7 @@ int prc_get_option(const char* name, int* value) {
     if (k == "fft") *value = g_fft.load();
     else if (k == "fft_min_n") *value = g_fft_min_n.load();
     else if (k == "caf_wave") *value = g_caf_wave.load();
+    else if (k == "frame_onepass") *value = g_frame_onepass.load();
     else if (const int* s = env_switch(k)) *value = *s;
     else if (k == "tma_active") *value = use_tma() ? 1 : 0;
     else if (fft_ctas_option(k) >= 0) {

@@ -8,8 +8,8 @@ tree (B) with the flags of passiveradar_b200/build.py into the git-ignored ``bui
 alternates ``bench.py --no-cpu-baseline`` between the two (each child loads its build through PRC_LIBRARY; the Python
 side is the working tree's for both), so a drift of clocks or temperature over the session hits both builds alike.  The
 first run of each build also writes its ``--dump-outputs`` maps, and the two are compared bit for bit.  Per run it keeps
-the headline ``value``, the single-frame ``latency_us``, the ``e2e`` rate, the per-frame times of ``lagcorr_ls`` and
-``lagcorr_caf``, the SM clocks bench.py sampled, and the card name and power limit; the summary has the median and
+the headline ``value``, the single-frame ``latency_us``, the ``e2e`` rate, the per-frame times of the kernels in
+``KERNELS`` (``lagcorr_ls`` is empty when the one-pass frame runs: ``lagcorr_caf`` is then ``frame_pass_kernel``), the SM clocks bench.py sampled, and the card name and power limit; the summary has the median and
 range per build.  On a power-capped card compare the sampled SM clocks too: a kernel that keeps more warps busy draws
 more power, and the cap then lowers the clock of everything running beside it.
 """
@@ -26,7 +26,7 @@ import tarfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 AB = os.path.join(ROOT, "build", "ab")
-KERNELS = ("lagcorr_ls", "lagcorr_caf")
+KERNELS = ("lagcorr_ls", "lagcorr_caf", "caf_combine", "levinson", "doppler_fft")
 
 
 def compile_lib(src_root: str, out_dir: str) -> str:

@@ -111,10 +111,105 @@ def model_caf(ref, srv, win, R, F, L, w=None, peek=0):
     return P
 
 
-def check(name, a, b, den=None):
+def onepass_limits(L, M, R, peek):
+    """segment limits of the one-pass frame (framepass.cuh): LS-only segments (lags M-1 .. 2M-2 of X_ls conj(Yr')) and
+    block segments (also the CAF lags peek .. R + peek of the cleaned window, whose W' wrap starts past L - M)"""
+    bls = L - 2 * M + 2
+    return bls, min(bls, L - M - R - peek + 1)
+
+
+def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
+    """framepass.cuh in numpy: per Doppler-block segment Ys' (srv from i0 - peek), Yr' (ref from i0 - (M-1)), X_ls and
+    X_caf; LS sums from X_ls, AccP / AccQ per block from X_caf, then AccP - AccQ conj(W') and lags peek .. R + peek.
+    The sample two blocks share goes to the first block's X_ls only; samples after the last block are LS-only
+    segments.  Returns (c, x, P)."""
+    n, M = len(ref), len(w)
+    D = n // F
+    ntaps = D + 1
+    half = (ntaps - 1) // 2
+    pre_pad = D - half % D
+    c0 = ((half + pre_pad) // D) * D - pre_pad
+    assert c0 - (ntaps - 1) <= 0, "no samples before the first block"
+    bls, bmax = limits or onepass_limits(L, M, R, peek)
+    assert bmax >= 1
+    Wp = taps_spectrum(w, L)
+    xw = ref * (win if win is not None else 1.0)
+
+    def spec(sig, base):
+        return np.fft.fft(sig[(base + np.arange(L)) % n])
+
+    def seg(sig, i0, ln, lo_off=0):
+        x = np.zeros(L, complex)
+        x[lo_off:ln] = sig[i0 + lo_off:i0 + ln]
+        return np.fft.fft(x)
+
+    accC = np.zeros(L, complex)
+    accX = np.zeros(L, complex)
+    P = np.zeros((F, R + 1), complex)
+    covered = np.zeros(n, int)
+    for j in range(F):
+        lo = max(j * D + c0 - (ntaps - 1), 0)
+        hi = min(j * D + c0 + 1, n)
+        ls_end = min(hi, max((j + 1) * D + c0 - (ntaps - 1), 0)) if j + 1 < F else hi
+        nseg = -(-(hi - lo) // bmax)
+        Bs = -(-(hi - lo) // nseg)
+        accP = np.zeros(L, complex)
+        accQ = np.zeros(L, complex)
+        for q in range(nseg):
+            i0 = lo + q * Bs
+            ln = min(Bs, hi - i0)
+            lx = max(0, min(ln, ls_end - i0))
+            covered[i0:i0 + lx] += 1
+            Ys = spec(srv, i0 - peek)
+            Yr = spec(ref, i0 - (M - 1))
+            Xls = seg(ref, i0, lx)
+            Xcaf = seg(xw, i0, ln)
+            accC += Xls * np.conj(Yr)
+            accX += Xls * np.conj(Ys)
+            accQ += Xcaf * np.conj(Yr)
+            accP += Xcaf * np.conj(Ys)
+        P[j] = np.fft.fft(accP - accQ * np.conj(Wp))[peek:peek + R + 1] / L
+    tail_lo = min((F - 1) * D + c0 + 1, n)
+    if n > tail_lo:
+        ntail = -(-(n - tail_lo) // bls)
+        Bt = -(-(n - tail_lo) // ntail)
+        for k in range(ntail):
+            i0 = tail_lo + k * Bt
+            ln = min(Bt, n - i0)
+            covered[i0:i0 + ln] += 1
+            Xls = seg(ref, i0, ln)
+            accC += Xls * np.conj(spec(ref, i0 - (M - 1)))
+            accX += Xls * np.conj(spec(srv, i0 - peek))
+    assert (covered == 1).all(), "every sample in exactly one X_ls"
+    c = np.fft.fft(accC)[M - 1:2 * M - 1] / L
+    x = np.fft.fft(accX)[:M] / L
+    return c, x, P
+
+
+def onepass_truth(ref, srv, win, w, R, F, peek):
+    """float64 direct sums of what the one-pass frame computes: LS lag sums and the CAF block sums of the cleaned channel"""
+    n, M = len(ref), len(w)
+    c = direct_lags(ref, ref, range(M), n)
+    x = direct_lags(ref, srv, range(-peek, M - peek), n)
+    s_eff = srv - sum(w[k] * np.roll(ref, k - peek) for k in range(M))
+    xw = ref * (win if win is not None else 1.0)
+    D = n // F
+    ntaps = D + 1
+    half = (ntaps - 1) // 2
+    pre_pad = D - half % D
+    c0 = ((half + pre_pad) // D) * D - pre_pad
+    P = np.zeros((F, R + 1), complex)
+    for d in range(R + 1):
+        prod = xw * np.conj(np.roll(s_eff, -d))
+        for j in range(F):
+            P[j, d] = prod[max(j * D + c0 - (ntaps - 1), 0):min(j * D + c0 + 1, n)].sum()
+    return c, x, P
+
+
+def check(name, a, b, den=None, tol=1e-9):
     e = np.abs(a - b).max() / (den if den else np.abs(b).max())
     print(f"{name:56s} {e:.2e}")
-    assert e < 1e-9, name
+    assert e < tol, name
 
 
 for n, M, peek, L in [(8192, 110, 10, 2048), (20000, 310, 10, 2048), (5000, 64, 0, 1024), (12345, 300, 7, 2048)]:
@@ -160,4 +255,32 @@ for n, F, R, M, peek, L in [(16384, 8, 40, 50, 10, 2048), (20000, 16, 100, 110, 
                 want[j] += xw[i] * np.conj(s_eff[(i + np.arange(R + 1)) % n])
     got = model_caf(ref, srv, win, R, F, L, w, peek)
     check(f"caf n={n} F={F} R={R} M={M} L={L}", got, want)
+# the one-pass frame: the headline shape (c2) and the planner's edges -- M = 1, 2, 1023, 1024 with peek 0 and M - 1, D = 32,
+# F = 1, n not a multiple of F, R + M near L (the CAF limit below the LS one), no window and a float window
+ONEPASS = [
+    # n, F, R, M, peek, L, window
+    (2 ** 20, 256, 300, 310, 10, 2048, True),
+    (20000, 16, 100, 1, 0, 2048, True),
+    (20000, 16, 100, 2, 0, 2048, False),
+    (20000, 16, 100, 2, 1, 2048, True),
+    (30000, 8, 200, 1023, 0, 4096, True),
+    (30000, 8, 200, 1024, 1023, 4096, False),
+    (32 * 128 + 17, 128, 40, 50, 10, 1024, True),
+    (10000, 1, 100, 60, 10, 1024, True),
+    (20011, 7, 60, 40, 39, 1024, True),
+    (12000, 10, 600, 200, 5, 1024, False),
+]
+for n, F, R, M, peek, L, use_win in ONEPASS:
+    ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+    srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+    win = np.kaiser(n, 5.0) if use_win else None
+    w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M
+    tc, tx, tP = onepass_truth(ref, srv, win, w, R, F, peek)
+    c, x, P = model_onepass(ref, srv, win, w, R, F, peek, L)
+    tag = f"onepass n={n} F={F} R={R} M={M} peek={peek} L={L}"
+    check(tag + " c", c, tc, tol=1e-12)
+    check(tag + " x", x, tx, tol=1e-12)
+    check(tag + " P", P, tP, tol=1e-12)
+# the headline shape: Bmax = 1429, three segments per block, a 2047-sample LS-only tail
+assert onepass_limits(2048, 310, 300, 10) == (1430, 1429)
 print("model OK")
