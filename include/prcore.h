@@ -236,7 +236,6 @@ int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int
  * Read-only (prc_get_option only; prc_set_option returns PRC_E_INVALID): the environment switches of INTEGRATION.md
  * section 6, latched once per process, so a caller can check which kernel variants are in force:
  *   "tma" (PRC_TMA), "tma_l2" (PRC_TMA_L2), "tc" (PRC_TC), "tc_caf" (PRC_TC_CAF), "tc_fir" (PRC_TC_FIR),
- *   "stream" (PRC_STREAM), "packed" (PRC_PACKED), "tile" (PRC_TILE, clamped to 0..2), "nlms_block" (PRC_NLMS_BLOCK),
  *   "tune_nchunk" (PRC_TUNE_NCHUNK, -1 = automatic), "tune_g" (PRC_TUNE_G, -1 = automatic);
  *   "tma_active"  1 when toepcorr_kernel uses TMA producers: "tma" is 1 and the driver has cuTensorMapEncodeTiled
  *                 (0: the cp.async loader warps)

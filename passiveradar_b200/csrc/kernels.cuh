@@ -11,12 +11,12 @@
 //   fir_apply_kernel out = srv - circular FIR(ref, w)              (clutter_removal.py:51)
 //   doppler_fft_*    chunk sum + FFT along Doppler + fftshift  (range_doppler_processing.py:89)
 //
-// lagcorr and fir_apply share one inner loop, slide_mac<>: a register-tiled sliding
-// window complex multiply-accumulate.  A thread owns TD accumulators and a ring of
-// TI+TD window samples; every step it pulls TI fresh window samples (128-bit LDS,
-// lane stride TD*8 B = an odd multiple of 16 B, hence bank-conflict free) and TI
-// broadcast operands, and issues TI*TD complex MACs (4 FFMA each).  That is
-// 4*TI*TD FFMA for TI 128-bit shared loads: the loop is FP32-pipe bound by design.
+// lagcorr, fir_apply and lagstream_kernel (lagstream.cuh) share one inner loop, a register-tiled
+// sliding-window complex multiply-accumulate on (re, im) register pairs (slide_mac2 / slide_mac2n).
+// A thread owns TD accumulator pairs per component and a ring of TI+TD window samples; every step
+// it pulls TI fresh window samples (128-bit LDS, lane stride TD*8 B = an odd multiple of 16 B,
+// hence bank-conflict free) and TI broadcast operands, and issues TI*TD complex MACs (4 FFMA
+// each): the loop is FP32-pipe bound by design.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -43,80 +43,19 @@ __device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
 template <int A, int B> struct Gcd { static constexpr int v = Gcd<B, A % B>::v; };
 template <int A> struct Gcd<A, 0> { static constexpr int v = A; };
 
-// acc += x * conj(w)   (CONJ)      or      acc += x * w
-template <bool CONJ>
-__device__ __forceinline__ void cmac(float2& acc, const float2 x, const float2 w) {
-    if (CONJ) {
-        acc.x = fmaf(x.x, w.x, acc.x);
-        acc.x = fmaf(x.y, w.y, acc.x);
-        acc.y = fmaf(x.y, w.x, acc.y);
-        acc.y = fmaf(-x.x, w.y, acc.y);
-    } else {
-        acc.x = fmaf(x.x, w.x, acc.x);
-        acc.x = fmaf(-x.y, w.y, acc.x);
-        acc.y = fmaf(x.x, w.y, acc.y);
-        acc.y = fmaf(x.y, w.x, acc.y);
-    }
-}
-
-// acc[v] += sum_{t<nsteps, u<TI}  xs[t*TI+u] (*) ws[t*TI+u+v]       v = 0..TD-1
-// xs: operand shared by the lanes of a group (broadcast loads); ws: this thread's window.
-// Both must be 16-byte aligned; ws must be readable up to index nsteps*TI + TD - 1.
-template <int TI, int TD, bool CONJ>
-__device__ __forceinline__ void slide_mac(float2 (&acc)[TD], const float2* __restrict__ xs,
-                                          const float2* __restrict__ ws, int nsteps) {
-    static_assert(TI % 2 == 0 && TD % 2 == 0, "128-bit shared loads need even tile sizes");
-    constexpr int RS = TI + TD;                       // ring size
-    constexpr int PERIOD = RS / Gcd<RS, TI>::v;       // steps after which ring slots repeat
-    static_assert(PERIOD <= 4, "unroll factor too large for the instruction cache");
-    float2 W[RS];
-#pragma unroll
-    for (int q = 0; q < TD; q += 2) {
-        const float4 v = *reinterpret_cast<const float4*>(ws + q);
-        W[q] = make_float2(v.x, v.y);
-        W[q + 1] = make_float2(v.z, v.w);
-    }
-    for (int t0 = 0; t0 < nsteps; t0 += PERIOD) {
-#pragma unroll
-        for (int p = 0; p < PERIOD; ++p) {
-            if (t0 + p < nsteps) {
-                const float2* wp = ws + (t0 + p) * TI + TD;
-                const float2* xp = xs + (t0 + p) * TI;
-#pragma unroll
-                for (int q = 0; q < TI; q += 2) {
-                    const float4 v = *reinterpret_cast<const float4*>(wp + q);
-                    W[(p * TI + TD + q) % RS] = make_float2(v.x, v.y);
-                    W[(p * TI + TD + q + 1) % RS] = make_float2(v.z, v.w);
-                }
-#pragma unroll
-                for (int u = 0; u < TI; u += 2) {
-                    const float4 xv = *reinterpret_cast<const float4*>(xp + u);
-                    const float2 x0 = make_float2(xv.x, xv.y);
-                    const float2 x1 = make_float2(xv.z, xv.w);
-#pragma unroll
-                    for (int v = 0; v < TD; ++v) cmac<CONJ>(acc[v], x0, W[(p * TI + u + v) % RS]);
-#pragma unroll
-                    for (int v = 0; v < TD; ++v) cmac<CONJ>(acc[v], x1, W[(p * TI + u + 1 + v) % RS]);
-                }
-            }
-        }
-    }
-}
-
-// Packed variant: the same sliding-window MAC on (re, im) register pairs (ffma2_rn).  With
-//   A1[v] += (xr, xr) * (wr, wi)      A2[v] += (xi, xi) * (wr, wi)
-// every operand is an aligned 64-bit register pair.  On sm_90a each pair is two scalar FFMAs, so the
-// instruction count equals the scalar form's; what differs is the operand layout (one broadcast
-// load per sample, accumulators in pairs).  Which form is faster on the H100 has not been measured:
-// PRC_PACKED selects it for A/B runs.  The caller combines
+// Sliding-window MAC on (re, im) register pairs (ffma2_rn):
+//   A1[v] += sum_{t<nsteps, u<TI} (xr, xr)[t*TI+u] * (wr, wi)[t*TI+u+v]      A2[v]: the same with (xi, xi)
+// v = 0..TD-1; every operand is an aligned 64-bit register pair (on sm_90a each pair is two scalar FFMAs).
+// xs4: operand shared by the lanes of a group, xs4[i] = (xr, xr, xi, xi) of sample i (one broadcast 128-bit
+// load per sample); ws: this thread's window.  Both must be 16-byte aligned; ws must be readable up to index
+// nsteps*TI + TD - 1.  The caller combines
 //   x*conj(w): re = A1.x + A2.y, im = A2.x - A1.y        x*w: re = A1.x - A2.y, im = A1.y + A2.x
-// xs4[i] = (xr, xr, xi, xi) of sample i (one broadcast 128-bit load per sample).
 template <int TI, int TD>
 __device__ __forceinline__ void slide_mac2(float2 (&A1)[TD], float2 (&A2)[TD], const float4* __restrict__ xs4,
                                            const float2* __restrict__ ws, int nsteps) {
     static_assert(TI % 2 == 0 && TD % 2 == 0, "128-bit shared loads need even tile sizes");
-    constexpr int RS = TI + TD;
-    constexpr int PERIOD = RS / Gcd<RS, TI>::v;
+    constexpr int RS = TI + TD;                       // ring size
+    constexpr int PERIOD = RS / Gcd<RS, TI>::v;       // steps after which ring slots repeat
     static_assert(PERIOD <= 4, "unroll factor too large for the instruction cache");
     float2 W[RS];
 #pragma unroll
@@ -223,8 +162,8 @@ struct LagCorrParams {
     float2* partial;
 };
 
-// PACKED: x is staged as (xr, xr, xi, xi) float4 and the MACs are FFMA2 (slide_mac2)
-template <int TI, int TD, bool PACKED>
+// x is staged as (xr, xr, xi, xi) float4 and the MACs are FFMA2 (slide_mac2)
+template <int TI, int TD>
 __global__ void __launch_bounds__(512) lagcorr_kernel(const __grid_constant__ LagCorrParams p) {
     extern __shared__ __align__(16) float2 smem[];
     const int tid = threadIdx.x;
@@ -235,7 +174,7 @@ __global__ void __launch_bounds__(512) lagcorr_kernel(const __grid_constant__ La
     const int Sg = p.steps * TI;
     const int Lpad = p.G * Sg;
     const int HT = p.H * TD;
-    constexpr int XW = PACKED ? 2 : 1;      // float2 slots per staged x sample
+    constexpr int XW = 2;                   // float2 slots per staged x sample
     float2* xs = smem;
     float2* ss = smem + XW * Lpad;
 
@@ -269,8 +208,7 @@ __global__ void __launch_bounds__(512) lagcorr_kernel(const __grid_constant__ La
             if (q < Lpad) {
                 float2 t = v[b];
                 if (p.win || p.taps) { t.x *= w[b]; t.y *= w[b]; }
-                if (PACKED) reinterpret_cast<float4*>(xs)[q] = make_float4(t.x, t.x, t.y, t.y);
-                else xs[q] = t;
+                reinterpret_cast<float4*>(xs)[q] = make_float4(t.x, t.x, t.y, t.y);
             }
         }
     }
@@ -307,16 +245,12 @@ __global__ void __launch_bounds__(512) lagcorr_kernel(const __grid_constant__ La
     const int g = tid / p.H;
     const bool active = g < p.G;
     if (active) {
-        if (PACKED) {
-            float2 A1[TD], A2[TD];
+        float2 A1[TD], A2[TD];
 #pragma unroll
-            for (int v = 0; v < TD; ++v) { A1[v] = make_float2(0.f, 0.f); A2[v] = make_float2(0.f, 0.f); }
-            slide_mac2<TI, TD>(A1, A2, reinterpret_cast<const float4*>(xs) + g * Sg, ss + g * Sg + h * TD, p.steps);
+        for (int v = 0; v < TD; ++v) { A1[v] = make_float2(0.f, 0.f); A2[v] = make_float2(0.f, 0.f); }
+        slide_mac2<TI, TD>(A1, A2, reinterpret_cast<const float4*>(xs) + g * Sg, ss + g * Sg + h * TD, p.steps);
 #pragma unroll
-            for (int v = 0; v < TD; ++v) acc[v] = make_float2(A1[v].x + A2[v].y, A2[v].x - A1[v].y);
-        } else {
-            slide_mac<TI, TD, true>(acc, xs + g * Sg, ss + g * Sg + h * TD, p.steps);
-        }
+        for (int v = 0; v < TD; ++v) acc[v] = make_float2(A1[v].x + A2[v].y, A2[v].x - A1[v].y);
     }
     __syncthreads();
 
@@ -365,25 +299,20 @@ __device__ __forceinline__ uint16_t fir_bf16_rn(float v) {
     return (uint16_t)(u >> 16);
 }
 
-// MODE 0: scalar FFMA; 1: FFMA2 with (t,t) pairs staged in shared memory; 2: FFMA2 with the pairs
-// built in registers (fewest shared-memory bytes per MAC, see slide_mac2n in lagstream.cuh)
-template <int TK, int TO, int MODE>
-__global__ void __launch_bounds__((TK * TO > 100) ? 256 : 512) fir_apply_kernel(const __grid_constant__ FirParams p) {
-    constexpr bool PACKED = (MODE == 1);
+// FFMA2 with the (t, t) operand pairs built in registers (slide_mac2n: fewest shared-memory bytes per MAC)
+template <int TK, int TO>
+__global__ void __launch_bounds__(512) fir_apply_kernel(const __grid_constant__ FirParams p) {
     extern __shared__ __align__(16) float2 smem[];
     const int tid = threadIdx.x;
     const int nthr = blockDim.x;
     const int LO = nthr * TO;
-    constexpr int XW = PACKED ? 2 : 1;
-    float2* tr = smem;                   // Mpad reversed taps ((tr, tr, ti, ti) when PACKED)
-    float2* rs = smem + XW * p.Mpad;     // LO + Mpad window of ref
+    float2* tr = smem;                   // Mpad reversed taps
+    float2* rs = smem + p.Mpad;          // LO + Mpad window of ref
     const long long I0 = (long long)blockIdx.x * LO;
 
     for (int q = tid; q < p.Mpad; q += nthr) {
         const int k = p.Mpad - 1 - q;
-        const float2 tv = (k < p.M) ? p.taps[k] : make_float2(0.f, 0.f);
-        if (PACKED) reinterpret_cast<float4*>(tr)[q] = make_float4(tv.x, tv.x, tv.y, tv.y);
-        else tr[q] = tv;
+        tr[q] = (k < p.M) ? p.taps[k] : make_float2(0.f, 0.f);
     }
     {
         long long r0 = (I0 + p.peek - (p.Mpad - 1)) % p.n;
@@ -414,19 +343,12 @@ __global__ void __launch_bounds__((TK * TO > 100) ? 256 : 512) fir_apply_kernel(
     __syncthreads();
 
     float2 acc[TO];
+    float2 A1[TO], A2[TO];
 #pragma unroll
-    for (int v = 0; v < TO; ++v) acc[v] = make_float2(0.f, 0.f);
-    if (MODE >= 1) {
-        float2 A1[TO], A2[TO];
+    for (int v = 0; v < TO; ++v) { A1[v] = make_float2(0.f, 0.f); A2[v] = make_float2(0.f, 0.f); }
+    slide_mac2n<TK, TO>(A1, A2, tr, rs + tid * TO, p.Mpad / TK);
 #pragma unroll
-        for (int v = 0; v < TO; ++v) { A1[v] = make_float2(0.f, 0.f); A2[v] = make_float2(0.f, 0.f); }
-        if (MODE == 1) slide_mac2<TK, TO>(A1, A2, reinterpret_cast<const float4*>(tr), rs + tid * TO, p.Mpad / TK);
-        else slide_mac2n<TK, TO>(A1, A2, tr, rs + tid * TO, p.Mpad / TK);
-#pragma unroll
-        for (int v = 0; v < TO; ++v) acc[v] = make_float2(A1[v].x - A2[v].y, A1[v].y + A2[v].x);
-    } else {
-        slide_mac<TK, TO, false>(acc, tr, rs + tid * TO, p.Mpad / TK);
-    }
+    for (int v = 0; v < TO; ++v) acc[v] = make_float2(A1[v].x - A2[v].y, A1[v].y + A2[v].x);
 
     const long long i0 = I0 + (long long)tid * TO;
 #pragma unroll

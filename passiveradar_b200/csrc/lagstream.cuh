@@ -83,7 +83,7 @@ __device__ __forceinline__ SubChunk next_subchunk(const LagStreamParams& p, long
 }
 
 template <int TI, int TD>
-__global__ void __launch_bounds__((TI * TD > 100) ? 256 : 512) lagstream_kernel(const __grid_constant__ LagStreamParams p) {
+__global__ void __launch_bounds__(512) lagstream_kernel(const __grid_constant__ LagStreamParams p) {
     extern __shared__ __align__(16) float2 smem[];
     const int tid = threadIdx.x;
     const int nthr = blockDim.x;

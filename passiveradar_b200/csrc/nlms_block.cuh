@@ -3,8 +3,8 @@
 //
 // The reference recurrence
 //     e_k = d_k - w_k^H u_k,   w_{k+1} = w_k + mu u_k conj(e_k) / (u_k^H u_k),   u_k[j] = ref[M + k - j]
-// carries the whole tap vector from sample to sample, which makes the straightforward kernel (nlms.cuh) pay a
-// block-wide reduction over the M taps per sample (~330 cycles).  Inside a block of L samples that starts with
+// carries the whole tap vector from sample to sample, which makes a sample-serial kernel pay a block-wide
+// reduction over the M taps per sample (~330 cycles).  Inside a block of L samples that starts with
 // taps W the same numbers follow from a triangular system in the Gram matrix of the regressors:
 //     r_k = d_k - W^H u_k                                     (L dot products, independent of each other)
 //     e_k = r_k - mu * sum_{m<k} e_m g(m,k) / p_m,   g(m,k) = u_m^H u_k,  p_m = g(m,m)
@@ -16,10 +16,40 @@
 #pragma once
 #include <cuda_runtime.h>
 
-#include "nlms.cuh"
-
 namespace prc {
 
+struct NlmsParams {
+    const float2* ref;
+    const float2* srv;
+    const float2* init;      // M initial taps or nullptr
+    float2* out;             // n
+    float2* taps_out;        // M or nullptr
+    int n;
+    int filter_len;
+    int peek;
+    float mu;
+    int block_len;
+    // a batch of independent frames, one CTA each (gridDim.x): frame f reads ref/srv + f * frame_stride, writes
+    // out + f * frame_stride; init / taps_out advance by filter_len + peek taps per frame (init_shared: every frame
+    // starts from the same init taps)
+    long long frame_stride;
+    int init_shared;
+};
+
+__device__ __forceinline__ NlmsParams nlms_frame_params(const NlmsParams& g) {
+    NlmsParams p = g;
+    const size_t f = blockIdx.x;
+    const int M = g.filter_len + g.peek;
+    p.ref += f * g.frame_stride;
+    p.srv += f * g.frame_stride;
+    p.out += f * g.frame_stride;
+    if (p.init && !g.init_shared) p.init += f * M;
+    if (p.taps_out) p.taps_out += f * M;
+    return p;
+}
+
+constexpr int NLMS_TILE = 1024;      // samples staged per shared-memory tile
+constexpr int NLMS_MAXT = 4;         // max taps per thread (M <= 4096)
 constexpr int NB_L = 32;             // samples per exact block (one warp lane each)
 constexpr int NB_THREADS = 1024;
 constexpr int NB_PAD = 64;           // extra reference samples staged behind a tile (lag reach of the Gram)

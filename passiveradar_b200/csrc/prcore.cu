@@ -27,7 +27,6 @@
 #include "firtc.cuh"
 #include "frontend.cuh"
 #include "detect.cuh"
-#include "nlms.cuh"
 #include "nlms_block.cuh"
 #include "gal.cuh"
 #include "track.cuh"
@@ -40,16 +39,10 @@ namespace {
 
 using namespace prc;
 
-// slide_mac tile shapes (DESIGN.md section 3.1): 10 x 10 complex MACs per step, lane stride
+// Register tile of the FP32 sliding-window kernels (lagcorr, lagstream, fir_apply; DESIGN.md section 3.8):
+// TILE_I x TILE_D = 10 x 10 complex MACs per step (samples x lags, or taps x outputs), lane stride
 // 10 complex = 80 B (odd multiple of 16 B => conflict-free 128-bit shared loads).
-constexpr int LC_TI = 10, LC_TD = 10;     // one-shot lagcorr kernel: samples x lags per step
-constexpr int FIR_TK = 10, FIR_TO = 10;   // legacy fir variants: taps x outputs per step
-// Register-tile variants of the pipelined kernels (PRC_TILE).  Shared-memory loads cost the FMA
-// pipe ~9 cycles per 128-bit load (scripts/microbench/fma_peak2.cu), and a TI x TD tile needs
-// 2*TI loads per TI*TD MACs, so a larger TD buys efficiency until registers run out.
-//   0: 10 x 10   1: 6 x 18   2: 14 x 14      (TD*8 B must be an odd multiple of 16 B)
-struct TileShape { int ti, td; };
-constexpr TileShape kTiles[3] = {{10, 10}, {6, 18}, {14, 14}};
+constexpr int TILE_I = 10, TILE_D = 10;
 constexpr int FIR_THREADS = 128;
 constexpr size_t SMEM_LIMIT = 200 * 1024;
 
@@ -187,15 +180,11 @@ std::vector<Ctx*> g_all_ctx;
 std::atomic<bool> g_attrs_set[64];
 std::atomic<uint64_t> g_epoch{1};                      // bumped by prc_shutdown
 int g_tune_nchunk = -1, g_tune_g = -1;
-int g_tile = 0;          // register tile of the FP32 lag kernels: 10x10 (PRC_TILE=1: 6x18, 2: 14x14)
-int g_nlms_block = 1;       // block-exact NLMS kernel for NLMS_filter (PRC_NLMS_BLOCK=0: sample-serial kernel)
 int g_tma_l2 = 2;          // CUtensorMapL2promotion: 0 none, 1 64B, 2 128B, 3 256B (PRC_TMA_L2)
 int g_tma = 1;             // TMA (cp.async.bulk.tensor) producers for the wgmma kernels (PRC_TMA=0: 16-byte cp.async loaders)
 int g_tc_fir = 1;          // tensor-core path for the clutter FIR (PRC_TC_FIR=0: FP32 fir_apply_kernel)
 int g_tc_caf = 1;          // tensor-core path for the CAF block sums as well (PRC_TC_CAF=0: FP32 lagstream)
 int g_tc = 1;              // wgmma Toeplitz-GEMM for the LS correlations (PRC_TC=0: FP32 lagstream kernel)
-int g_stream = 1;          // persistent pipelined lag-correlation kernel (PRC_STREAM=0: one-shot kernel)
-int g_packed = 1;          // paired-FMA kernels (PRC_PACKED=0 selects the scalar-FFMA variant for A/B runs)
 std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: wgmma / FP32 direct form
 std::atomic<int> g_fft_min_n{8192};   // ... for channels of at least this many samples (PRC_FFT_MIN_N)
 std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks instead of one CTA per block
@@ -231,15 +220,11 @@ thread_local TlsCtx g_tls;
 void read_env() {
     if (const char* e = getenv("PRC_TUNE_NCHUNK")) g_tune_nchunk = atoi(e);
     if (const char* e = getenv("PRC_TUNE_G")) g_tune_g = atoi(e);
-    if (const char* e = getenv("PRC_PACKED")) g_packed = atoi(e);
-    if (const char* e = getenv("PRC_STREAM")) g_stream = atoi(e);
     if (const char* e = getenv("PRC_TC")) g_tc = atoi(e);
     if (const char* e = getenv("PRC_TC_CAF")) g_tc_caf = atoi(e);
     if (const char* e = getenv("PRC_TC_FIR")) g_tc_fir = atoi(e);
     if (const char* e = getenv("PRC_TMA")) g_tma = atoi(e);
-    if (const char* e = getenv("PRC_NLMS_BLOCK")) g_nlms_block = atoi(e);
     if (const char* e = getenv("PRC_TMA_L2")) g_tma_l2 = atoi(e);
-    if (const char* e = getenv("PRC_TILE")) g_tile = std::max(0, std::min(2, atoi(e)));
     if (const char* e = getenv("PRC_FFT")) g_fft.store(atoi(e));
     if (const char* e = getenv("PRC_FFT_MIN_N")) g_fft_min_n.store(atoi(e));
 }
@@ -247,29 +232,19 @@ void read_env() {
 int set_kernel_attrs(int device) {
     if (g_attrs_set[device].load()) return PRC_OK;
     const int lim = (int)SMEM_LIMIT;
-    CU(cudaFuncSetAttribute(lagcorr_kernel<LC_TI, LC_TD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(lagcorr_kernel<LC_TI, LC_TD, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(lagcorr_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(tc::firtc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(tc::toepcorr_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(tc::toepcorr_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(tc::toepcorr_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(tc::toepcorr_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(lagstream_kernel<10, 10>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(lagstream_kernel<6, 18>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(lagstream_kernel<14, 14>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(fir_apply_kernel<FIR_TK, FIR_TO, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(fir_apply_kernel<FIR_TK, FIR_TO, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(fir_apply_kernel<10, 10, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(fir_apply_kernel<6, 18, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(fir_apply_kernel<14, 14, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(lagstream_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
+    CU(cudaFuncSetAttribute(fir_apply_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(levinson_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(levinson_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(doppler_fft_pow2_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(doppler_fft_pow2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(doppler_fft_pow2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(nlms_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(nlms_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(nlms_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(nlms_block_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
@@ -385,7 +360,7 @@ struct Geo {
 int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 int choose_geo(int blk_len, long long outer, int nlag, int nsm, Geo* g) {
-    const int TI = LC_TI, TD = LC_TD;
+    const int TI = TILE_I, TD = TILE_D;
     g->H = ceil_div(nlag, TD);
     g->HT = g->H * TD;
     if (g->H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
@@ -402,7 +377,7 @@ int choose_geo(int blk_len, long long outer, int nlag, int nsm, Geo* g) {
         g->G = std::max(1, std::min(gmax, ceil_div(g->chunk_len, TI * 4)));
         g->steps = ceil_div(ceil_div(g->chunk_len, g->G), TI);
         const size_t Lpad = (size_t)g->G * g->steps * TI;
-        g->smem = std::max((g_packed ? 3 : 2) * Lpad + g->HT, (size_t)g->G * g->HT) * sizeof(float2);
+        g->smem = std::max(3 * Lpad + g->HT, (size_t)g->G * g->HT) * sizeof(float2);
         if (g->smem <= 100 * 1024 || g->chunk_len <= TI) break;
         nchunk = nchunk * 2;
     }
@@ -419,14 +394,12 @@ struct StreamGeo {
 
 // CTAs per problem: fill every SM with two co-resident CTAs, but keep >= 2 full steps per CTA
 int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo* g) {
-    const int TI = kTiles[g_tile].ti, TD = kTiles[g_tile].td;
+    const int TI = TILE_I, TD = TILE_D;
     g->H = ceil_div(nlag, TD);
     g->HT = g->H * TD;
     if (g->H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
-    const int max_threads = (TI * TD > 100) ? 256 : 512;     // the big tiles are compiled for <= 256 threads
-    if (g->H > max_threads) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, max_threads * TD);
     int G = std::max(1, std::min(32, 256 / g->H));
-    if (g_tune_g > 0) G = std::max(1, std::min(g_tune_g, max_threads / g->H));
+    if (g_tune_g > 0) G = std::max(1, std::min(g_tune_g, 512 / g->H));
     g->total = (long long)nblk * blk_len;
     long long want = std::max(1, 2 * nsm / nprob);
     if (g_tune_nchunk > 0) want = g_tune_nchunk;
@@ -450,11 +423,7 @@ int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo
 }
 
 void launch_lagstream(dim3 grid, int threads, size_t smem, cudaStream_t st, const LagStreamParams& sp) {
-    switch (g_tile) {
-        case 0: lagstream_kernel<10, 10><<<grid, threads, smem, st>>>(sp); break;
-        case 1: lagstream_kernel<6, 18><<<grid, threads, smem, st>>>(sp); break;
-        default: lagstream_kernel<14, 14><<<grid, threads, smem, st>>>(sp); break;
-    }
+    lagstream_kernel<TILE_I, TILE_D><<<grid, threads, smem, st>>>(sp);
 }
 
 // ---- tensor maps (TMA).  cuTensorMapEncodeTiled is a host-only driver call, resolved through the runtime
@@ -892,7 +861,7 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
         g.HT = ct.ht;
         bnd_x = xw;
         bnd_w_all = bnd_w;
-    } else if (g_stream && taps == nullptr && ntaps >= 64) {   // tiny Doppler blocks: one flush per block would dominate
+    } else if (taps == nullptr && ntaps >= 64) {   // tiny Doppler blocks: one flush per block would dominate
         StreamGeo sg;
         TRY(choose_stream((int)ntaps, F, 1, R + 1, c->nsm, &sg));
         TRY(c->partial.ensure((size_t)F * sg.maxpieces * sg.HT * sizeof(float2)));
@@ -952,8 +921,7 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
     {
         ProfScope ps(c, K_LAGCORR_CAF);
         const dim3 grid((unsigned)((long long)F * g.nchunk), 1);
-        if (g_packed) lagcorr_kernel<LC_TI, LC_TD, true><<<grid, g.threads, g.smem, c->stream>>>(p);
-        else lagcorr_kernel<LC_TI, LC_TD, false><<<grid, g.threads, g.smem, c->stream>>>(p);
+        lagcorr_kernel<TILE_I, TILE_D><<<grid, g.threads, g.smem, c->stream>>>(p);
     }
     TRY(check_launch("lagcorr_kernel(caf)"));
     }
@@ -1118,7 +1086,7 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
         TRY(check_launch("toepcorr_kernel"));
         g.nchunk = tc_npass * tc_ranges;
         g.HT = tc_ht;
-    } else if (g_stream || linear) {
+    } else {
         StreamGeo sg;
         TRY(choose_stream((int)n, 1, 2, M, c->nsm, &sg));
         TRY(c->partial.ensure((size_t)2 * sg.maxpieces * sg.HT * sizeof(float2)));
@@ -1144,30 +1112,6 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
         TRY(check_launch("lagstream_kernel(ls)"));
         g.nchunk = sg.maxpieces;      // == pieces of the single block == ncta
         g.HT = sg.HT;
-    } else {
-    TRY(choose_geo((int)n, 2, M, c->nsm, &g));
-    TRY(c->partial.ensure((size_t)2 * g.nchunk * g.HT * sizeof(float2)));
-
-    LagCorrParams p{};
-    p.x = ref;
-    p.s[0] = ref; p.s[1] = srv;
-    p.dmin[0] = 0; p.dmin[1] = -peek;
-    p.win = nullptr; p.taps = nullptr;
-    p.n = (int)n;
-    p.blk_first_lo = 0;
-    p.blk_stride = 0;
-    p.blk_len = (int)n;
-    p.nblk = 1;
-    p.nchunk = g.nchunk;
-    p.chunk_len = g.chunk_len;
-    p.H = g.H; p.G = g.G; p.steps = g.steps;
-    p.partial = c->partial.as<float2>();
-    {
-        ProfScope ps(c, K_LAGCORR_LS);
-        if (g_packed) lagcorr_kernel<LC_TI, LC_TD, true><<<dim3(g.nchunk, 2), g.threads, g.smem, c->stream>>>(p);
-        else lagcorr_kernel<LC_TI, LC_TD, false><<<dim3(g.nchunk, 2), g.threads, g.smem, c->stream>>>(p);
-    }
-    TRY(check_launch("lagcorr_kernel(ls)"));
     }
 
     LevinsonParams lp{};
@@ -1228,21 +1172,14 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
     }
     fp.n = (int)n; fp.M = M; fp.peek = peek;
     fp.linear = linear ? 1 : 0;
-    const int mode = g_stream ? 2 : (g_packed ? 1 : 0);
-    const int tk = mode == 2 ? kTiles[g_tile].ti : FIR_TK, to = mode == 2 ? kTiles[g_tile].td : FIR_TO;
-    fp.Mpad = ceil_div(M, tk) * tk;
-    if (fp.Mpad & 1) fp.Mpad += tk;          // keep the ref window 16-byte aligned behind the taps
-    const int LO = FIR_THREADS * to;
-    const size_t sm = (size_t)((mode == 1 ? 2 : 1) * fp.Mpad + LO + fp.Mpad) * sizeof(float2);
+    fp.Mpad = ceil_div(M, TILE_I) * TILE_I;
+    if (fp.Mpad & 1) fp.Mpad += TILE_I;      // keep the ref window 16-byte aligned behind the taps
+    const int LO = FIR_THREADS * TILE_D;
+    const size_t sm = (size_t)(fp.Mpad + LO + fp.Mpad) * sizeof(float2);
     if (sm > SMEM_LIMIT) return fail(PRC_E_INVALID, "%d taps exceed the FIR kernel's shared memory", M);
     {
         ProfScope ps(c, K_FIR);
-        const int grid = ceil_div(n, LO);
-        if (mode == 0) fir_apply_kernel<FIR_TK, FIR_TO, 0><<<grid, FIR_THREADS, sm, c->stream>>>(fp);
-        else if (mode == 1) fir_apply_kernel<FIR_TK, FIR_TO, 1><<<grid, FIR_THREADS, sm, c->stream>>>(fp);
-        else if (g_tile == 0) fir_apply_kernel<10, 10, 2><<<grid, FIR_THREADS, sm, c->stream>>>(fp);
-        else if (g_tile == 1) fir_apply_kernel<6, 18, 2><<<grid, FIR_THREADS, sm, c->stream>>>(fp);
-        else fir_apply_kernel<14, 14, 2><<<grid, FIR_THREADS, sm, c->stream>>>(fp);
+        fir_apply_kernel<TILE_I, TILE_D><<<ceil_div(n, LO), FIR_THREADS, sm, c->stream>>>(fp);
     }
     TRY(check_launch("fir_apply_kernel"));
     if (taps_out)
@@ -1454,30 +1391,21 @@ int nlms_device(Ctx* c, const float2* ref, const float2* srv, long long n, int f
     p.ref = ref; p.srv = srv; p.init = init; p.out = out; p.taps_out = taps_out;
     p.n = (int)n; p.filter_len = filter_len; p.peek = peek; p.mu = mu; p.block_len = block_len;
     p.frame_stride = bt.nf > 1 ? bt.stride : 0; p.init_shared = init_shared ? 1 : 0;
-    const int kt = M <= 1024 ? 1 : (M <= 2048 ? 2 : 4);
-    const int threads = std::min(1024, ((ceil_div(M, kt) + 31) / 32) * 32);
-    const size_t sm = (size_t)(NLMS_TILE + ((M + 1) & ~1) + NLMS_TILE) * sizeof(float2) + 64 * sizeof(float4);
+    // exact evaluation 32 samples at a time (nlms_block.cuh); block_len > 1 (block_NLMS) freezes the taps inside a
+    // user block
+    const size_t sb = nlms_block_smem(M);
     ProfScope ps(c, K_NLMS);
-    if (g_nlms_block) {
-        // exact evaluation 32 samples at a time (nlms_block.cuh), 4x the speed of the sample-serial kernel at
-        // config 4; block_len > 1 (block_NLMS) freezes the taps inside a user block
-        const size_t sb = nlms_block_smem(M);
-        if (bt.nf > c->nsm && M <= 2048) {
-            // more frames than SMs: 512-thread CTAs, two resident per SM (a 1024-thread CTA owns the SM's registers)
-            if (M <= 512) nlms_block_kernel<1, 512><<<bt.nf, 512, sb, c->stream>>>(p);
-            else if (M <= 1024) nlms_block_kernel<2, 512><<<bt.nf, 512, sb, c->stream>>>(p);
-            else nlms_block_kernel<4, 512><<<bt.nf, 512, sb, c->stream>>>(p);
-            return check_launch("nlms_block_kernel");
-        }
-        if (kt == 1) nlms_block_kernel<1><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
-        else if (kt == 2) nlms_block_kernel<2><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
-        else nlms_block_kernel<4><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
+    if (bt.nf > c->nsm && M <= 2048) {
+        // more frames than SMs: 512-thread CTAs, two resident per SM (a 1024-thread CTA owns the SM's registers)
+        if (M <= 512) nlms_block_kernel<1, 512><<<bt.nf, 512, sb, c->stream>>>(p);
+        else if (M <= 1024) nlms_block_kernel<2, 512><<<bt.nf, 512, sb, c->stream>>>(p);
+        else nlms_block_kernel<4, 512><<<bt.nf, 512, sb, c->stream>>>(p);
         return check_launch("nlms_block_kernel");
     }
-    if (kt == 1) nlms_kernel<1><<<bt.nf, threads, sm, c->stream>>>(p);
-    else if (kt == 2) nlms_kernel<2><<<bt.nf, threads, sm, c->stream>>>(p);
-    else nlms_kernel<4><<<bt.nf, threads, sm, c->stream>>>(p);
-    return check_launch("nlms_kernel");
+    if (M <= 1024) nlms_block_kernel<1><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
+    else if (M <= 2048) nlms_block_kernel<2><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
+    else nlms_block_kernel<4><<<bt.nf, NB_THREADS, sb, c->stream>>>(p);
+    return check_launch("nlms_block_kernel");
 }
 
 // GAL_JPE on bt.nf independent frames (gal.cuh): delay lines up to GAL_WARP_MAX_D taps run one frame per warp
@@ -1906,7 +1834,6 @@ int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, 
 const int* env_switch(const std::string& k) {
     static const std::pair<const char*, const int*> kSwitches[] = {
         {"tma", &g_tma}, {"tma_l2", &g_tma_l2}, {"tc", &g_tc}, {"tc_caf", &g_tc_caf}, {"tc_fir", &g_tc_fir},
-        {"stream", &g_stream}, {"packed", &g_packed}, {"tile", &g_tile}, {"nlms_block", &g_nlms_block},
         {"tune_nchunk", &g_tune_nchunk}, {"tune_g", &g_tune_g}};
     for (const auto& s : kSwitches)
         if (k == s.first) return s.second;

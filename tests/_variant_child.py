@@ -28,16 +28,13 @@ from passiveradar_b200 import synth     # noqa: E402
 # prc_get_option name -> (environment variable, value when the variable is unset: prcore.cu's defaults)
 SWITCHES = {
     "tma": ("PRC_TMA", 1), "tma_l2": ("PRC_TMA_L2", 2), "tc": ("PRC_TC", 1), "tc_caf": ("PRC_TC_CAF", 1),
-    "tc_fir": ("PRC_TC_FIR", 1), "stream": ("PRC_STREAM", 1), "packed": ("PRC_PACKED", 1), "tile": ("PRC_TILE", 0),
-    "nlms_block": ("PRC_NLMS_BLOCK", 1), "tune_nchunk": ("PRC_TUNE_NCHUNK", -1), "tune_g": ("PRC_TUNE_G", -1),
+    "tc_fir": ("PRC_TC_FIR", 1), "tune_nchunk": ("PRC_TUNE_NCHUNK", -1), "tune_g": ("PRC_TUNE_G", -1),
 }
 
 
 def expected_switches(env):
-    """What the library must report for environment `env` (PRC_TILE is clamped to 0..2, as read_env does)."""
-    want = {k: int(env[var]) if var in env else default for k, (var, default) in SWITCHES.items()}
-    want["tile"] = max(0, min(2, want["tile"]))
-    return want
+    """What the library must report for environment `env`."""
+    return {k: int(env[var]) if var in env else default for k, (var, default) in SWITCHES.items()}
 
 
 def library_switches():
@@ -103,7 +100,7 @@ def frame_inputs():
 
 
 NLMS = dict(n=2 ** 15, profile="P1", frame=4, mu=0.05, peek=10)
-NLMS_FILTER_LENS = (400, 1100, 3000)       # M = 410, 1110, 3010: nlms_block_kernel<1>, <2>, <4> (nlms_kernel<1/2/4>)
+NLMS_FILTER_LENS = (400, 1100, 3000)       # M = 410, 1110, 3010: nlms_block_kernel<1>, <2>, <4>
 NLMS_BLOCK = dict(filter_len=1100, block_len=64)
 
 
