@@ -286,6 +286,18 @@ int prc_resample_out_len(int64_t n_in, int up, int down, int nh, int64_t* n_out)
 int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc, double fs, double phase_offset,
                      int up, int down, const double* h, int nh, prc_c64* out, int64_t out_capacity,
                      int mem_kind, int device, void* stream, unsigned flags);
+/* prc_frontend_chunks_c64: prc_frontend_c64 on nchunks chunks of n complex samples in one launch, what main.py:105-166
+ * does to every chunk of a recording.  Chunk b starts at complex sample b * chunk_stride of `in` (any element: I and Q
+ * are read as scalars, so `in` itself may sit at an odd raw element), is mixed with phase_offsets[b] and resampled
+ * with the line extension of its own end points.  phase_offsets is nchunks doubles in host memory whatever mem_kind
+ * is; they are copied before the call returns, also with PRC_FLAG_ASYNC.  Its prc_resample_out_len() samples go to
+ * out + b * out_stride (out_stride >= that length when nchunks > 1).  out_capacity counts complex samples from `out`.
+ * Every chunk's output is bit-identical to a prc_frontend_c64 call on that chunk; the errors are the same.
+ */
+int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks, int64_t chunk_stride, int mode,
+                            double fc, double fs, const double* phase_offsets, int up, int down, const double* h, int nh,
+                            prc_c64* out, int64_t out_stride, int64_t out_capacity, int mem_kind, int device,
+                            void* stream, unsigned flags);
 
 /* ---- CFAR detector ---------------------------------------------------------------------------------
  * Replaces CFAR_2D(X, fw, gw, thresh), reference passiveRadar/target_detection.py:683-703: X / mean|X|

@@ -18,12 +18,13 @@ from .signal_utils import (deinterleave_IQ, frequency_shift, resample, frontend,
 from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
                                multitarget_tracker_frames, simple_tracker_frames, cfar_track,
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
+from .recording import RecordingPipeline                                     # noqa: F401
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
            "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
            "find_channel_offset", "offset_compensation", "shift", "xcorr", "CFAR_2D",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
-           "simple_tracker_frames", "cfar_track"]
+           "simple_tracker_frames", "cfar_track", "RecordingPipeline"]
 __version__ = "0.1.0"
 
 

@@ -86,6 +86,9 @@ SIGNATURES = {
     "prc_frontend_c64": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double, C.c_double,
                                    C.c_int, C.c_int, C.c_void_p, C.c_int, _c64p, C.c_int64,
                                    C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_frontend_chunks_c64": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_double,
+                                          C.c_double, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, _c64p,
+                                          C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_cfar2d_f32": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_get_measurements_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,

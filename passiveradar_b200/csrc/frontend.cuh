@@ -98,18 +98,20 @@ __global__ void resample_ends_kernel(const __grid_constant__ MixParams p, float2
     }
 }
 
-__global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_constant__ ResampleParams p, float2* __restrict__ out) {
-    extern __shared__ __align__(16) unsigned char rs_smem[];
-    float* hp = reinterpret_cast<float*>(rs_smem);                               // [up][tpp]
-    float2* xs = reinterpret_cast<float2*>(rs_smem + (((size_t)p.up * p.tpp * 4 + 15) & ~(size_t)15));
+// The two halves of a resample CTA, shared by resample_kernel and the per-chunk front end (recording.cuh) so that
+// both compute every output with the same instructions.
+// rs_stage: the polyphase table and the CTA's window xext[i_lo, i_lo + span) into shared memory; returns i_lo.
+// load(i) gives the (mixed) input sample i for 0 <= i < n; x0, x1 are load(0), load(n - 1).
+template <class Load>
+__device__ __forceinline__ long long rs_stage(const ResampleParams& p, long long n, const float2* ends, float* hp,
+                                              float2* xs, Load load) {
     const long long m0 = (long long)blockIdx.x * RS_THREADS;
-    const long long n = p.mix.n;
     // input index range of this CTA: output m uses i = floor(T / up) - j, j = 0 .. tpp-1, T = (m + npr) * down
     const long long Tlo = (m0 + p.n_pre_remove) * (long long)p.down;
     const long long i_hi0 = Tlo / p.up;                      // largest index of the first output
     const long long i_lo = i_hi0 - (p.tpp - 1);              // smallest index any output of the CTA needs
     for (int q = threadIdx.x; q < p.up * p.tpp; q += RS_THREADS) hp[q] = p.hp[q];
-    const float2 x0 = p.ends[0], x1 = p.ends[1];
+    const float2 x0 = ends[0], x1 = ends[1];
     // n == 1 gives 0/0 = NaN, and every output NaN, as scipy's padtype='line' does
     const float2 slope = make_float2((x1.x - x0.x) / (float)(n - 1), (x1.y - x0.y) / (float)(n - 1));
     for (int q = threadIdx.x; q < p.span; q += RS_THREADS) {
@@ -117,12 +119,15 @@ __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_const
         float2 v;
         if (i < 0) v = make_float2(x0.x + (float)i * slope.x, x0.y + (float)i * slope.y);
         else if (i >= n) v = make_float2(x1.x + (float)(i - n + 1) * slope.x, x1.y + (float)(i - n + 1) * slope.y);
-        else v = mix_sample(p.mix, iq_load(p.mix.in, p.mix.kind, i), i);
+        else v = load(i);
         xs[q] = v;
     }
-    __syncthreads();
-    const long long m = m0 + threadIdx.x;
-    if (m >= p.n_out) return;
+    return i_lo;
+}
+
+// rs_sum: output m of the CTA whose window rs_stage staged at i_lo
+__device__ __forceinline__ float2 rs_sum(const ResampleParams& p, const float* hp, const float2* xs, long long i_lo,
+                                         long long m) {
     const long long T = (m + p.n_pre_remove) * (long long)p.down;
     const long long ih = T / p.up;
     const int ph = (int)(T - ih * p.up);                     // hpad index of the newest sample: k = ph + j * up
@@ -141,7 +146,23 @@ __global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_const
         const float2 v0 = x[-j];
         ar = fmaf(h0, v0.x, ar); ai = fmaf(h0, v0.y, ai);
     }
-    out[m] = make_float2(ar + br, ai + bi);
+    return make_float2(ar + br, ai + bi);
+}
+
+__device__ __forceinline__ size_t rs_table_bytes(const ResampleParams& p) {
+    return ((size_t)p.up * p.tpp * 4 + 15) & ~(size_t)15;
+}
+
+__global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_constant__ ResampleParams p, float2* __restrict__ out) {
+    extern __shared__ __align__(16) unsigned char rs_smem[];
+    float* hp = reinterpret_cast<float*>(rs_smem);                               // [up][tpp]
+    float2* xs = reinterpret_cast<float2*>(rs_smem + rs_table_bytes(p));
+    const long long i_lo = rs_stage(p, p.mix.n, p.ends, hp, xs,
+                                    [&p](long long i) { return mix_sample(p.mix, iq_load(p.mix.in, p.mix.kind, i), i); });
+    __syncthreads();
+    const long long m = (long long)blockIdx.x * RS_THREADS + threadIdx.x;
+    if (m >= p.n_out) return;
+    out[m] = rs_sum(p, hp, xs, i_lo, m);
 }
 
 }  // namespace prc

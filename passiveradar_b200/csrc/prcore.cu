@@ -34,6 +34,7 @@
 #include "chanoff.cuh"
 #include "lssvd.cuh"
 #include "framepass.cuh"
+#include "recording.cuh"
 
 namespace {
 
@@ -52,12 +53,12 @@ std::atomic<uint64_t> g_launches{0};
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
-                K_CAF_COMBINE, K_COUNT };
+                K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
                                            "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
-                                           "caf_combine"};
+                                           "caf_combine", "frontend_chunks"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -124,6 +125,7 @@ struct Ctx {
     std::mutex mu;
     DBuf firb[3];             // Wm^T planes of the tensor-core FIR
     DBuf fe_in, fe_mid, fe_out, fe_hp, fe_ends;    // front end: raw IQ, mixed, resampled, polyphase taps, end points
+    DBuf fe_po, fe_cends;                          // front end over chunks: phase offsets, end points of every chunk
     DBuf cf_in, cf_cr, cf_det, cf_part;            // CFAR_2D
     uint64_t fe_hp_key = 0;                        // which taps fe_hp holds
     // tensor maps of the last LS / CAF launch of this context: the planes live in DBufs, so the operand addresses
@@ -159,7 +161,7 @@ struct Ctx {
         for (DBuf& b : fft_tw) b.release();
         for (bool& r : fft_tw_ready) r = false;
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP, &fpacc}) b->release();
-        for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
+        for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
                         &trk_slots, &trk_out, &trk_cnt, &svd_part, &svd_cr, &svd_ws, &svd_taps, &svd_rank})
@@ -1249,18 +1251,10 @@ int resample_geo(long long n_in, int up, int down, int nh, ResampleGeo* g) {
     return PRC_OK;
 }
 
-// h: host doubles (already multiplied by `up`, as resample_poly does before upfirdn)
-int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const double* h, int nh, float2* out,
-                    long long* n_out) {
-    ResampleGeo g;
-    TRY(resample_geo(mix.n, up_in, down_in, nh, &g));
-    if (mix.n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", mix.n);
-    if (n_out) *n_out = g.n_out;
-    if (g.up == 1 && g.down == 1) {           // resample_poly returns a copy
-        return mix_device(c, mix, out);
-    }
-    ResampleParams rp{};
-    rp.mix = mix;
+// The geometry, shared-memory check and polyphase table of one resample CTA (resample_kernel and
+// rec_resample_kernel).  h: host doubles (already multiplied by `up`, as resample_poly does before upfirdn).
+int resample_table(Ctx* c, const ResampleGeo& g, const double* h, int nh, ResampleParams* out, size_t* smem_out) {
+    ResampleParams& rp = *out;
     rp.up = g.up; rp.down = g.down; rp.nh = nh;
     rp.n_pre_pad = g.n_pre_pad; rp.n_pre_remove = g.n_pre_remove; rp.tpp = g.tpp;
     rp.n_out = g.n_out;
@@ -1279,7 +1273,6 @@ int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const 
     mixin(h, (size_t)nh * sizeof(double));
     mixin(&g.up, sizeof(int));
     mixin(&g.down, sizeof(int));
-    TRY(c->fe_ends.ensure(2 * sizeof(float2)));
     if (key != c->fe_hp_key || !c->fe_hp.p) {
         std::vector<float> hp((size_t)g.up * g.tpp, 0.f);
         for (int k = g.n_pre_pad; k < g.n_pre_pad + nh; ++k) hp[(size_t)(k % g.up) * g.tpp + k / g.up] = (float)h[k - g.n_pre_pad];
@@ -1289,6 +1282,24 @@ int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const 
         c->fe_hp_key = key;
     }
     rp.hp = c->fe_hp.as<float>();
+    *smem_out = smem;
+    return PRC_OK;
+}
+
+int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const double* h, int nh, float2* out,
+                    long long* n_out) {
+    ResampleGeo g;
+    TRY(resample_geo(mix.n, up_in, down_in, nh, &g));
+    if (mix.n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", mix.n);
+    if (n_out) *n_out = g.n_out;
+    if (g.up == 1 && g.down == 1) {           // resample_poly returns a copy
+        return mix_device(c, mix, out);
+    }
+    ResampleParams rp{};
+    size_t smem = 0;
+    TRY(resample_table(c, g, h, nh, &rp, &smem));
+    rp.mix = mix;
+    TRY(c->fe_ends.ensure(2 * sizeof(float2)));
     rp.ends = c->fe_ends.as<float2>();
     static std::atomic<bool> attr_set[64];
     if (!attr_set[c->device].exchange(true))
@@ -1299,6 +1310,37 @@ int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const 
         resample_kernel<<<ceil_div(g.n_out, RS_THREADS), RS_THREADS, smem, c->stream>>>(rp, out);
     }
     return check_launch("resample_kernel");
+}
+
+// resample_device on nchunks chunks of mix.n samples each, chunk b at raw sample b * chunk_stride of mix.in, mixed
+// with phase offset po[b] (device doubles), its output at out + b * out_stride (recording.cuh)
+int frontend_chunks_device(Ctx* c, const MixParams& mix, int nchunks, long long chunk_stride, const double* po,
+                           int up_in, int down_in, const double* h, int nh, float2* out, long long out_stride) {
+    ResampleGeo g;
+    TRY(resample_geo(mix.n, up_in, down_in, nh, &g));
+    rec::ChunkParams p{};
+    p.rs.mix = mix;
+    p.rs.n_out = g.n_out;
+    p.chunk_bytes = (long long)iq_bytes(mix.kind, chunk_stride);
+    p.out_stride = out_stride;
+    p.po = po;
+    p.nchunks = nchunks;
+    if (g.up == 1 && g.down == 1) {           // resample_poly returns a copy
+        ProfScope ps(c, K_FRONTEND_CHUNKS);
+        rec::launch_mix(p, out, c->stream);
+        return check_launch("rec_mix_kernel");
+    }
+    size_t smem = 0;
+    TRY(resample_table(c, g, h, nh, &p.rs, &smem));
+    TRY(c->fe_cends.ensure((size_t)nchunks * 2 * sizeof(float2)));
+    p.ends = c->fe_cends.as<float2>();
+    static std::atomic<bool> attr_set[64];
+    if (!attr_set[c->device].exchange(true)) CU(rec::allow_smem((int)SMEM_LIMIT));
+    {
+        ProfScope ps(c, K_FRONTEND_CHUNKS);
+        rec::launch_resample(p, smem, out, c->stream);
+    }
+    return check_launch("rec_resample_kernel");
 }
 
 // ---- CFAR_2D (detect.cuh) -----------------------------------------------------------------------
@@ -2716,6 +2758,58 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
     long long n_out = 0;
     TRY(resample_device(c, make_mix(din, in_kind, n, mode, fc, fs, phase_offset), up, down, h, nh, dout, &n_out));
     if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, (size_t)n_out * sizeof(float2), flags));
+    return finish(c, flags);
+}
+
+int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks, int64_t chunk_stride, int mode,
+                            double fc, double fs, const double* phase_offsets, int up, int down, const double* h, int nh,
+                            prc_c64* out, int64_t out_stride, int64_t out_capacity, int mem_kind, int device,
+                            void* stream, unsigned flags) {
+    if (!in || !out || !h || !phase_offsets) return fail(PRC_E_INVALID, "in/out/h/phase_offsets must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    if (nchunks < 1 || nchunks > 65535) return fail(PRC_E_INVALID, "nchunks=%d outside [1, 65535]", nchunks);
+    if (nchunks > 1 && chunk_stride < 0) return fail(PRC_E_INVALID, "chunk_stride=%lld invalid", (long long)chunk_stride);
+    if (in_kind < IQ_C64 || in_kind > IQ_I16) return fail(PRC_E_INVALID, "in_kind=%d invalid", in_kind);
+    if (mode < MIX_NONE || mode > MIX_FS64) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
+    if (mode != MIX_NONE && !(fs != 0.0)) return fail(PRC_E_INVALID, "fs must not be 0");
+    ResampleGeo g;
+    TRY(resample_geo(n, up, down, nh, &g));
+    if (nchunks > 1 && out_stride < g.n_out)
+        return fail(PRC_E_INVALID, "out_stride=%lld smaller than the %lld samples of one chunk", (long long)out_stride, g.n_out);
+    const long long ostride = nchunks > 1 ? out_stride : g.n_out;
+    const long long cstride = nchunks > 1 ? chunk_stride : n;
+    const long long need = (long long)(nchunks - 1) * ostride + g.n_out;
+    if (out_capacity < need) return fail(PRC_E_INVALID, "out holds %lld samples, %lld needed", (long long)out_capacity, need);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    const void* din = in;
+    float2* dout = reinterpret_cast<float2*>(out);
+    long long dstride = ostride;
+    if (mem_kind == PRC_MEM_HOST) {
+        const size_t in_bytes = iq_bytes(in_kind, (long long)(nchunks - 1) * cstride + n);
+        TRY(c->fe_in.ensure(in_bytes));
+        TRY(c->fe_out.ensure((size_t)nchunks * g.n_out * sizeof(float2)));
+        TRY(h2d(c, c->fe_in.p, in, in_bytes, flags));
+        din = c->fe_in.p;
+        dout = c->fe_out.as<float2>();
+        dstride = g.n_out;
+    }
+    // copied out of the caller's memory before the call returns: the transfer below is from pageable memory this
+    // function owns, which the runtime stages before cudaMemcpyAsync returns, so it is safe under PRC_FLAG_ASYNC even
+    // when the caller's array is page-locked and goes away right after the call
+    const std::vector<double> po(phase_offsets, phase_offsets + nchunks);
+    TRY(c->fe_po.ensure((size_t)nchunks * sizeof(double)));
+    CU(cudaMemcpyAsync(c->fe_po.p, po.data(), (size_t)nchunks * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    TRY(frontend_chunks_device(c, make_mix(din, in_kind, n, mode, fc, fs, 0.0), nchunks, cstride, c->fe_po.as<double>(),
+                               up, down, h, nh, dout, dstride));
+    if (mem_kind == PRC_MEM_HOST) {
+        if (ostride == g.n_out) TRY(d2h(c, out, dout, (size_t)nchunks * g.n_out * sizeof(float2), flags));
+        else
+            for (int b = 0; b < nchunks; ++b)
+                TRY(d2h(c, out + (size_t)b * ostride, dout + (size_t)b * g.n_out, (size_t)g.n_out * sizeof(float2), flags));
+    }
     return finish(c, flags);
 }
 

@@ -1,7 +1,8 @@
 """Frame pipeline: streams of CPI frames through  LS_Filter -> fast_xambg  on one H100.
 
-The reference processes one dask chunk (= one CPI frame) per task on a thread pool
-(``main.py:169-194``).  On the GPU the same independence is used differently: a
+The reference processes one dask chunk per task on a thread pool (``main.py:169-194``); with ``overlap_cpi`` on, the
+shipped setting, a CPI frame is a chunk plus a quarter CPI of each neighbour (``passiveradar_b200.recording`` builds
+those frames).  This pipeline takes frames that are already whole.  On the GPU the same independence is used differently: a
 ``FramePipeline`` owns ``nslots`` CUDA streams, each with its own device buffers and
 libprcore workspace, and issues batch ``b`` of ``batch`` frames on slot ``b % nslots`` through
 ``prc_frames_c64`` (one launch of each kernel per batch).  Host->device copies, the kernels of

@@ -129,3 +129,77 @@ def offset_pair(n1, n2, kind="int8", delay=0, seed=5):
     if kind == "uint8":
         return (s1 + 128).astype(np.uint8), (s2 + 128).astype(np.uint8)
     raise ValueError(f"unknown offset-pair kind {kind!r}")
+
+
+def recording(n, fs, fo, up, dn, *, delay, fd, channel_delay=0, multipath=0.3, clutter=True, kind="int8", seed=23):
+    """Seeded two-channel raw recording of one FM-like illuminator for the recording chain (main.py:44-194): ``(ref,
+    srv)`` interleaved I/Q of ``n`` complex samples each at the input rate ``fs``.
+
+    The illuminator is complex noise low-passed to 0.4 of the IF rate ``fs * up / dn`` and sits at ``-fo``, where
+    ``frequency_shift(x, fo, fs)`` brings it to 0 Hz.  ``srv`` holds the direct path (gain 1), one zero-Doppler multipath
+    echo of gain ``multipath`` ``up / gcd(up, dn)`` IF samples late and one target ``delay`` IF samples late with Doppler ``fd`` Hz
+    (gain 0.05), plus independent receiver noise on each channel.  Delays are whole input samples, so ``delay`` must be a multiple of ``up / gcd(up, dn)``.  ``srv`` lags ``ref`` by ``channel_delay`` input
+    samples (``ref[j]`` and ``srv[j + channel_delay]`` see the same instant; find_channel_offset on the raw arrays gives
+    ``-2 * channel_delay``).  ``clutter=False`` leaves the direct path and the multipath out of ``srv``.  ``kind`` is
+    ``int8`` or ``int16``."""
+    from scipy.signal import fftconvolve, firwin
+    g = np.gcd(up, dn)
+    up, dn = up // g, dn // g
+    if delay % up:
+        raise ValueError(f"delay must be a multiple of {up} IF samples")
+    d_in, m_in = delay // up * dn, dn
+    rng = np.random.default_rng(seed)
+    lead = d_in + m_in + abs(channel_delay) + 1
+    total = n + lead + abs(channel_delay)
+    h = firwin(257, 0.4 * up / dn)
+    u = fftconvolve(white_iq(rng, total + 256).astype(np.complex128), h, mode="valid")[:total]
+    u *= np.exp(-2j * np.pi * (fo / fs) * np.arange(total))
+    t = np.arange(total)
+    echo = np.zeros(total, np.complex128)
+    echo[m_in:] += multipath * u[:total - m_in]
+    tgt = np.zeros(total, np.complex128)
+    tgt[d_in:] = 0.05 * u[:total - d_in]
+    scene = (u + echo if clutter else 0) + tgt * np.exp(2j * np.pi * (fd / fs) * t)
+    r0 = lead
+    s0 = lead - channel_delay
+    ref = u[r0:r0 + n] + 0.02 * white_iq(rng, n)
+    srv = scene[s0:s0 + n] + 0.02 * white_iq(rng, n)
+    scale, top = (24.0, 127) if kind == "int8" else (2000.0, 32767)
+    dt = {"int8": np.int8, "int16": np.int16}[kind]
+
+    def raw(x):
+        x = x / np.sqrt(np.mean(np.abs(u) ** 2)) * scale
+        iq = np.empty(2 * n)
+        iq[0::2], iq[1::2] = x.real, x.imag
+        return np.clip(np.round(iq), -top, top).astype(dt)
+
+    return raw(ref), raw(srv)
+
+
+# main.py geometries for the recording chain: what the reference's getConfiguration derives from PRconfig.yaml
+# ("shipped"), and from it with channel_bandwidth 50 kHz, cpi_seconds_nominal 1, max_doppler_nominal 64 and
+# max_range_nominal 300 ("fast")
+RECORDING_CONFIGS = {
+    "shipped": {'cpi_samples': 524288, 'resamp_up': 13, 'resamp_dn': 119, 'input_sample_rate': 2400000,
+                'offset_freq': 100000, 'IF_sample_rate': 262184.87394957984, 'input_chunk_length': 4799250,
+                'window_overlap': 131072, 'num_range_cells': 175, 'num_doppler_cells': 1024, 'num_frames': 1200,
+                'overlap_cpi': True, 'interleaved_input_channels': False, 'frame_interval': 0.9998441025641025,
+                'range_cell_width': 1.1434679487179487, 'doppler_cell_width': 0.5000779608718487},
+    "fast": {'cpi_samples': 65536, 'resamp_up': 8, 'resamp_dn': 293, 'input_sample_rate': 2400000,
+             'offset_freq': 100000, 'IF_sample_rate': 65529.01023890785, 'input_chunk_length': 2400256,
+             'window_overlap': 16384, 'num_range_cells': 66, 'num_doppler_cells': 128, 'num_frames': 1200,
+             'overlap_cpi': True, 'interleaved_input_channels': False, 'frame_interval': 0.5000533333333333,
+             'range_cell_width': 4.575072916666667, 'doppler_cell_width': 0.9998933447098975},
+}
+
+
+def recording_for(config, nchunks, channel_delay=0, clutter=True, seed=1):
+    """``recording`` sized so that main.py makes exactly ``nchunks`` chunks of ``config`` from it (no channel offset),
+    with the target 3 * resamp_up IF samples late at 40 Doppler cells.  Returns (ref, srv, delay, doppler_cells)."""
+    icl = config["input_chunk_length"]
+    up, dn = config["resamp_up"], config["resamp_dn"]
+    n = nchunks * icl // 2 + 40 + abs(channel_delay)
+    fd = 40 * config["doppler_cell_width"]
+    ref, srv = recording(n, config["input_sample_rate"], config["offset_freq"], up, dn, delay=3 * up, fd=fd,
+                         channel_delay=channel_delay, clutter=clutter, seed=seed)
+    return ref, srv, 3 * up, 40
