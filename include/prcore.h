@@ -226,7 +226,7 @@ int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int
 
 /* ---- run-time switches (also read once from the environment: PRC_FFT, PRC_FFT_MIN_N) ----------------
  *   "fft"        1 (default): LS correlations, clutter FIR and CAF block sums as FFT-domain block correlations
- *                (csrc/fftcorr.cuh);  0: direct form on wgmma / FP32 (csrc/toepcorr.cuh, firtc.cuh, lagstream.cuh)
+ *                (csrc/fftcorr.cuh);  0: FP32 direct form (csrc/lagstream.cuh, kernels.cuh)
  *   "fft_min_n"  smallest channel length the FFT-domain path takes (default 8192)
  *   "caf_wave"   1: the FFT-domain CAF kernel runs one wave of CTAs, each walking several Doppler blocks (default 0)
  *   "frame_onepass"  1 (default): prc_frames_c64 / prc_frame_c64 on the FFT-domain path form the LS lag sums and the
@@ -235,10 +235,7 @@ int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int
  *                caf_fft_kernel.  Acceptance and results within float32 round-off are the same either way.
  * Read-only (prc_get_option only; prc_set_option returns PRC_E_INVALID): the environment switches of INTEGRATION.md
  * section 6, latched once per process, so a caller can check which kernel variants are in force:
- *   "tma" (PRC_TMA), "tma_l2" (PRC_TMA_L2), "tc" (PRC_TC), "tc_caf" (PRC_TC_CAF), "tc_fir" (PRC_TC_FIR),
  *   "tune_nchunk" (PRC_TUNE_NCHUNK, -1 = automatic), "tune_g" (PRC_TUNE_G, -1 = automatic);
- *   "tma_active"  1 when toepcorr_kernel uses TMA producers: "tma" is 1 and the driver has cuTensorMapEncodeTiled
- *                 (0: the cp.async loader warps)
  *   "fft_ctas_ls", "fft_ctas_fir", "fft_ctas_caf"  CTAs per SM of lscorr_fft_kernel, fir_fft_kernel and the fused
  *                 caf_fft_kernel at L = 2048 on the calling thread's current device, as the runtime's occupancy
  *                 calculator gives it for the launch configuration: the number their one-wave grids are sized from

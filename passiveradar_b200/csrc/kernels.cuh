@@ -286,18 +286,8 @@ struct FirParams {
     int M;
     int Mpad;     // multiple of TK
     int peek;
-    // optional: BF16 planes of the cleaned channel for the tensor-core CAF, cafs[(i + caf_off) mod' ...]:
-    // plane[q] = out[(q - caf_off) mod n] for q < caf_slen (interleaved re/im, three planes)
-    uint16_t* cafs[3];
-    long long caf_off, caf_slen;
     int linear;   // 1: ref[j] = 0 for j < 0 instead of wrapping (np.convolve of LS_Filter_Toeplitz)
 };
-
-__device__ __forceinline__ uint16_t fir_bf16_rn(float v) {
-    uint32_t u = __float_as_uint(v);
-    u += 0x7FFFu + ((u >> 16) & 1u);
-    return (uint16_t)(u >> 16);
-}
 
 // FFMA2 with the (t, t) operand pairs built in registers (slide_mac2n: fewest shared-memory bytes per MAC)
 template <int TK, int TO>
@@ -356,26 +346,7 @@ __global__ void __launch_bounds__(512) fir_apply_kernel(const __grid_constant__ 
         const long long i = i0 + v;
         if (i < p.n) {
             const float2 d = p.srv[i];
-            const float2 o = make_float2(d.x - acc[v].x, d.y - acc[v].y);
-            p.out[i] = o;
-            if (p.cafs[0]) {
-                uint32_t c[3];
-                float rr = o.x, ri = o.y;
-#pragma unroll
-                for (int pl = 0; pl < 3; ++pl) {
-                    const uint16_t br = fir_bf16_rn(rr), bi = fir_bf16_rn(ri);
-                    rr -= __uint_as_float((uint32_t)br << 16);
-                    ri -= __uint_as_float((uint32_t)bi << 16);
-                    c[pl] = (uint32_t)br | ((uint32_t)bi << 16);
-                }
-                const long long q1 = i + p.caf_off, q2 = i - (p.n - p.caf_off);
-#pragma unroll
-                for (int pl = 0; pl < 3; ++pl) {
-                    uint32_t* dst = reinterpret_cast<uint32_t*>(p.cafs[pl]);
-                    if (q1 < p.caf_slen) dst[q1] = c[pl];
-                    if (q2 >= 0 && q2 < p.caf_slen) dst[q2] = c[pl];
-                }
-            }
+            p.out[i] = make_float2(d.x - acc[v].x, d.y - acc[v].y);
         }
     }
 }
@@ -618,8 +589,8 @@ struct DopplerParams {
     int HT;
     int blk_len;             // stream layout (lagstream_kernel): rows actually written for block j =
     long long per_cta;       //   stream_pieces(j, blk_len, per_cta); per_cta == 0: all nchunk rows
-    // optional boundary sample of every Doppler block (tensor-core CAF: the GEMM covers D of the D+1
-    // samples of a block, the last one, i = j*bstride + boff, is added here)
+    // optional boundary sample of every Doppler block, i = j*bstride + boff, added to its lag sums
+    // (bx == nullptr: none; every launch in prcore.cu leaves it null)
     const float2* bx;
     const float2* bs;
     const float* bwin;       // optional: bx is the unweighted reference, multiply by bwin[i]

@@ -23,8 +23,6 @@
 #include "prcore.h"
 #include "kernels.cuh"
 #include "lagstream.cuh"
-#include "toepcorr.cuh"
-#include "firtc.cuh"
 #include "frontend.cuh"
 #include "detect.cuh"
 #include "nlms_block.cuh"
@@ -123,17 +121,11 @@ struct Ctx {
     bool own_stream = false;
     int nsm = 148;
     std::mutex mu;
-    DBuf firb[3];             // Wm^T planes of the tensor-core FIR
     DBuf fe_in, fe_mid, fe_out, fe_hp, fe_ends;    // front end: raw IQ, mixed, resampled, polyphase taps, end points
     DBuf fe_po, fe_cends;                          // front end over chunks: phase offsets, end points of every chunk
     DBuf cf_in, cf_cr, cf_det, cf_part;            // CFAR_2D
     uint64_t fe_hp_key = 0;                        // which taps fe_hp holds
-    // tensor maps of the last LS / CAF launch of this context: the planes live in DBufs, so the operand addresses
-    // repeat from frame to frame and the nine cuTensorMapEncodeTiled calls per launch are paid once
-    struct MapCache { bool valid = false; const void* ptr[9] = {nullptr}; int nk = 0, npass = 0; tc::ToepMaps maps; } map_cache[2];
     DBuf rs, clean2;          // LS_Filter_Toeplitz: rolled / frequency-shifted reference, ping-pong output
-    DBuf cafplane[6];         // bf16 planes of the tensor-core CAF: x[3], s[3]
-    DBuf tcplane[9];          // bf16 planes of the tensor-core path: x[3], s0[3], s1[3]
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
         nl_init, nl_taps, gal_k, gal_h;
     DBuf svd_part, svd_cr, svd_ws, svd_taps, svd_rank;   // LS_Filter_SVD: lag-sum partials, c / rhs, A and Z
@@ -153,9 +145,6 @@ struct Ctx {
     std::vector<ProfRec> recs;
     void release() {
         cudaSetDevice(device);
-        for (DBuf& b : tcplane) b.release();
-        for (DBuf& b : cafplane) b.release();
-        for (DBuf& b : firb) b.release();
         rs.release();
         clean2.release();
         for (DBuf& b : fft_tw) b.release();
@@ -182,12 +171,7 @@ std::vector<Ctx*> g_all_ctx;
 std::atomic<bool> g_attrs_set[64];
 std::atomic<uint64_t> g_epoch{1};                      // bumped by prc_shutdown
 int g_tune_nchunk = -1, g_tune_g = -1;
-int g_tma_l2 = 2;          // CUtensorMapL2promotion: 0 none, 1 64B, 2 128B, 3 256B (PRC_TMA_L2)
-int g_tma = 1;             // TMA (cp.async.bulk.tensor) producers for the wgmma kernels (PRC_TMA=0: 16-byte cp.async loaders)
-int g_tc_fir = 1;          // tensor-core path for the clutter FIR (PRC_TC_FIR=0: FP32 fir_apply_kernel)
-int g_tc_caf = 1;          // tensor-core path for the CAF block sums as well (PRC_TC_CAF=0: FP32 lagstream)
-int g_tc = 1;              // wgmma Toeplitz-GEMM for the LS correlations (PRC_TC=0: FP32 lagstream kernel)
-std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: wgmma / FP32 direct form
+std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: FP32 direct form
 std::atomic<int> g_fft_min_n{8192};   // ... for channels of at least this many samples (PRC_FFT_MIN_N)
 std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks instead of one CTA per block
 std::atomic<int> g_frame_onepass{1};  // FFT-domain frame: LS lag sums and CAF block spectra in one pass (framepass.cuh); 0: two passes
@@ -222,11 +206,6 @@ thread_local TlsCtx g_tls;
 void read_env() {
     if (const char* e = getenv("PRC_TUNE_NCHUNK")) g_tune_nchunk = atoi(e);
     if (const char* e = getenv("PRC_TUNE_G")) g_tune_g = atoi(e);
-    if (const char* e = getenv("PRC_TC")) g_tc = atoi(e);
-    if (const char* e = getenv("PRC_TC_CAF")) g_tc_caf = atoi(e);
-    if (const char* e = getenv("PRC_TC_FIR")) g_tc_fir = atoi(e);
-    if (const char* e = getenv("PRC_TMA")) g_tma = atoi(e);
-    if (const char* e = getenv("PRC_TMA_L2")) g_tma_l2 = atoi(e);
     if (const char* e = getenv("PRC_FFT")) g_fft.store(atoi(e));
     if (const char* e = getenv("PRC_FFT_MIN_N")) g_fft_min_n.store(atoi(e));
 }
@@ -235,11 +214,6 @@ int set_kernel_attrs(int device) {
     if (g_attrs_set[device].load()) return PRC_OK;
     const int lim = (int)SMEM_LIMIT;
     CU(cudaFuncSetAttribute(lagcorr_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(tc::firtc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(tc::toepcorr_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(tc::toepcorr_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(tc::toepcorr_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
-    CU(cudaFuncSetAttribute(tc::toepcorr_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(lagstream_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(fir_apply_kernel<TILE_I, TILE_D>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
     CU(cudaFuncSetAttribute(levinson_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim));
@@ -426,100 +400,6 @@ int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo
 
 void launch_lagstream(dim3 grid, int threads, size_t smem, cudaStream_t st, const LagStreamParams& sp) {
     lagstream_kernel<TILE_I, TILE_D><<<grid, threads, smem, st>>>(sp);
-}
-
-// ---- tensor maps (TMA).  cuTensorMapEncodeTiled is a host-only driver call, resolved through the runtime
-// (no link-time dependency on libcuda).
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode_tiled = nullptr;
-std::once_flag g_encode_once;
-
-void resolve_encode() {
-    std::call_once(g_encode_once, [] {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            g_encode_tiled = reinterpret_cast<EncodeTiledFn>(fn);
-    });
-}
-// TMA producers need the driver's tensor-map encoder; without it the cp.async loaders (same layout family,
-// same speed) are used
-bool use_tma() {
-    if (!g_tma) return false;
-    resolve_encode();
-    return g_encode_tiled != nullptr;
-}
-
-// BF16, 2-D: element (c0, c1) = base[c1 * stride_elems + c0]; rows may overlap (stride_elems < inner)
-int make_map_bf16(CUtensorMap* tm, const void* base, uint64_t inner, uint64_t rows, uint64_t stride_elems,
-                  uint32_t box_inner, uint32_t box_rows) {
-    resolve_encode();
-    if (!g_encode_tiled) return fail(PRC_E_CUDA, "cuTensorMapEncodeTiled is not available in this driver");
-    const cuuint64_t dims[2] = {inner, rows};
-    const cuuint64_t strides[1] = {stride_elems * 2};
-    const cuuint32_t box[2] = {box_inner, box_rows};
-    const cuuint32_t es[2] = {1, 1};
-    const CUresult r = g_encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
-                                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                                      (CUtensorMapL2promotion)g_tma_l2, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(PRC_E_CUDA, "cuTensorMapEncodeTiled failed (CUresult %d)", (int)r);
-    return PRC_OK;
-}
-
-// maps of the Toeplitz-GEMM operands: x rows are 128 elements, s rows 256 * npass elements wide, both 128 apart
-int make_toep_maps(const tc::ToepParams& tp, tc::ToepMaps* m) {
-    const uint64_t rows = (uint64_t)tp.nk * tc::KSTEP;
-    for (int k = 0; k < tc::NPLANE; ++k) {
-        TRY(make_map_bf16(&m->x[k], tp.x[k], tc::ROW, rows, tc::ROW, 64, tc::KSTEP));
-        for (int pr = 0; pr < 2; ++pr)
-            TRY(make_map_bf16(&m->s[pr][k], tp.s[pr][k], (uint64_t)tp.npass * tc::NPASS, rows, tc::ROW, 64, tc::KSTEP));
-    }
-    return PRC_OK;
-}
-
-// cached variant: slot 0 = LS, slot 1 = CAF
-int cached_toep_maps(Ctx* c, int slot, const tc::ToepParams& tp, const tc::ToepMaps** out) {
-    Ctx::MapCache& mc = c->map_cache[slot];
-    const void* ptr[9];
-    for (int k = 0; k < 3; ++k) { ptr[k] = tp.x[k]; ptr[3 + k] = tp.s[0][k]; ptr[6 + k] = tp.s[1][k]; }
-    bool same = mc.valid && mc.nk == tp.nk && mc.npass == tp.npass;
-    for (int k = 0; same && k < 9; ++k) same = mc.ptr[k] == ptr[k];
-    if (!same) {
-        mc.valid = false;
-        TRY(make_toep_maps(tp, &mc.maps));
-        for (int k = 0; k < 9; ++k) mc.ptr[k] = ptr[k];
-        mc.nk = tp.nk; mc.npass = tp.npass;
-        mc.valid = true;
-    }
-    *out = &mc.maps;
-    return PRC_OK;
-}
-
-// Tensor-core CAF eligibility and geometry (shared by the frame pipeline, which lets the LS stage's prep
-// and FIR kernels write the CAF operands while the data is in registers, and by xambg_device)
-struct CafTc {
-    bool on = false;
-    long long D = 0, nx = 0, slen = 0;
-    int npass = 0, ht = 0;
-    bool planes_ready = false;    // x and s planes already written by the LS stage
-};
-
-CafTc caf_tc_plan(const Ctx* c, long long n, int R, int F, bool has_taps) {
-    CafTc t;
-    if (!g_tc || !g_tc_caf || has_taps || F < 1) return t;
-    const long long D = n / F;
-    if (D < 1024 || D % 1024 != 0) return t;
-    t.npass = ceil_div(2 * (64 + R + 1), tc::NPASS);
-    t.ht = ceil_div(R + 1, 2) * 2;
-    if ((long long)F * t.npass < c->nsm || tc::toep_smem_bytes(t.ht) > SMEM_LIMIT) return t;
-    t.on = true;
-    t.D = D;
-    t.nx = (long long)F * D;
-    t.slen = t.nx + (long long)t.npass * 128;
-    return t;
 }
 
 // --------------------------------------------------------------------------- FFT-domain path (fftcorr.cuh)
@@ -757,8 +637,7 @@ int decimator_offset(long long ntaps, long long D) {   // resample_poly alignmen
 // [nf][L] for the transform length of caf_fft_plan(..., fuse_M)) exist on the FFT-domain path only; p_ready: the block
 // sums are already in c->fftP (one-pass frame), only the Doppler stage runs
 int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int R, int F,
-                 const float* win32, const float* dtaps32, long long ndtaps, float2* out,
-                 bool refw_ready = false, bool caf_planes_ready = false, Batch bt = Batch{},
+                 const float* win32, const float* dtaps32, long long ndtaps, float2* out, Batch bt = Batch{},
                  const float2* fuse_wp = nullptr, int fuse_M = 0, int fuse_peek = 0, bool p_ready = false) {
     if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
     if (F < 1 || R < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", F, R);
@@ -781,13 +660,10 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
     if (ntaps > (1ll << 30)) return fail(PRC_E_INVALID, "decimator too long");
     Geo g{};
     long long d_per_cta = 0;
-    const float2* bnd_x = nullptr;                  // boundary-sample correction of the tensor-core path
-    const float* bnd_w_all = nullptr;               // ... window to apply to bnd_x on the fly (bnd_x unweighted)
     const float2* dop_src = nullptr;                // Doppler-stage input when it is not c->partial
     const CafFftPlan fp = caf_fft_plan(n, R, F, ntaps, D, taps == nullptr && ntaps == D + 1, fuse_wp ? fuse_M : 0);
     if ((bt.nf > 1 || fuse_wp) && !fp.on && !p_ready)
         return fail(PRC_E_INVALID, "batched / fused CAF needs the FFT-domain path (n=%lld, F=%d, R=%d not eligible)", n, F, R);
-    const CafTc ct = (!p_ready && !fp.on && ntaps == D + 1 && c0 == D / 2) ? caf_tc_plan(c, n, R, F, taps != nullptr) : CafTc{};
     if (p_ready) {
         // ---- block sums already in c->fftP ([nf][F][HT], the one-pass frame's caf_combine_kernel): Doppler stage only
         g.nchunk = 1;
@@ -799,78 +675,12 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
         g.nchunk = 1;
         g.HT = fp.HT;
         dop_src = c->fftP.as<float2>();
-    } else if (ct.on) {
-        // ---- tensor-core CAF: one (Doppler block, pass) item per accumulation, persistent CTAs
-        // ref * window as complex64 is needed to build the x planes here; when the LS stage already wrote them
-        // (caf_planes_ready) only the F boundary samples use it, and those are weighted on the fly
-        const float2* xw = ref;
-        const float* bnd_w = nullptr;
-        if (win32 && refw_ready) {
-            xw = c->refw.as<float2>();
-        } else if (win32 && caf_planes_ready) {
-            bnd_w = win32;
-        } else if (win32) {
-            TRY(c->refw.ensure((size_t)n * sizeof(float2)));
-            {
-                ProfScope ps(c, K_MISC);
-                weight_kernel<<<ceil_div(n, 256), 256, 0, c->stream>>>(ref, win32, c->refw.as<float2>(), (int)n);
-            }
-            TRY(check_launch("weight_kernel"));
-            xw = c->refw.as<float2>();
-        }
-        for (int k = 0; k < 6; ++k) TRY(c->cafplane[k].ensure((size_t)(k < 3 ? ct.nx : ct.slen) * 2 * sizeof(uint16_t)));
-        TRY(c->partial.ensure((size_t)F * ct.npass * ct.ht * sizeof(float2)));
-        if (!caf_planes_ready) {
-            tc::PrepParams px{};
-            px.sig[0] = xw; px.sig[1] = xw;
-            px.dmin[0] = px.dmin[1] = -(int)(D / 2);
-            px.zero_outside[0] = px.zero_outside[1] = 1;
-            for (int k = 0; k < 3; ++k) px.plane[0][k] = px.plane[1][k] = c->cafplane[k].as<uint16_t>();
-            px.n = (int)n;
-            px.len = ct.nx;
-            tc::PrepParams py = px;
-            py.sig[0] = py.sig[1] = srv;
-            py.zero_outside[0] = py.zero_outside[1] = 0;
-            for (int k = 0; k < 3; ++k) py.plane[0][k] = py.plane[1][k] = c->cafplane[3 + k].as<uint16_t>();
-            py.len = ct.slen;
-            {
-                ProfScope ps(c, K_MISC);
-                tc::tc_prep_kernel<<<dim3(ceil_div(ct.nx, 1024), 1), 256, 0, c->stream>>>(px);
-                tc::tc_prep_kernel<<<dim3(ceil_div(ct.slen, 1024), 1), 256, 0, c->stream>>>(py);
-            }
-            TRY(check_launch("tc_prep_kernel(caf)"));
-        }
-        tc::ToepParams tp{};
-        for (int k = 0; k < 3; ++k) {
-            tp.x[k] = c->cafplane[k].as<uint16_t>();
-            tp.s[0][k] = tp.s[1][k] = c->cafplane[3 + k].as<uint16_t>();
-        }
-        tp.nk = (int)(ct.nx / 1024); tp.nlag = R + 1; tp.npass = ct.npass; tp.ranges = 0;
-        tp.kb = (int)(D / 1024); tp.nblk = F; tp.HT = ct.ht;
-        tp.partial = c->partial.as<float2>();
-        static const tc::ToepMaps no_maps{};
-        const tc::ToepMaps* mp = &no_maps;
-        const bool tma = use_tma();
-        if (tma) TRY(cached_toep_maps(c, 1, tp, &mp));
-        const tc::ToepMaps& maps = *mp;
-        {
-            ProfScope ps(c, K_LAGCORR_CAF);
-            if (tma) tc::toepcorr_kernel<false, true><<<c->nsm, tc::THREADS, tc::toep_smem_bytes(ct.ht), c->stream>>>(tp, maps);
-            else tc::toepcorr_kernel<false, false><<<c->nsm, tc::THREADS, tc::toep_smem_bytes(ct.ht), c->stream>>>(tp, maps);
-        }
-        TRY(check_launch("toepcorr_kernel(caf)"));
-        g.nchunk = ct.npass;
-        g.HT = ct.ht;
-        bnd_x = xw;
-        bnd_w_all = bnd_w;
     } else if (taps == nullptr && ntaps >= 64) {   // tiny Doppler blocks: one flush per block would dominate
         StreamGeo sg;
         TRY(choose_stream((int)ntaps, F, 1, R + 1, c->nsm, &sg));
         TRY(c->partial.ensure((size_t)F * sg.maxpieces * sg.HT * sizeof(float2)));
         const float2* xw = ref;
-        if (win32 && refw_ready) {
-            xw = c->refw.as<float2>();           // ref * window already written by the LS stage's prep kernel
-        } else if (win32) {
+        if (win32) {
             TRY(c->refw.ensure((size_t)n * sizeof(float2)));
             {
                 ProfScope ps(c, K_MISC);
@@ -943,7 +753,6 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
     d.partial_fstride = (long long)F * g.nchunk * g.HT;
     d.out_fstride = (long long)F * (R + 1);
     d.blk_len = (int)ntaps; d.per_cta = d_per_cta;
-    d.bx = bnd_x; d.bs = srv; d.bwin = bnd_x ? bnd_w_all : nullptr; d.bstride = D; d.boff = c0; d.n = (int)n;
     int logF = 0;
     while ((1 << logF) < F) ++logF;
     d.logF = logF;
@@ -978,11 +787,8 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
 // bt.nf > 1 (a batch of frames; taps_out then receives [nf][M]) and need_out == false (only the taps are wanted: the
 // caller applies them inside the CAF kernel) exist on the FFT-domain path only
 int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int filter_len, int peek,
-              double reg, float2* out, float2* taps_out, const float* win32 = nullptr, bool* refw_ready = nullptr,
-              CafTc* caf = nullptr, bool linear = false, Batch bt = Batch{}, bool need_out = true) {
+              double reg, float2* out, float2* taps_out, bool linear = false, Batch bt = Batch{}, bool need_out = true) {
     // linear: LS_Filter_Toeplitz semantics -- correlations and FIR treat ref/srv as zero outside [0, n)
-    if (refw_ready) *refw_ready = false;
-    bool caf_x_done = false;
     if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
     if (filter_len < 0 || peek < 0 || filter_len + peek < 1)
         return fail(PRC_E_INVALID, "filter_len=%d peek=%d invalid", filter_len, peek);
@@ -1000,126 +806,36 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
             CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)bt.nf * M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
         return PRC_OK;
     }
-    Geo g{};
-    bool use_fir_tc = false;
-    int lead = 0, fir_shift = 0, fir_kv = 0, fir_nblk = 0;
-    long long fir_zoff = 0;
     TRY(c->lstaps.ensure((size_t)M * sizeof(float2)));
     TRY(c->status.ensure(sizeof(int)));
-    const int tc_npass = ceil_div(2 * (64 + M), tc::NPASS);
-    const int tc_ranges = c->nsm / (2 * tc_npass);
-    const int tc_nk = ceil_div(n, 1024);
-    const int tc_ht = ceil_div(M, 2) * 2;
-    if (g_tc && tc_ranges >= 1 && tc_nk >= 2 * tc_ranges && tc::toep_smem_bytes(tc_ht) <= SMEM_LIMIT) {
-        // ---- tensor-core path: BF16x3 Toeplitz GEMM (toepcorr.cuh)
-        const long long nx = (long long)tc_nk * 1024;
-        long long slen = nx + (long long)tc_npass * 128;
-        const bool alias_x = (nx == n) || linear;    // x (zero tail) and s0 (circular tail) only differ beyond n
-        // tensor-core FIR geometry (firtc.cuh): the ref planes get a lead-in of `lead` samples so that the
-        // window of output row a starts at plane sample 64 a + lead - pre
-        const int fir_pre = std::max(0, ceil_div(M - 1 - peek, 4) * 4);
-        const int fir_lead = ceil_div(fir_pre, 64) * 64;
-        const int fir_kvp = ceil_div(2 * (64 + peek + fir_pre), 64) * 64;
-        const long long fir_rows = ceil_div(n, 64);
-        const int fir_grid = ceil_div(fir_rows, tc::FIR_ROWS);
-        use_fir_tc = g_tc_fir && fir_grid >= 32 && fir_kvp <= 64 * tc::FIR_MAX_ATOMS && tc::firtc_smem_bytes() <= SMEM_LIMIT;
-        lead = use_fir_tc ? fir_lead : 0;
-        if (use_fir_tc) {
-            fir_shift = peek + fir_pre;
-            fir_kv = fir_kvp;
-            fir_nblk = fir_grid;
-            fir_zoff = 2ll * (fir_lead - fir_pre);
-            slen = std::max(slen, ((long long)fir_grid * tc::FIR_ROWS + tc::FIR_MAX_ATOMS / 2 + 2) * 64);
-        }
-        for (int k = 0; k < 9; ++k) {
-            if (k < 3 && alias_x) continue;
-            TRY(c->tcplane[k].ensure((size_t)(k < 3 ? nx : slen + lead) * 2 * sizeof(uint16_t)));
-        }
-        TRY(c->partial.ensure((size_t)2 * tc_npass * tc_ranges * tc_ht * sizeof(float2)));
-        const bool fold = win32 != nullptr && refw_ready != nullptr;
-        if (fold) TRY(c->refw.ensure((size_t)n * sizeof(float2)));
-        {
-            ProfScope ps(c, K_MISC);
-            if (!alias_x)
-                tc::bf16_split_kernel<<<ceil_div(nx, 256), 256, 0, c->stream>>>(
-                    ref, (int)n, 0, c->tcplane[0].as<uint16_t>(), c->tcplane[1].as<uint16_t>(), c->tcplane[2].as<uint16_t>(), nx, n);
-            tc::PrepParams pp{};
-            pp.sig[0] = ref; pp.sig[1] = srv;
-            pp.dmin[0] = -lead; pp.dmin[1] = -peek;         // ref planes start `lead` samples early (FIR window)
-            pp.zero_outside[0] = pp.zero_outside[1] = linear ? 1 : 0;
-            for (int k = 0; k < 3; ++k) { pp.plane[0][k] = c->tcplane[3 + k].as<uint16_t>(); pp.plane[1][k] = c->tcplane[6 + k].as<uint16_t>(); }
-            pp.win = fold ? win32 : nullptr;
-            // the complex64 ref*window is only needed by the FP32 CAF; the tensor-core CAF takes its x planes (cafx)
-            const bool need_refw = fold && !(caf && caf->on);
-            pp.refw = need_refw ? c->refw.as<float2>() : nullptr;
-            pp.n = (int)n;
-            pp.len = slen + lead;
-            if (fold && caf && caf->on) {          // also emit the CAF x operand (ref * window, shifted by D/2)
-                for (int k = 0; k < 3; ++k) {
-                    TRY(c->cafplane[k].ensure((size_t)caf->nx * 2 * sizeof(uint16_t)));
-                    pp.cafx[k] = c->cafplane[k].as<uint16_t>();
-                }
-                pp.caf_off = caf->D / 2;
-                pp.caf_nx = caf->nx;
-                caf_x_done = true;
-            }
-            tc::tc_prep_kernel<<<dim3(ceil_div(slen + lead, 1024), 2), 256, 0, c->stream>>>(pp);
-        }
-        TRY(check_launch("tc_prep_kernel"));
-        if (fold && !(caf && caf->on)) *refw_ready = true;
-        tc::ToepParams tp{};
-        for (int k = 0; k < 3; ++k) {
-            tp.x[k] = alias_x ? c->tcplane[3 + k].as<uint16_t>() + 2 * lead : c->tcplane[k].as<uint16_t>();
-            tp.s[0][k] = c->tcplane[3 + k].as<uint16_t>() + 2 * lead;
-            tp.s[1][k] = c->tcplane[6 + k].as<uint16_t>();
-        }
-        tp.nk = tc_nk; tp.nlag = M; tp.npass = tc_npass; tp.ranges = tc_ranges; tp.HT = tc_ht;
-        tp.partial = c->partial.as<float2>();
-        static const tc::ToepMaps no_maps{};
-        const tc::ToepMaps* mp = &no_maps;
-        const bool tma = use_tma();
-        if (tma) TRY(cached_toep_maps(c, 0, tp, &mp));
-        const tc::ToepMaps& maps = *mp;
-        {
-            ProfScope ps(c, K_LAGCORR_LS);
-            if (tma) tc::toepcorr_kernel<true, true><<<2 * tc_npass * tc_ranges, tc::THREADS, tc::toep_smem_bytes(tc_ht), c->stream>>>(tp, maps);
-            else tc::toepcorr_kernel<true, false><<<2 * tc_npass * tc_ranges, tc::THREADS, tc::toep_smem_bytes(tc_ht), c->stream>>>(tp, maps);
-        }
-        TRY(check_launch("toepcorr_kernel"));
-        g.nchunk = tc_npass * tc_ranges;
-        g.HT = tc_ht;
-    } else {
-        StreamGeo sg;
-        TRY(choose_stream((int)n, 1, 2, M, c->nsm, &sg));
-        TRY(c->partial.ensure((size_t)2 * sg.maxpieces * sg.HT * sizeof(float2)));
-        LagStreamParams sp{};
-        sp.x = ref;
-        sp.s[0] = ref; sp.s[1] = srv;
-        sp.dmin[0] = 0; sp.dmin[1] = -peek;
-        sp.n = (int)n;
-        sp.blk_first_lo = 0;
-        sp.blk_stride = 0;
-        sp.blk_len = (int)n;
-        sp.nblk = 1;
-        sp.total = sg.total;
-        sp.per_cta = sg.per_cta;
-        sp.H = sg.H; sp.G = sg.G; sp.steps = sg.steps;
-        sp.maxpieces = sg.maxpieces;
-        sp.s_linear = linear ? 1 : 0;
-        sp.partial = c->partial.as<float2>();
-        {
-            ProfScope ps(c, K_LAGCORR_LS);
-            launch_lagstream(dim3(sg.ncta, 2), sg.threads, sg.smem, c->stream, sp);
-        }
-        TRY(check_launch("lagstream_kernel(ls)"));
-        g.nchunk = sg.maxpieces;      // == pieces of the single block == ncta
-        g.HT = sg.HT;
+    StreamGeo sg;
+    TRY(choose_stream((int)n, 1, 2, M, c->nsm, &sg));
+    TRY(c->partial.ensure((size_t)2 * sg.maxpieces * sg.HT * sizeof(float2)));
+    LagStreamParams sp{};
+    sp.x = ref;
+    sp.s[0] = ref; sp.s[1] = srv;
+    sp.dmin[0] = 0; sp.dmin[1] = -peek;
+    sp.n = (int)n;
+    sp.blk_first_lo = 0;
+    sp.blk_stride = 0;
+    sp.blk_len = (int)n;
+    sp.nblk = 1;
+    sp.total = sg.total;
+    sp.per_cta = sg.per_cta;
+    sp.H = sg.H; sp.G = sg.G; sp.steps = sg.steps;
+    sp.maxpieces = sg.maxpieces;
+    sp.s_linear = linear ? 1 : 0;
+    sp.partial = c->partial.as<float2>();
+    {
+        ProfScope ps(c, K_LAGCORR_LS);
+        launch_lagstream(dim3(sg.ncta, 2), sg.threads, sg.smem, c->stream, sp);
     }
+    TRY(check_launch("lagstream_kernel(ls)"));
 
     LevinsonParams lp{};
     lp.partial = c->partial.as<float2>();
-    lp.nchunk = g.nchunk;
-    lp.HT = g.HT;
+    lp.nchunk = sg.maxpieces;      // == pieces of the single block == ncta
+    lp.HT = sg.HT;
     lp.M = M;
     lp.reg = reg;
     lp.taps = c->lstaps.as<float2>();
@@ -1131,47 +847,8 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
     }
     TRY(check_launch("levinson_kernel"));
 
-    if (use_fir_tc) {
-        for (int k = 0; k < 3; ++k) TRY(c->firb[k].ensure((size_t)tc::FIR_N * fir_kv * sizeof(uint16_t)));
-        {
-            ProfScope ps(c, K_MISC);          // the taps-matrix builder is bookkeeping, not the FIR itself
-            tc::fir_bmat_kernel<<<ceil_div(tc::FIR_N * fir_kv, 256), 256, 0, c->stream>>>(
-                c->lstaps.as<float2>(), M, fir_shift, fir_kv, c->firb[0].as<uint16_t>(), c->firb[1].as<uint16_t>(), c->firb[2].as<uint16_t>());
-        }
-        {
-            ProfScope ps(c, K_FIR);
-            tc::FirTcParams ft{};
-            for (int k = 0; k < 3; ++k) { ft.z[k] = c->tcplane[3 + k].as<uint16_t>(); ft.b[k] = c->firb[k].as<uint16_t>(); }
-            ft.zoff = fir_zoff;
-            ft.kvp = fir_kv;
-            ft.srv = srv; ft.out = out; ft.n = (int)n;
-            if (caf && caf->on && caf_x_done) {
-                for (int k = 0; k < 3; ++k) {
-                    TRY(c->cafplane[3 + k].ensure((size_t)caf->slen * 2 * sizeof(uint16_t)));
-                    ft.cafs[k] = c->cafplane[3 + k].as<uint16_t>();
-                }
-                ft.caf_off = caf->D / 2;
-                ft.caf_slen = caf->slen;
-                caf->planes_ready = true;
-            }
-            tc::firtc_kernel<<<fir_nblk, tc::FIR_THREADS, tc::firtc_smem_bytes(), c->stream>>>(ft);
-        }
-        TRY(check_launch("firtc_kernel"));
-        if (taps_out)
-            CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
-        return PRC_OK;
-    }
     FirParams fp{};
     fp.ref = ref; fp.srv = srv; fp.taps = c->lstaps.as<float2>(); fp.out = out;
-    if (caf && caf->on && caf_x_done) {           // the FIR writes the CAF s operand (cleaned channel) as well
-        for (int k = 0; k < 3; ++k) {
-            TRY(c->cafplane[3 + k].ensure((size_t)caf->slen * 2 * sizeof(uint16_t)));
-            fp.cafs[k] = c->cafplane[3 + k].as<uint16_t>();
-        }
-        fp.caf_off = caf->D / 2;
-        fp.caf_slen = caf->slen;
-        caf->planes_ready = true;
-    }
     fp.n = (int)n; fp.M = M; fp.peek = peek;
     fp.linear = linear ? 1 : 0;
     fp.Mpad = ceil_div(M, TILE_I) * TILE_I;
@@ -1208,7 +885,7 @@ int ls_toeplitz_device(Ctx* c, const float2* ref, const float2* srv, long long n
                                                                                  1.0f / (float)fs, stride);
     }
     TRY(check_launch("shift_roll_kernel"));
-    return ls_device(c, c->rs.as<float2>(), srv, n, filter_len + peek, 0, 0.0, out, taps_out, nullptr, nullptr, nullptr, true, bt);
+    return ls_device(c, c->rs.as<float2>(), srv, n, filter_len + peek, 0, 0.0, out, taps_out, true, bt);
 }
 
 // ---- front end (frontend.cuh) -------------------------------------------------------------------
@@ -1692,8 +1369,7 @@ int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2
             fftc::launch_caf_combine(q, gc, nf, c->stream);
         }
         TRY(check_launch("caf_combine_kernel"));
-        TRY(xambg_device(c, r, s, n, R, F, win32, nullptr, 0, maps + (size_t)f0 * F * (R + 1), false, false, b, nullptr, 0, 0,
-                         true));
+        TRY(xambg_device(c, r, s, n, R, F, win32, nullptr, 0, maps + (size_t)f0 * F * (R + 1), b, nullptr, 0, 0, true));
     }
     if (taps_out)
         CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)bt.nf * M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
@@ -1713,26 +1389,22 @@ int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batc
     if (lf.on && cf.on) {
         // FFT-domain frame: lag sums -> Toeplitz solve -> taps spectrum -> CAF with the clutter filter applied to the
         // surveillance spectrum inside the kernel (the cleaned channel exists only if the caller asks for it)
-        TRY(ls_device(c, ref, srv, n, filter_len, peek, reg, cleaned_out, taps_out, nullptr, nullptr, nullptr, false, bt,
-                      cleaned_out != nullptr));
+        TRY(ls_device(c, ref, srv, n, filter_len, peek, reg, cleaned_out, taps_out, false, bt, cleaned_out != nullptr));
         TRY(taps_spectrum(c, cf.r3, M, bt.nf, &c->wp_caf));
-        return xambg_device(c, ref, srv, n, R, F, win32, nullptr, 0, maps, false, false, bt, c->wp_caf.as<float2>(), M, peek);
+        return xambg_device(c, ref, srv, n, R, F, win32, nullptr, 0, maps, bt, c->wp_caf.as<float2>(), M, peek);
     }
-    // direct-form kernels (wgmma / FP32), frame by frame
+    // FP32 direct-form kernels, frame by frame
     TRY(c->clean.ensure((size_t)n * sizeof(float2)));
     TRY(c->status.ensure((size_t)bt.nf * sizeof(int)));
     for (int fr = 0; fr < bt.nf; ++fr) {
         const float2* r = ref + (size_t)fr * bt.stride;
         const float2* sv = srv + (size_t)fr * bt.stride;
         float2* dclean = cleaned_out ? cleaned_out + (size_t)fr * bt.stride : c->clean.as<float2>();
-        bool refw_ready = false;
-        CafTc caf = (n / F) % 2 == 0 ? caf_tc_plan(c, n, R, F, false) : CafTc{};
         c->status_slot = fr;            // frame fr reports its Toeplitz-solve status in status[fr]
-        const int rc = ls_device(c, r, sv, n, filter_len, peek, reg, dclean, taps_out ? taps_out + (size_t)fr * M : nullptr, win32,
-                                 &refw_ready, &caf);
+        const int rc = ls_device(c, r, sv, n, filter_len, peek, reg, dclean, taps_out ? taps_out + (size_t)fr * M : nullptr);
         c->status_slot = 0;
         TRY(rc);
-        TRY(xambg_device(c, r, dclean, n, R, F, win32, nullptr, 0, maps + (size_t)fr * F * (R + 1), refw_ready, caf.planes_ready));
+        TRY(xambg_device(c, r, dclean, n, R, F, win32, nullptr, 0, maps + (size_t)fr * F * (R + 1)));
     }
     return PRC_OK;
 }
@@ -1875,7 +1547,6 @@ int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, 
 // switches latched from the environment once per process (read_env): readable by name (prc_get_option), never settable
 const int* env_switch(const std::string& k) {
     static const std::pair<const char*, const int*> kSwitches[] = {
-        {"tma", &g_tma}, {"tma_l2", &g_tma_l2}, {"tc", &g_tc}, {"tc_caf", &g_tc_caf}, {"tc_fir", &g_tc_fir},
         {"tune_nchunk", &g_tune_nchunk}, {"tune_g", &g_tune_g}};
     for (const auto& s : kSwitches)
         if (k == s.first) return s.second;
@@ -2485,7 +2156,7 @@ int prc_xambg_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
     const long long D = n / freq_bins;
     const bool batched = D >= 2 && caf_fft_plan(n, range_bins, freq_bins, D + 1, D, true, 0).on;
     if (batched || nframes == 1) {
-        TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, nullptr, 0, dout, false, false, bt));
+        TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, nullptr, 0, dout, bt));
     } else {
         for (int fr = 0; fr < nframes; ++fr)       // direct-form kernels, frame by frame
             TRY(xambg_device(c, dref + (size_t)fr * bt.stride, dsrv + (size_t)fr * bt.stride, n, range_bins, freq_bins, win32,
@@ -2583,7 +2254,7 @@ int prc_set_option(const char* name, int value) {
     else if (k == "fft_min_n") g_fft_min_n.store(value);
     else if (k == "caf_wave") g_caf_wave.store(value);
     else if (k == "frame_onepass") g_frame_onepass.store(value);
-    else if (env_switch(k) || k == "tma_active")
+    else if (env_switch(k))
         return fail(PRC_E_INVALID, "option '%s' is read-only (set from the environment when the library starts)", name);
     else if (fft_ctas_option(k) >= 0)
         return fail(PRC_E_INVALID, "option '%s' is read-only (CTAs per SM of the build's kernels on this device)", name);
@@ -2600,7 +2271,6 @@ int prc_get_option(const char* name, int* value) {
     else if (k == "caf_wave") *value = g_caf_wave.load();
     else if (k == "frame_onepass") *value = g_frame_onepass.load();
     else if (const int* s = env_switch(k)) *value = *s;
-    else if (k == "tma_active") *value = use_tma() ? 1 : 0;
     else if (fft_ctas_option(k) >= 0) {
         int dev = 0;
         CU(cudaGetDevice(&dev));

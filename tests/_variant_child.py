@@ -26,10 +26,7 @@ import _golden as G                      # noqa: E402
 from passiveradar_b200 import synth     # noqa: E402
 
 # prc_get_option name -> (environment variable, value when the variable is unset: prcore.cu's defaults)
-SWITCHES = {
-    "tma": ("PRC_TMA", 1), "tma_l2": ("PRC_TMA_L2", 2), "tc": ("PRC_TC", 1), "tc_caf": ("PRC_TC_CAF", 1),
-    "tc_fir": ("PRC_TC_FIR", 1), "tune_nchunk": ("PRC_TUNE_NCHUNK", -1), "tune_g": ("PRC_TUNE_G", -1),
-}
+SWITCHES = {"tune_nchunk": ("PRC_TUNE_NCHUNK", -1), "tune_g": ("PRC_TUNE_G", -1)}
 
 
 def expected_switches(env):
@@ -50,7 +47,7 @@ KAISER = ("kaiser", 5.0)
 
 def ls_items(case):
     """LS_Filter inputs: (item, profile, golden name or None, ref, srv, filter_len, reg, peek)."""
-    if case == "ls_big":          # n = 2**20, 310 taps: toepcorr_kernel<true, *>, firtc_kernel, levinson_kernel<1>
+    if case == "ls_big":          # n = 2**20, 310 taps: lagstream_kernel, levinson_kernel<1>, fir_apply_kernel
         for name in ("ls_c2_p1", "frame_c2_p0"):
             g = G.load(name)
             ref, srv = G.inputs(g)
@@ -62,7 +59,7 @@ def ls_items(case):
             g = G.load(name)
             ref, srv = G.inputs(g)
             yield name, str(g["profile"]), name, ref, srv, int(g["filter_len"]), float(g["reg"]), int(g["peek"])
-    elif case == "ls_wide":       # 1110 taps: levinson_kernel<4>; toepcorr's shared memory is exceeded, so FP32 kernels
+    elif case == "ls_wide":       # 1110 taps: levinson_kernel<4>
         for profile in ("P1", "P0"):
             ref, srv = synth.make_frame(2 ** 18, profile, frame=2)
             yield f"n262144_{profile}", profile, None, ref, srv, 1100, 1.0, 10
@@ -77,7 +74,7 @@ def toep_items():
 
 def caf_items(case):
     """fast_xambg inputs: (item, profile, golden or None, ref, srv, R, F, input_len, window, short_filt)."""
-    if case == "caf_big":         # D = 4096: toepcorr_kernel<false, *> (CAF), tc_prep_kernel, weight_kernel
+    if case == "caf_big":         # D = 4096: weight_kernel, lagstream_kernel (CAF)
         n = 2 ** 20
         ref, srv = synth.make_frame(n, "P0", frame=21)
         yield "n1048576", "P0", None, ref, srv, 300, 256, n, signal.get_window(KAISER, n), True
@@ -132,8 +129,8 @@ def run_caf(case, res):
 
 
 def run_frame(res):
-    """One frame through prc_frame_c64 (the entry point of FramePipeline): on the direct form the LS stage's prep and
-    FIR kernels write the operands of the tensor-core CAF."""
+    """One frame through prc_frame_c64 (the entry point of FramePipeline) on the direct form: the LS stage's kernels, then
+    the CAF of the cleaned channel against the reference weighted by weight_kernel."""
     from passiveradar_b200 import _lib
     g, ref, srv, n, R, F = frame_inputs()
     M = FRAME["filter_len"] + FRAME["peek"]
@@ -189,12 +186,11 @@ def main(argv):
     if got != want:
         raise SystemExit(f"the library reports switches {got}, the environment asks for {want}")
     from passiveradar_b200 import _lib
-    _lib.set_option("fft", 0)            # every case but NLMS is a direct-form (wgmma / FP32) case
+    _lib.set_option("fft", 0)            # every case but NLMS is a direct-form (FP32) case
     res = {}
     for case in cases:
         RUNNERS[case](res)
     res["switches"] = np.array([got[k] for k in SWITCHES], dtype=np.int64)
-    res["tma_active"] = np.int64(_lib.get_option("tma_active"))
     res["cases"] = np.array(cases)
     np.savez(out_path, **res)
     return 0

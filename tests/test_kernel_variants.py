@@ -6,9 +6,8 @@ Three parts:
   variant runs in a child process (tests/_variant_child.py) that saves its outputs; this process computes each oracle
   once and makes every comparison.  A variant's outputs are held to the float64 truth (1e-5) and to the
   reference-pinned oracle or golden (1e-5 + 1.2 x reference-vs-truth), as in tests/test_gpu_parity.py.  They are also
-  compared with the default child: the loader-only switches (PRC_TMA, PRC_TMA_L2) change how the same bytes reach
-  shared memory and must be bit-identical; the other switches change the arithmetic and are held to 3e-6 on
-  independent channels (P0), the bound tests/test_gpu_fft.py uses between arithmetics.
+  compared with the default child: the switches change the arithmetic and are held to 3e-6 on independent channels
+  (P0), the bound tests/test_gpu_fft.py uses between arithmetics.
 * In-process GPU cases for dispatches of the default configuration no other test reaches: NLMS with more than 1024
   taps, the Doppler stage at F = 4096 .. 16384, the tap-weighted decimator at full size, and caf_wave = 1.
 * A CPU guard: every kernel launch site of prcore.cu must appear in COVERAGE with the GPU tests that reach it.
@@ -41,15 +40,8 @@ DIRECT = ["ls_big", "ls_small", "ls_wide", "toep", "caf_big", "caf_small", "fram
 # variant -> (environment, cases it runs).  The switches only change the direct form.
 VARIANTS = {
     "default": ({}, DIRECT + ["nlms"]),
-    "tma0": ({"PRC_TMA": "0"}, DIRECT),                     # cp.async loader warps of toepcorr_kernel (driver fallback)
-    "tma_l2_0": ({"PRC_TMA_L2": "0"}, DIRECT),              # L2 promotion hint of the tensor maps only
-    "tma_l2_3": ({"PRC_TMA_L2": "3"}, DIRECT),
-    "tc0": ({"PRC_TC": "0"}, DIRECT),                       # lagstream for LS and CAF, fir_apply
-    "tc_caf0": ({"PRC_TC_CAF": "0"}, DIRECT),               # tensor-core LS, lagstream CAF at D % 1024 == 0
-    "tc_fir0": ({"PRC_TC_FIR": "0"}, DIRECT),               # fir_apply writes the tensor-core CAF's s planes
-    "tune": ({"PRC_TC": "0", "PRC_TUNE_NCHUNK": "1", "PRC_TUNE_G": "1"}, DIRECT),  # one chunk / group per problem
+    "tune": ({"PRC_TUNE_NCHUNK": "1", "PRC_TUNE_G": "1"}, DIRECT),  # one chunk / group per problem
 }
-LOADER_ONLY = ("tma0", "tma_l2_0", "tma_l2_3")
 _ENV_NAMES = {var for var, _ in VC.SWITCHES.values()} | {"PRC_FFT", "PRC_FFT_MIN_N"}
 
 
@@ -289,8 +281,6 @@ def test_variant_matches_truth_and_reference(variant, variant_outputs, oracles):
     assert list(res["cases"]) == cases
     echo = dict(zip(VC.SWITCHES, res["switches"].tolist()))
     assert echo == VC.expected_switches(env), echo
-    # the H100's driver has cuTensorMapEncodeTiled: only PRC_TMA=0 selects the cp.async loaders
-    assert int(res["tma_active"]) == (0 if env.get("PRC_TMA") == "0" else 1)
     for case in cases:
         fig = {}
         _check(case, res, oracles, fig)
@@ -304,43 +294,39 @@ def test_variant_matches_default_child(variant, variant_outputs):
     keys = [k for k in res if k.count(".") == 3]
     assert keys and all(k in base for k in keys)
     worst = 0.0
-    if variant in LOADER_ONLY:
-        # the loaders write the same shared-memory image; the MMA order is unchanged
-        for k in keys:
-            assert np.array_equal(res[k], base[k]), k
-    else:
-        for k in keys:
-            if k.split(".")[2] != "P0":
-                continue                 # strong clutter: what is left after ~55 dB of cancellation, held to the truth only
-            e = G.rel_inf(res[k], base[k])
-            worst = max(worst, e)
-            assert e <= XVAR, (k, e)
+    for k in keys:
+        if k.split(".")[2] != "P0":
+            continue                     # strong clutter: what is left after ~55 dB of cancellation, held to the truth only
+        e = G.rel_inf(res[k], base[k])
+        worst = max(worst, e)
+        assert e <= XVAR, (k, e)
     record_parity(f"variants/{variant}/vs_default", E=worst)
 
 
 # ------------------------------------------------------------------ switch echo (no GPU needed)
 def test_switch_echo_reports_the_environment():
-    env = {"PRC_TUNE_G": "2", "PRC_TC": "0", "PRC_TMA": "0"}
+    env = {"PRC_TUNE_G": "2", "PRC_TUNE_NCHUNK": "3"}
     got = json.loads(_run_child(["--switches"], env, timeout=300))
-    assert (got["tune_g"], got["tc"], got["tma"]) == (2, 0, 0)
+    assert (got["tune_g"], got["tune_nchunk"]) == (2, 3)
     assert got == VC.expected_switches(env)
     defaults = json.loads(_run_child(["--switches"], {}, timeout=300))
-    assert defaults == {"tma": 1, "tma_l2": 2, "tc": 1, "tc_caf": 1, "tc_fir": 1, "tune_nchunk": -1, "tune_g": -1}
+    assert defaults == {"tune_nchunk": -1, "tune_g": -1}
 
 
-@pytest.mark.parametrize("name", list(VC.SWITCHES) + ["tma_active"])
+@pytest.mark.parametrize("name", list(VC.SWITCHES))
 def test_environment_switches_are_read_only(name):
     lib = _lib.load()
     assert lib.prc_set_option(name.encode(), 1) == _lib.PRC_E_INVALID
     assert b"read-only" in lib.prc_last_error()
-    if name != "tma_active":             # resolving the TMA encoder needs a driver
-        assert _lib.get_option(name) == VC.expected_switches(os.environ)[name]
+    assert _lib.get_option(name) == VC.expected_switches(os.environ)[name]
 
 
-@pytest.mark.parametrize("name", ["stream", "packed", "tile", "nlms_block"])
+@pytest.mark.parametrize("name", ["stream", "packed", "tile", "nlms_block", "tma", "tma_l2", "tc", "tc_caf", "tc_fir",
+                                  "tma_active"])
 def test_retired_switches_are_unknown_options(name):
-    """PRC_STREAM, PRC_PACKED, PRC_TILE and PRC_NLMS_BLOCK are no longer read; their option names are unknown, not
-    read-only, so a library that still kept one of them fails here."""
+    """The environment switches INTEGRATION.md section 6 lists as no longer read, and "tma_active", which reported the
+    loader the "tma" switch selected: their option names are unknown, not read-only, so a library that still kept one
+    of them fails here."""
     lib = _lib.load()
     with pytest.raises(_lib.PrcoreError):
         _lib.get_option(name)
@@ -507,7 +493,7 @@ PS = "tests/test_path_sweep.py::"
 VARIANT_TEST = KV + "test_variant_matches_truth_and_reference"
 COVERAGE = {
     "launch_lagstream: lagstream_kernel<TILE_I, TILE_D>": [(PAR + "test_ls_matches_live_oracle", "direct", "LS, n <= 20000"),
-                                                           (VARIANT_TEST, "tc0", "LS and CAF at config 2")],
+                                                           (VARIANT_TEST, "default", "ls_big, caf_big, frame: LS and CAF at config 2")],
     "fft_twiddles: fft::fft_twiddle_kernel<R3>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 (n = 200000) and 8 (n = 10**6)"),
         (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
@@ -540,13 +526,8 @@ COVERAGE = {
         (FFT + "test_xambg_large_shapes_sampled_columns", "fft", "R3 = 8 (F = 64, D >= 16384)"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16 (R = 1200)"),
         (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
-    "xambg_device: weight_kernel": [(VARIANT_TEST, "default", "tensor-core CAF, caf_big"),
+    "xambg_device: weight_kernel": [(VARIANT_TEST, "default", "caf_big, frame"),
                                     (PAR + "test_xambg_matches_live_oracle", "direct", "lagstream CAF with a window")],
-    "xambg_device: tc::tc_prep_kernel": [(VARIANT_TEST, "default", "caf_big"),
-                                         (FFT + "test_xambg_large_shapes_sampled_columns", "direct", "D = 1024 .. 65536")],
-    "xambg_device: tc::toepcorr_kernel<false, true>": [(VARIANT_TEST, "default", "caf_big, frame"),
-                                                       (FFT + "test_xambg_large_shapes_sampled_columns", "direct", "")],
-    "xambg_device: tc::toepcorr_kernel<false, false>": [(VARIANT_TEST, "tma0", "caf_big, frame: cp.async loaders")],
     "xambg_device: lagcorr_kernel<TILE_I, TILE_D>": [
         (VARIANT_TEST, "default", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
         (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps")],
@@ -561,19 +542,12 @@ COVERAGE = {
                                        (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
     "xambg_device: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
                                          (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
-    "ls_device: tc::bf16_split_kernel": [(FFT + "test_ls_config4_size_and_readme_shape", "direct", "n = 10**6, not a multiple of 1024")],
-    "ls_device: tc::tc_prep_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
-    "ls_device: tc::toepcorr_kernel<true, true>": [(VARIANT_TEST, "default", "ls_big, frame"),
-                                                   (PAR + "test_ls_matches_reference_golden", "direct", "ls_c2_p1")],
-    "ls_device: tc::toepcorr_kernel<true, false>": [(VARIANT_TEST, "tma0", "ls_big, frame: cp.async loaders")],
     "ls_device: levinson_kernel<1>": [(VARIANT_TEST, "default", "ls_big, ls_small"),
                                       (PAR + "test_ls_matches_live_oracle", "direct", "")],
     "ls_device: levinson_kernel<4>": [(VARIANT_TEST, "default", "ls_wide"),
                                       (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", "")],
-    "ls_device: tc::fir_bmat_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
-    "ls_device: tc::firtc_kernel": [(VARIANT_TEST, "default", "ls_big, frame")],
     "ls_device: fir_apply_kernel<TILE_I, TILE_D>": [(VARIANT_TEST, "default", "ls_small, ls_wide, toep"),
-                                                    (VARIANT_TEST, "tc_fir0", "frame: writes the tensor-core CAF's s planes")],
+                                                    (VARIANT_TEST, "default", "ls_big, frame at config 2")],
     "ls_toeplitz_device: shift_roll_kernel": [(VARIANT_TEST, "default", "toep"),
                                               (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins")],
     "mix_device: iq_mix_kernel": [
@@ -661,7 +635,7 @@ def _is_gpu_test(test_id):
 
 def test_every_launch_site_has_a_covering_gpu_test():
     sites = launch_sites()
-    assert len(sites) == 55
+    assert len(sites) == 46
     missing = sorted(set(sites) - set(COVERAGE))
     stale = sorted(set(COVERAGE) - set(sites))
     assert not missing, "launch sites of prcore.cu without a covering test in COVERAGE: " + \
