@@ -54,7 +54,10 @@ typedef struct prc_c64 { float re, im; } prc_c64;
 #define PRC_FLAG_ASYNC        1u   /* do not synchronise `stream` before returning */
 #define PRC_FLAG_WINDOW_F32   2u   /* `window` points at float, not double */
 #define PRC_FLAG_ABS_C64      4u   /* prc_cfar2d_f32: `x` is a complex64 map, |x| is used */
-#define PRC_FLAG_MAP_F64      8u   /* tracker entry points: maps are float64, not float32 */
+#define PRC_FLAG_MAP_F64      8u   /* tracker entry points, prc_persistence_frames: maps are float64, not float32 */
+#define PRC_FLAG_CR_F64      16u   /* prc_cfar2d_frames: cr_out receives the float64 CR, not its float32 rounding */
+#define PRC_FLAG_PROD_F32    32u   /* prc_persistence_frames: float32 products float32(x) * float32(w) */
+#define PRC_FLAG_ORIENT      64u   /* prc_persistence_frames: frames are written as fliplr(P.T) */
 
 /* ---- lifecycle / diagnostics ------------------------------------------------ */
 int         prc_version(void);
@@ -308,6 +311,34 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
  */
 int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const float* thresh, float* cr_out,
                    uint8_t* det_out, int mem_kind, int device, void* stream, unsigned flags);
+
+/* ---- the frame chain of range_doppler_plot.py:45-85 -------------------------------------------------------------
+ * prc_cfar2d_frames: CFAR_2D(x[b], fw, gw) for b < nframes in one launch; map b at x + b*frame_stride elements (float32,
+ *   or complex64 with PRC_FLAG_ABS_C64), its CR at cr_out + b*cr_stride elements: float32, bit-identical to a
+ *   prc_cfar2d_f32 call on that map, or with PRC_FLAG_CR_F64 the float64 value that call rounds.  Limits and
+ *   messages are prc_cfar2d_f32's; nframes <= 65535, strides >= rows*cols when nframes > 1.
+ * prc_persistence_frames: persistence() of reference passiveRadar/plotting_tools.py:9-30 along the frame axis.  x holds
+ *   n_carry carried frames followed by nframes new ones (frame f at x + f*frame_stride, rows x cols, float32 or float64
+ *   with PRC_FLAG_MAP_F64); out receives, for every new frame k, P[k] = sum_{i < min(k+1, hold)} X[k-i] * weights[i]
+ *   with k counted from the first carried frame, summed from +0.0 in the order i = 0, 1, ...  A stream continues across
+ *   calls when the last min(k, hold-1) input frames are carried.  weights: min(hold, n_carry+nframes) host doubles
+ *   (decay**i as the caller's Python computes it), copied before the call returns.  PRC_FLAG_PROD_F32 forms the
+ *   products in float32 (a float32 stack and a float32 or Python-float decay under NumPy 2 promotion), else float64.
+ *   out: nframes frames of rows*cols doubles, each P[k] (rows x cols) or, with PRC_FLAG_ORIENT, fliplr(P[k].T)
+ *   (cols x rows).  Requires hold >= 1 and 0 <= n_carry <= hold-1.
+ * prc_percentiles_frames: np.percentile(frame, q[j]) (linear method) of nframes float64 frames of n values (frame b
+ *   at x + b*frame_stride), times scale[j] when scale is not NULL: out[b*nq + j].  1 <= n <= 2 147 483 135,
+ *   1 <= nq <= 4, 0 <= q[j] <= 100;
+ *   q and scale are host doubles.  Bit-identical to NumPy; a frame holding NaN gives NaN.  -0.0 and +0.0 rank as
+ *   equal, and a statistic that falls on either is returned as +0.0.
+ */
+int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int fw, int gw,
+                      void* cr_out, int64_t cr_stride, int mem_kind, int device, void* stream, unsigned flags);
+int prc_persistence_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int n_carry, int hold,
+                           const double* weights, double* out, int mem_kind, int device, void* stream, unsigned flags);
+int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t frame_stride, const double* q,
+                           const double* scale, int nq, double* out, int mem_kind, int device, void* stream,
+                           unsigned flags);
 
 /* ---- Kalman target trackers ------------------------------------------------------------------------
  * Replace get_measurements(), multitarget_tracker() and simple_target_tracker(), reference

@@ -19,12 +19,14 @@ from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, s
                                multitarget_tracker_frames, simple_tracker_frames, cfar_track,
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
 from .recording import RecordingPipeline                                     # noqa: F401
+from .plotting_tools import persistence, persistence_frames, RenderPipeline  # noqa: F401
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
            "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
            "find_channel_offset", "offset_compensation", "shift", "xcorr", "CFAR_2D",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
-           "simple_tracker_frames", "cfar_track", "RecordingPipeline"]
+           "simple_tracker_frames", "cfar_track", "RecordingPipeline", "persistence", "persistence_frames",
+           "RenderPipeline"]
 __version__ = "0.1.0"
 
 
@@ -51,6 +53,8 @@ def install(reference_package: str = "passiveRadar"):
                              "multitarget_tracker": multitarget_tracker, "simple_target_tracker": simple_target_tracker},
         "clutter_removal": {"LS_Filter": LS_Filter, "NLMS_filter": NLMS_filter,
                             "LS_Filter_Toeplitz": LS_Filter_Toeplitz, "LS_Filter_Multiple": LS_Filter_Multiple},
+        # the reference's plotting_tools imports matplotlib: skipped like any optional module that does not import
+        "plotting_tools": {"persistence": persistence},
     }
     for modname, attrs in table.items():
         try:

@@ -27,6 +27,9 @@ FLAG_ASYNC = 1
 FLAG_WINDOW_F32 = 2
 FLAG_ABS_C64 = 4
 FLAG_MAP_F64 = 8
+FLAG_CR_F64 = 16
+FLAG_PROD_F32 = 32
+FLAG_ORIENT = 64
 IQ_C64, IQ_I8, IQ_I16 = 0, 1, 2
 MIX_NONE, MIX_C64, MIX_C128, MIX_F64, MIX_FS64 = 0, 1, 2, 3, 4
 DT_I8, DT_U8, DT_I16, DT_F32, DT_F64, DT_C64, DT_C128 = 0, 1, 2, 3, 4, 5, 6
@@ -91,6 +94,12 @@ SIGNATURES = {
                                           C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_cfar2d_f32": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_cfar2d_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                    C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_persistence_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
+                                         C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_percentiles_frames": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_get_measurements_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
                                               C.c_double, C.c_double, C.c_int64, C.c_void_p, C.c_void_p,
                                               C.c_int, C.c_int, C.c_void_p, C.c_uint]),

@@ -33,6 +33,7 @@
 #include "lssvd.cuh"
 #include "framepass.cuh"
 #include "recording.cuh"
+#include "render.cuh"
 
 namespace {
 
@@ -51,12 +52,14 @@ std::atomic<uint64_t> g_launches{0};
 // optional per-kernel timing (prc_profile_*): CUDA events on the launching stream around each launch
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
-                K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_COUNT };
+                K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_CFAR_FRAMES, K_PERSISTENCE,
+                K_PERCENTILE, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
                                            "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
-                                           "caf_combine", "frontend_chunks"};
+                                           "caf_combine", "frontend_chunks", "cfar_frames",
+                                           "persistence", "percentile"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -124,6 +127,7 @@ struct Ctx {
     DBuf fe_in, fe_mid, fe_out, fe_hp, fe_ends;    // front end: raw IQ, mixed, resampled, polyphase taps, end points
     DBuf fe_po, fe_cends;                          // front end over chunks: phase offsets, end points of every chunk
     DBuf cf_in, cf_cr, cf_det, cf_part;            // CFAR_2D
+    DBuf rd_in, rd_out, rd_part, rd_w;             // frame chain of range_doppler_plot.py: maps, results, CFAR partial sums, weights
     uint64_t fe_hp_key = 0;                        // which taps fe_hp holds
     DBuf rs, clean2;          // LS_Filter_Toeplitz: rolled / frequency-shifted reference, ping-pong output
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
@@ -150,7 +154,8 @@ struct Ctx {
         for (DBuf& b : fft_tw) b.release();
         for (bool& r : fft_tw_ready) r = false;
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP, &fpacc}) b->release();
-        for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part}) b->release();
+        for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part,
+                        &rd_in, &rd_out, &rd_part, &rd_w}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
                         &trk_slots, &trk_out, &trk_cnt, &svd_part, &svd_cr, &svd_ws, &svd_taps, &svd_rank})
@@ -1057,6 +1062,44 @@ int cfar_device(Ctx* c, const void* x, bool is_complex, int rows, int cols, int 
     }
     cfar2d_kernel<<<dim3(ceil_div(cols, CFAR_TX), ceil_div(rows, CFAR_TY)), dim3(CFAR_TX, CFAR_TY), smem, c->stream>>>(p);
     return check_launch("cfar2d_kernel");
+}
+
+// ---- frame chain of range_doppler_plot.py:45-85 (render.cuh) --------------------------------------------------------
+// CFAR_2D's limits, messages and window geometry, as cfar_device sets them
+int cfar_window(int rows, int cols, int fw, int gw, CfarParams* p) {
+    if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
+    if (rows > CFAR_MAX_ROWS)
+        return fail(PRC_E_INVALID, "rows=%d exceed the CFAR maximum of %d rows", rows, CFAR_MAX_ROWS);
+    if (fw < 1 || fw > CFAR_MAX_FW) return fail(PRC_E_INVALID, "fw=%d outside [1, %d]", fw, CFAR_MAX_FW);
+    if (gw < 0 || fw * fw - gw * gw == 0) return fail(PRC_E_INVALID, "fw=%d gw=%d: fw^2 - gw^2 must not be 0", fw, gw);
+    *p = CfarParams{};
+    p->rows = rows; p->cols = cols; p->fw = fw;
+    int e1 = (fw - gw) >= 0 ? (fw - gw) / 2 : -((gw - fw + 1) / 2);
+    int e2 = fw - e1 + 1;
+    if (e1 < 0) e1 = std::max(0, e1 + fw);
+    p->e1 = std::min(e1, fw); p->e2 = std::min(std::max(e2, 0), fw);
+    p->c = (fw - 1) / 2;
+    p->scale = 1.0 / ((double)fw * fw - (double)gw * gw);
+    return PRC_OK;
+}
+
+int cfar_frames_device(Ctx* c, rdr::CfarFramesParams& f, int nframes) {
+    TRY(c->rd_part.ensure((size_t)nframes * CFAR_MEAN_CTAS * sizeof(double)));
+    f.partial = c->rd_part.as<double>();
+    {   // under a lock: a concurrent first call must not launch before the attribute is set
+        static std::mutex attr_mu;
+        static bool attr_set[64];
+        std::lock_guard<std::mutex> g(attr_mu);
+        if (!attr_set[c->device]) {
+            CU(rdr::allow_smem((int)SMEM_LIMIT));
+            attr_set[c->device] = true;
+        }
+    }
+    {
+        ProfScope ps(c, K_CFAR_FRAMES);
+        rdr::launch_cfar(f, nframes, c->stream);
+    }
+    return check_launch("cfar_frames_kernel");
 }
 
 // ---- direct_xambg (reference range_doppler_processing.py:93-124) ---------------------------------
@@ -2510,6 +2553,163 @@ int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const floa
         if (cr_out) TRY(d2h(c, cr_out, dcr, cells * sizeof(float), flags));
         if (det_out) TRY(d2h(c, det_out, ddet, cells, flags));
     }
+    return finish(c, flags);
+}
+
+int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int fw, int gw,
+                      void* cr_out, int64_t cr_stride, int mem_kind, int device, void* stream, unsigned flags) {
+    if (!x || !cr_out) return fail(PRC_E_INVALID, "x and cr_out must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    rdr::CfarFramesParams f{};
+    TRY(cfar_window(rows, cols, fw, gw, &f.p));
+    if (nframes < 0 || nframes > 65535) return fail(PRC_E_INVALID, "nframes=%d outside [0, 65535]", nframes);
+    const long long cells = (long long)rows * cols;
+    if (nframes > 1 && (frame_stride < cells || cr_stride < cells))
+        return fail(PRC_E_INVALID, "frame_stride=%lld / cr_stride=%lld smaller than the %lld cells of a map",
+                    (long long)frame_stride, (long long)cr_stride, cells);
+    const bool cplx = (flags & PRC_FLAG_ABS_C64) != 0, f64 = (flags & PRC_FLAG_CR_F64) != 0;
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (nframes == 0) return finish(c, flags);
+    const size_t ine = cplx ? sizeof(float2) : sizeof(float), oute = f64 ? sizeof(double) : sizeof(float);
+    f.p.x = x;
+    f.p.is_complex = cplx ? 1 : 0;
+    f.frame_stride = nframes > 1 ? frame_stride : cells;
+    f.cr = cr_out;
+    f.cr_stride = nframes > 1 ? cr_stride : cells;
+    f.cr_f64 = f64 ? 1 : 0;
+    if (mem_kind == PRC_MEM_HOST) {            // staged frame after frame, compact
+        TRY(c->rd_in.ensure((size_t)nframes * cells * ine));
+        TRY(c->rd_out.ensure((size_t)nframes * cells * oute));
+        for (int b = 0; b < nframes; ++b)
+            TRY(h2d(c, c->rd_in.as<char>() + (size_t)b * cells * ine,
+                    static_cast<const char*>(x) + (size_t)b * f.frame_stride * ine, cells * ine, flags));
+        f.p.x = c->rd_in.p;
+        f.frame_stride = cells;
+        f.cr = c->rd_out.p;
+        f.cr_stride = cells;
+    }
+    TRY(cfar_frames_device(c, f, nframes));
+    if (mem_kind == PRC_MEM_HOST) {
+        const long long os = nframes > 1 ? cr_stride : cells;
+        for (int b = 0; b < nframes; ++b)
+            TRY(d2h(c, static_cast<char*>(cr_out) + (size_t)b * os * oute, c->rd_out.as<char>() + (size_t)b * cells * oute,
+                    cells * oute, flags));
+    }
+    return finish(c, flags);
+}
+
+int prc_persistence_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int n_carry, int hold,
+                           const double* weights, double* out, int mem_kind, int device, void* stream, unsigned flags) {
+    if (!x || !out || !weights) return fail(PRC_E_INVALID, "x/weights/out must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
+    if ((rows + rdr::PST_TY - 1) / rdr::PST_TY > 65535)
+        return fail(PRC_E_INVALID, "rows=%d exceed the persistence maximum of %d rows", rows, 65535 * rdr::PST_TY);
+    if (hold < 1) return fail(PRC_E_INVALID, "hold=%d must be >= 1", hold);
+    if (nframes < 0) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (n_carry < 0 || n_carry > hold - 1)
+        return fail(PRC_E_INVALID, "n_carry=%d outside [0, hold - 1 = %d]", n_carry, hold - 1);
+    const long long cells = (long long)rows * cols;
+    const int total = n_carry + nframes;
+    if (total > 1 && frame_stride < cells)
+        return fail(PRC_E_INVALID, "frame_stride=%lld smaller than the %lld cells of a map", (long long)frame_stride, cells);
+    const bool f64 = (flags & PRC_FLAG_MAP_F64) != 0, prod32 = (flags & PRC_FLAG_PROD_F32) != 0;
+    if (f64 && prod32) return fail(PRC_E_INVALID, "float32 products need a float32 stack (PRC_FLAG_MAP_F64 is set)");
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (nframes == 0) return finish(c, flags);
+    // the weights a call uses (min(hold, frames)) are copied out of the caller's memory before the call returns, as
+    // prc_frontend_chunks_c64 does with its phase offsets
+    const int nw = std::min(hold, total);
+    const std::vector<double> w(weights, weights + nw);
+    TRY(c->rd_w.ensure((size_t)nw * sizeof(double)));
+    CU(cudaMemcpyAsync(c->rd_w.p, w.data(), (size_t)nw * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    rdr::PersistParams p{};
+    const size_t ine = f64 ? sizeof(double) : sizeof(float);
+    p.x = x;
+    p.frame_stride = total > 1 ? frame_stride : cells;
+    p.f64 = f64 ? 1 : 0;
+    p.f32prod = prod32 ? 1 : 0;
+    p.oriented = (flags & PRC_FLAG_ORIENT) ? 1 : 0;
+    p.rows = rows; p.cols = cols;
+    p.n_carry = n_carry; p.nframes = nframes; p.hold = hold;
+    p.w = c->rd_w.as<double>();
+    p.out = out;
+    const size_t ob = (size_t)nframes * cells * sizeof(double);
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->rd_in.ensure((size_t)total * cells * ine));
+        TRY(c->rd_out.ensure(ob));
+        for (int b = 0; b < total; ++b)
+            TRY(h2d(c, c->rd_in.as<char>() + (size_t)b * cells * ine,
+                    static_cast<const char*>(x) + (size_t)b * p.frame_stride * ine, cells * ine, flags));
+        p.x = c->rd_in.p;
+        p.frame_stride = cells;
+        p.out = c->rd_out.as<double>();
+    }
+    {
+        ProfScope ps(c, K_PERSISTENCE);
+        rdr::launch_persistence(p, c->stream);
+    }
+    TRY(check_launch("pst_kernel"));
+    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, p.out, ob, flags));
+    return finish(c, flags);
+}
+
+int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t frame_stride, const double* q,
+                           const double* scale, int nq, double* out, int mem_kind, int device, void* stream,
+                           unsigned flags) {
+    if (!x || !out || !q) return fail(PRC_E_INVALID, "x/q/out must not be NULL");
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (n < 1 || n > rdr::PCT_MAX_N) return fail(PRC_E_INVALID, "n=%lld outside [1, %d]", (long long)n, rdr::PCT_MAX_N);
+    if (nq < 1 || nq > rdr::PCT_MAX_Q) return fail(PRC_E_INVALID, "nq=%d outside [1, %d]", nq, rdr::PCT_MAX_Q);
+    if (nframes < 0) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (nframes > 1 && frame_stride < n)
+        return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    rdr::PctParams p{};
+    p.n = (int)n;
+    p.nq = nq;
+    for (int j = 0; j < nq; ++j) {
+        if (!(q[j] >= 0.0 && q[j] <= 100.0)) return fail(PRC_E_INVALID, "q[%d]=%g outside [0, 100]", j, q[j]);
+        // np.percentile on float64 data, linear method: v = (n - 1) * (q / 100.0); order statistics floor(v) and
+        // floor(v) + 1, gamma = v - floor(v).  From v >= n - 1 on both are the maximum and NumPy's gamma is v + 1.
+        const double v = (double)(n - 1) * (q[j] / 100.0);
+        if (v >= (double)(n - 1)) {
+            p.k[j] = (int)(n - 1);
+            p.g[j] = v + 1.0;
+        } else {
+            p.k[j] = (int)std::floor(v);
+            p.g[j] = v - std::floor(v);
+        }
+        p.scale[j] = scale ? scale[j] : 1.0;
+    }
+    p.has_scale = scale ? 1 : 0;
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (nframes == 0) return finish(c, flags);
+    p.x = x;
+    p.frame_stride = nframes > 1 ? frame_stride : n;
+    p.out = out;
+    const size_t ob = (size_t)nframes * nq * sizeof(double);
+    if (mem_kind == PRC_MEM_HOST) {
+        TRY(c->rd_in.ensure((size_t)nframes * n * sizeof(double)));
+        TRY(c->rd_out.ensure(ob));
+        for (int b = 0; b < nframes; ++b)
+            TRY(h2d(c, c->rd_in.as<double>() + (size_t)b * n, x + (size_t)b * p.frame_stride, (size_t)n * sizeof(double),
+                    flags));
+        p.x = c->rd_in.as<double>();
+        p.frame_stride = n;
+        p.out = c->rd_out.as<double>();
+    }
+    {
+        ProfScope ps(c, K_PERCENTILE);
+        rdr::launch_percentiles(p, nframes, c->stream);
+    }
+    TRY(check_launch("pct_kernel"));
+    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, p.out, ob, flags));
     return finish(c, flags);
 }
 
