@@ -124,7 +124,7 @@ struct Ctx {
     bool own_stream = false;
     int nsm = 148;
     std::mutex mu;
-    DBuf fe_in, fe_mid, fe_out, fe_hp, fe_ends;    // front end: raw IQ, mixed, resampled, polyphase taps, end points
+    DBuf fe_in, fe_out, fe_hp, fe_ends;            // front end: raw IQ, resampled, polyphase taps, end points
     DBuf fe_po, fe_cends;                          // front end over chunks: phase offsets, end points of every chunk
     DBuf cf_in, cf_cr, cf_det, cf_part;            // CFAR_2D
     DBuf rd_in, rd_out, rd_part, rd_w;             // frame chain of range_doppler_plot.py: maps, results, CFAR partial sums, weights
@@ -154,7 +154,7 @@ struct Ctx {
         for (DBuf& b : fft_tw) b.release();
         for (bool& r : fft_tw_ready) r = false;
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP, &fpacc}) b->release();
-        for (DBuf* b : {&fe_in, &fe_mid, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part,
+        for (DBuf* b : {&fe_in, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part,
                         &rd_in, &rd_out, &rd_part, &rd_w}) b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
@@ -1269,27 +1269,101 @@ int d2h(Ctx* c, void* dst, const void* src, size_t bytes, unsigned flags) {
     return PRC_OK;
 }
 
+// ---- arguments and operands of the C entry points
+bool bad_mem_kind(int k) { return k != PRC_MEM_HOST && k != PRC_MEM_DEVICE; }
+
+// The checks of an entry point that takes ref / srv stacks, made before any CUDA call.  `names` names the three
+// operands in the message; range_bins / freq_bins are the CAF's (the defaults pass).  *bt (when given): the frames and
+// the caller's stride between them.
+int stack_args(const void* a, const void* b, const void* o, const char* names, int mem_kind, long long n, int nframes,
+               long long frame_stride, Batch* bt, int range_bins = 0, int freq_bins = 1) {
+    if (!a || !b || !o) return fail(PRC_E_INVALID, "%s must not be NULL", names);
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", n);
+    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", frame_stride, n);
+    if (freq_bins < 1 || range_bins < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", freq_bins, range_bins);
+    if (bt) {
+        bt->nf = nframes;
+        bt->stride = nframes > 1 ? frame_stride : n;
+    }
+    return PRC_OK;
+}
+
+// The checks the front-end entry points share, made before any CUDA call
+int frontend_args(int mem_kind, long long n, int in_kind, int mode, double fs) {
+    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
+    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", n);
+    if (in_kind < IQ_C64 || in_kind > IQ_I16) return fail(PRC_E_INVALID, "in_kind=%d invalid", in_kind);
+    if (mode < MIX_NONE || mode > MIX_FS64) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
+    if (mode != MIX_NONE && !(fs != 0.0)) return fail(PRC_E_INVALID, "fs must not be 0");
+    return PRC_OK;
+}
+
+// `rows` rows of `row_bytes`: the host side's rows are `stride` bytes apart, the device side's packed.  One copy when
+// the host rows are contiguous, one per row otherwise.
+int rows_h2d(Ctx* c, void* dst, const void* src, size_t rows, size_t row_bytes, size_t stride, unsigned flags) {
+    if (rows == 1 || stride == row_bytes) return h2d(c, dst, src, rows * row_bytes, flags);
+    for (size_t r = 0; r < rows; ++r)
+        TRY(h2d(c, static_cast<char*>(dst) + r * row_bytes, static_cast<const char*>(src) + r * stride, row_bytes, flags));
+    return PRC_OK;
+}
+
+int rows_d2h(Ctx* c, void* dst, const void* src, size_t rows, size_t row_bytes, size_t stride, unsigned flags) {
+    if (rows == 1 || stride == row_bytes) return d2h(c, dst, src, rows * row_bytes, flags);
+    for (size_t r = 0; r < rows; ++r)
+        TRY(d2h(c, static_cast<char*>(dst) + r * stride, static_cast<const char*>(src) + r * row_bytes, row_bytes, flags));
+    return PRC_OK;
+}
+
+// A caller's input as the kernels read it: a device array (or NULL) where it is, a host one copied into `buf` with its
+// rows packed (row stride row_bytes)
+template <class T>
+int stage_in(Ctx* c, const void* src, int mem_kind, size_t rows, size_t row_bytes, size_t stride, DBuf& buf,
+             unsigned flags, const T** dev) {
+    *dev = static_cast<const T*>(src);
+    if (mem_kind == PRC_MEM_DEVICE || !src) return PRC_OK;
+    TRY(buf.ensure(rows * row_bytes));
+    *dev = buf.as<T>();
+    return rows_h2d(c, buf.p, src, rows, row_bytes, stride, flags);
+}
+
+// Where the kernels write a caller's output: a device array (or NULL) itself, `bytes` of `buf` for a host one
+template <class T>
+int stage_out(void* dst, int mem_kind, size_t bytes, DBuf& buf, T** dev) {
+    *dev = static_cast<T*>(dst);
+    if (mem_kind == PRC_MEM_DEVICE || !dst) return PRC_OK;
+    TRY(buf.ensure(bytes));
+    *dev = buf.as<T>();
+    return PRC_OK;
+}
+
+// Results, rows packed at `src`, back to a caller's host output whose rows are `stride` bytes apart; nothing to do for
+// a device output (the kernels wrote it) or a NULL one
+int unstage(Ctx* c, void* dst, const void* src, int mem_kind, size_t rows, size_t row_bytes, size_t stride, unsigned flags) {
+    if (mem_kind == PRC_MEM_DEVICE || !dst) return PRC_OK;
+    return rows_d2h(c, dst, src, rows, row_bytes, stride, flags);
+}
+
+// A parameter array of the call -> `buf`.  It is copied out of the caller's memory before the call returns: the
+// transfer below is from pageable memory this function owns, which the runtime stages before cudaMemcpyAsync returns,
+// so it is safe under PRC_FLAG_ASYNC even when the caller's array is page-locked and goes away right after the call
+int copy_params(Ctx* c, const double* src, int count, DBuf& buf) {
+    const std::vector<double> v(src, src + count);
+    TRY(buf.ensure((size_t)count * sizeof(double)));
+    CU(cudaMemcpyAsync(buf.p, v.data(), (size_t)count * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    return PRC_OK;
+}
+
 // window (host or device, double or float) -> device float
 int stage_window(Ctx* c, const void* window, long long n, int mem_kind, unsigned flags, const float** win32) {
     *win32 = nullptr;
     if (!window) return PRC_OK;
-    if (flags & PRC_FLAG_WINDOW_F32) {
-        if (mem_kind == PRC_MEM_DEVICE) {
-            *win32 = static_cast<const float*>(window);
-            return PRC_OK;
-        }
-        TRY(c->win32.ensure((size_t)n * sizeof(float)));
-        TRY(h2d(c, c->win32.p, window, (size_t)n * sizeof(float), flags));
-        *win32 = c->win32.as<float>();
-        return PRC_OK;
-    }
-    const double* w64 = static_cast<const double*>(window);
+    if (flags & PRC_FLAG_WINDOW_F32)
+        return stage_in(c, window, mem_kind, 1, (size_t)n * sizeof(float), (size_t)n * sizeof(float), c->win32, flags, win32);
+    const double* w64;
+    TRY(stage_in(c, window, mem_kind, 1, (size_t)n * sizeof(double), (size_t)n * sizeof(double), c->win64, flags, &w64));
     TRY(c->win32.ensure((size_t)n * sizeof(float)));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->win64.ensure((size_t)n * sizeof(double)));
-        TRY(h2d(c, c->win64.p, window, (size_t)n * sizeof(double), flags));
-        w64 = c->win64.as<double>();
-    }
     f64_to_f32_kernel<<<ceil_div(n, 256), 256, 0, c->stream>>>(w64, c->win32.as<float>(), n);
     TRY(check_launch("f64_to_f32_kernel"));
     *win32 = c->win32.as<float>();
@@ -1452,8 +1526,6 @@ int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batc
     return PRC_OK;
 }
 
-bool bad_mem_kind(int k) { return k != PRC_MEM_HOST && k != PRC_MEM_DEVICE; }
-
 // ---- Kalman trackers (track.cuh) -----------------------------------------------------------------
 constexpr size_t TRK_SLOT_BUDGET = 256u << 20;     // candidate slots of one multi-tracker launch (bytes)
 
@@ -1525,15 +1597,9 @@ int trk_stage(Ctx* c, const void* maps, int rows, int cols, int nseq, int nframe
         TRY(c->trk_map.ensure((size_t)nseq * nframes * n * esz));
         char* d = c->trk_map.as<char>();
         const char* h = static_cast<const char*>(maps);
-        for (int s = 0; s < nseq; ++s) {
-            if (frame_stride == n) {
-                TRY(h2d(c, d + (size_t)s * nframes * n * esz, h + (size_t)s * seq_stride * esz, (size_t)nframes * n * esz, flags));
-                continue;
-            }
-            for (int f = 0; f < nframes; ++f)
-                TRY(h2d(c, d + ((size_t)s * nframes + f) * n * esz, h + ((size_t)s * seq_stride + (size_t)f * frame_stride) * esz,
-                        n * esz, flags));
-        }
+        for (int s = 0; s < nseq; ++s)
+            TRY(rows_h2d(c, d + (size_t)s * nframes * n * esz, h + (size_t)s * seq_stride * esz, nframes, n * esz,
+                         (size_t)frame_stride * esz, flags));
         mp->maps = d;
         mp->seq_stride = (long long)nframes * n;
         mp->frame_stride = n;
@@ -1763,7 +1829,7 @@ int chanoff_stage(Ctx* c, AsyncScratch& ws, const void** s, int dt, int64_t n, i
     const size_t b = (size_t)n * chanoff::dt_size(dt);
     void* d;
     TRY(ws.get(&d, b));
-    TRY(h2d(c, d, *s, b, flags));
+    TRY(rows_h2d(c, d, *s, 1, b, b, flags));
     *s = d;
     return PRC_OK;
 }
@@ -1827,6 +1893,54 @@ int ls_svd_device(Ctx* c, const float2* ref, const float2* srv, long long n, Bat
     p.taps = c->svd_taps.as<double2>();
     lssvd::launch_fir(p, bt.nf, c->stream);
     return check_launch("svd_fir_kernel");
+}
+
+// ---- bodies the single-frame entry points share with their batched twins
+// prc_xambg_c64 / prc_xambg_frames_c64 after their checks, with c locked; bt: the caller's frames.  taps32 (device,
+// float32) is the tap-weighted decimator, which only the single-frame entry takes, or NULL
+int xambg_entry(Ctx* c, const prc_c64* ref, const prc_c64* srv, long long n, Batch bt, int range_bins, int freq_bins,
+                const void* window, const float* taps32, long long ndtaps, prc_c64* out, int mem_kind, unsigned flags) {
+    const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
+    const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2) * bt.nf;
+    const float2 *dref, *dsrv;
+    float2* dout;
+    TRY(stage_in(c, ref, mem_kind, bt.nf, nb, sb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, bt.nf, nb, sb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, ob, c->out, &dout));
+    if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
+    const float* win32;
+    TRY(stage_window(c, window, n, mem_kind, flags, &win32));
+    const long long D = n / freq_bins;
+    const bool batched = D >= 2 && caf_fft_plan(n, range_bins, freq_bins, D + 1, D, true, 0).on;
+    if (batched || bt.nf == 1) {
+        TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, taps32, ndtaps, dout, bt));
+    } else {
+        for (int fr = 0; fr < bt.nf; ++fr)       // direct-form kernels, frame by frame
+            TRY(xambg_device(c, dref + (size_t)fr * bt.stride, dsrv + (size_t)fr * bt.stride, n, range_bins, freq_bins, win32,
+                             nullptr, 0, dout + (size_t)fr * freq_bins * (range_bins + 1)));
+    }
+    TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
+    return finish(c, flags);
+}
+
+// LS_Filter_Multiple's bins (prc_ls_multiple_c64 / prc_ls_multiple_frames_c64) on bt.nf frames, every buffer bt.stride
+// samples apart: the last bin writes out and, when taps is given, its taps
+int ls_bins(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len, int peek,
+            double sample_rate, const double* doppler_bins, int nbins, float2* out, float2* taps, unsigned flags) {
+    const size_t span = ((size_t)(bt.nf - 1) * bt.stride + n) * sizeof(float2);
+    if (nbins > 1) TRY(c->clean.ensure(span));
+    if (nbins > 2) TRY(c->clean2.ensure(span));
+    // bins are applied one after the other on the running residual (clutter_removal.py:178-187)
+    const float2* cur = srv;
+    for (int b = 0; b < nbins; ++b) {
+        const double fc = doppler_bins ? doppler_bins[b] : 0.0;
+        const bool last = (b == nbins - 1);
+        float2* dst = last ? out : (((nbins - 1 - b) & 1) ? c->clean.as<float2>() : c->clean2.as<float2>());
+        TRY(ls_toeplitz_device(c, ref, cur, n, filter_len, peek, fc != 0.0, fc, sample_rate, dst, last ? taps : nullptr, bt));
+        if (!(flags & PRC_FLAG_ASYNC)) TRY(check_ls_status(c, 0, bt.nf));      // singular systems are reported per bin
+        cur = dst;
+    }
+    return PRC_OK;
 }
 
 }  // namespace
@@ -1941,79 +2055,41 @@ int prc_host_unregister(void* ptr) {
 int prc_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int range_bins, int freq_bins,
                   const void* window, const double* dtaps, int64_t ndtaps, prc_c64* out, int mem_kind,
                   int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, 1, n, &bt, range_bins, freq_bins));
     if (dtaps && ndtaps < 1) return fail(PRC_E_INVALID, "ndtaps=%lld invalid", (long long)ndtaps);
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
-    const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2);
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (mem_kind == PRC_MEM_HOST) {
-        if (freq_bins < 1 || range_bins < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", freq_bins, range_bins);
-        TRY(c->ref.ensure(nb));
-        TRY(c->srv.ensure(nb));
-        TRY(c->out.ensure(ob));
-        TRY(h2d(c, c->ref.p, ref, nb, flags));
-        TRY(h2d(c, c->srv.p, srv, nb, flags));
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->out.as<float2>();
-    }
-    const float* win32;
-    TRY(stage_window(c, window, n, mem_kind, flags, &win32));
     const float* taps32 = nullptr;
     if (dtaps) {
+        const double* t64;
+        TRY(stage_in(c, dtaps, mem_kind, 1, (size_t)ndtaps * sizeof(double), (size_t)ndtaps * sizeof(double), c->dtaps64,
+                     flags, &t64));
         TRY(c->dtaps32.ensure((size_t)ndtaps * sizeof(float)));
-        const double* t64 = dtaps;
-        if (mem_kind == PRC_MEM_HOST) {
-            TRY(c->dtaps64.ensure((size_t)ndtaps * sizeof(double)));
-            TRY(h2d(c, c->dtaps64.p, dtaps, (size_t)ndtaps * sizeof(double), flags));
-            t64 = c->dtaps64.as<double>();
-        }
         f64_to_f32_kernel<<<ceil_div(ndtaps, 256), 256, 0, c->stream>>>(t64, c->dtaps32.as<float>(), ndtaps);
         TRY(check_launch("f64_to_f32_kernel"));
         taps32 = c->dtaps32.as<float>();
     }
-    TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, taps32, ndtaps, dout));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, c->out.p, ob, flags));
-    return finish(c, flags);
+    return xambg_entry(c, ref, srv, n, bt, range_bins, freq_bins, window, taps32, ndtaps, out, mem_kind, flags);
 }
 
 int prc_ls_filter_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int filter_len, int peek, float reg,
                       prc_c64* out, prc_c64* taps, int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, 1, n, nullptr));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dtaps = reinterpret_cast<float2*>(taps);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb));
-        TRY(c->srv.ensure(nb));
-        TRY(c->clean.ensure(nb));
-        TRY(h2d(c, c->ref.p, ref, nb, flags));
-        TRY(h2d(c, c->srv.p, srv, nb, flags));
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->clean.as<float2>();
-        dtaps = nullptr;
-    }
+    const size_t nb = (size_t)n * sizeof(float2), mb = (size_t)(filter_len + peek) * sizeof(float2);
+    const float2 *dref, *dsrv;
+    float2* dout;
+    TRY(stage_in(c, ref, mem_kind, 1, nb, nb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, 1, nb, nb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, nb, c->clean, &dout));
+    float2* dtaps = mem_kind == PRC_MEM_DEVICE ? reinterpret_cast<float2*>(taps) : nullptr;   // host: from c->lstaps
     TRY(ls_device(c, dref, dsrv, n, filter_len, peek, (double)reg, dout, dtaps));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, out, c->clean.p, nb, flags));
-        if (taps)
-            TRY(d2h(c, taps, c->lstaps.p, (size_t)(filter_len + peek) * sizeof(float2), flags));
-    }
+    TRY(unstage(c, out, dout, mem_kind, 1, nb, nb, flags));
+    TRY(unstage(c, taps, c->lstaps.p, mem_kind, 1, mb, mb, flags));
     TRY(check_ls_status(c, flags));
     return finish(c, flags);
 }
@@ -2021,94 +2097,32 @@ int prc_ls_filter_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int fil
 int prc_nlms_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int filter_len, int peek, float mu,
                  int block_len, const prc_c64* init_taps, prc_c64* out, prc_c64* taps_out, int mem_kind,
                  int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    Ctx* c;
-    TRY(get_ctx(device, stream, &c));
-    std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
-    const int M = filter_len + peek;
-    const size_t mb = (size_t)(M > 0 ? M : 1) * sizeof(float2);
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    const float2* dinit = reinterpret_cast<const float2*>(init_taps);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dtaps = reinterpret_cast<float2*>(taps_out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb));
-        TRY(c->srv.ensure(nb));
-        TRY(c->clean.ensure(nb));
-        TRY(c->nl_taps.ensure(mb));
-        TRY(h2d(c, c->ref.p, ref, nb, flags));
-        TRY(h2d(c, c->srv.p, srv, nb, flags));
-        if (init_taps) {
-            TRY(c->nl_init.ensure(mb));
-            TRY(h2d(c, c->nl_init.p, init_taps, mb, flags));
-            dinit = c->nl_init.as<float2>();
-        }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->clean.as<float2>();
-        dtaps = c->nl_taps.as<float2>();
-    }
-    TRY(nlms_device(c, dref, dsrv, n, filter_len, peek, mu, block_len, dinit, dout, dtaps));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, out, c->clean.p, nb, flags));
-        if (taps_out) TRY(d2h(c, taps_out, c->nl_taps.p, mb, flags));
-    }
-    return finish(c, flags);
+    return prc_nlms_frames_c64(ref, srv, n, 1, n, filter_len, peek, mu, block_len, init_taps, out, taps_out, mem_kind,
+                               device, stream, flags);
 }
 
 int prc_nlms_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
                         int filter_len, int peek, float mu, int block_len, const prc_c64* init_taps, prc_c64* out,
                         prc_c64* taps_out, int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, nframes, frame_stride, &bt));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
+    const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
     const int M = filter_len + peek;
     const size_t mb = (size_t)(M > 0 ? M : 1) * sizeof(float2);
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    const float2* dinit = reinterpret_cast<const float2*>(init_taps);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dtaps = reinterpret_cast<float2*>(taps_out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb * nframes));
-        TRY(c->srv.ensure(nb * nframes));
-        TRY(c->clean.ensure(nb * nframes));
-        TRY(c->nl_taps.ensure(mb * nframes));
-        for (int fr = 0; fr < nframes; ++fr) {
-            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
-            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
-        }
-        if (init_taps) {
-            TRY(c->nl_init.ensure(mb));
-            TRY(h2d(c, c->nl_init.p, init_taps, mb, flags));
-            dinit = c->nl_init.as<float2>();
-        }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->clean.as<float2>();
-        dtaps = c->nl_taps.as<float2>();
-        bt.stride = n;
-    }
+    const float2 *dref, *dsrv, *dinit;
+    float2 *dout, *dtaps;
+    TRY(stage_in(c, ref, mem_kind, nframes, nb, sb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, nframes, nb, sb, c->srv, flags, &dsrv));
+    TRY(stage_in(c, init_taps, mem_kind, 1, mb, mb, c->nl_init, flags, &dinit));
+    TRY(stage_out(out, mem_kind, nb * nframes, c->clean, &dout));
+    TRY(stage_out(taps_out, mem_kind, mb * nframes, c->nl_taps, &dtaps));
+    if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     TRY(nlms_device(c, dref, dsrv, n, filter_len, peek, mu, block_len, dinit, dout, dtaps, bt, true));
-    if (mem_kind == PRC_MEM_HOST) {
-        const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
-        for (int fr = 0; fr < nframes; ++fr)
-            TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
-        if (taps_out) TRY(d2h(c, taps_out, c->nl_taps.p, mb * nframes, flags));
-    }
+    TRY(unstage(c, out, dout, mem_kind, nframes, nb, sb, flags));
+    TRY(unstage(c, taps_out, dtaps, mem_kind, 1, mb * nframes, mb * nframes, flags));
     return finish(c, flags);
 }
 
@@ -2116,157 +2130,73 @@ int prc_gal_jpe_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, in
                            int lattice_len, int delay_line_len, double mu1, double mu2, int peek,
                            prc_c64* out, prc_c64* k_out, prc_c64* h_out,
                            int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, nframes, frame_stride, &bt));
     TRY(gal_check(n, lattice_len, delay_line_len, peek));      // before any CUDA call
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
+    const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
     const size_t db = (size_t)delay_line_len * sizeof(float2);
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dk = reinterpret_cast<float2*>(k_out);
-    float2* dh = reinterpret_cast<float2*>(h_out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb * nframes));
-        TRY(c->srv.ensure(nb * nframes));
-        TRY(c->clean.ensure(nb * nframes));
-        for (int fr = 0; fr < nframes; ++fr) {
-            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
-            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
-        }
-        if (k_out) { TRY(c->gal_k.ensure(db * nframes)); dk = c->gal_k.as<float2>(); }
-        if (h_out) { TRY(c->gal_h.ensure(db * nframes)); dh = c->gal_h.as<float2>(); }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->clean.as<float2>();
-        bt.stride = n;
-    }
+    const float2 *dref, *dsrv;
+    float2 *dout, *dk, *dh;
+    TRY(stage_in(c, ref, mem_kind, nframes, nb, sb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, nframes, nb, sb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, nb * nframes, c->clean, &dout));
+    TRY(stage_out(k_out, mem_kind, db * nframes, c->gal_k, &dk));
+    TRY(stage_out(h_out, mem_kind, db * nframes, c->gal_h, &dh));
+    if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     TRY(gal_device(c, dref, dsrv, n, bt, lattice_len, delay_line_len, mu1, mu2, peek, dout, dk, dh));
-    if (mem_kind == PRC_MEM_HOST) {
-        const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
-        for (int fr = 0; fr < nframes; ++fr)
-            TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
-        if (k_out) TRY(d2h(c, k_out, c->gal_k.p, db * nframes, flags));
-        if (h_out) TRY(d2h(c, h_out, c->gal_h.p, db * nframes, flags));
-    }
+    TRY(unstage(c, out, dout, mem_kind, nframes, nb, sb, flags));
+    TRY(unstage(c, k_out, dk, mem_kind, 1, db * nframes, db * nframes, flags));
+    TRY(unstage(c, h_out, dh, mem_kind, 1, db * nframes, db * nframes, flags));
     return finish(c, flags);
 }
 
 int prc_xambg_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
                          int range_bins, int freq_bins, const void* window, prc_c64* out, int mem_kind, int device,
                          void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
-    if (freq_bins < 1 || range_bins < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", freq_bins, range_bins);
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, nframes, frame_stride, &bt, range_bins, freq_bins));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
-    const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2);
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb * nframes));
-        TRY(c->srv.ensure(nb * nframes));
-        TRY(c->out.ensure(ob * nframes));
-        for (int fr = 0; fr < nframes; ++fr) {
-            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
-            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
-        }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->out.as<float2>();
-        bt.stride = n;
-    }
-    const float* win32;
-    TRY(stage_window(c, window, n, mem_kind, flags, &win32));
-    const long long D = n / freq_bins;
-    const bool batched = D >= 2 && caf_fft_plan(n, range_bins, freq_bins, D + 1, D, true, 0).on;
-    if (batched || nframes == 1) {
-        TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, nullptr, 0, dout, bt));
-    } else {
-        for (int fr = 0; fr < nframes; ++fr)       // direct-form kernels, frame by frame
-            TRY(xambg_device(c, dref + (size_t)fr * bt.stride, dsrv + (size_t)fr * bt.stride, n, range_bins, freq_bins, win32,
-                             nullptr, 0, dout + (size_t)fr * freq_bins * (range_bins + 1)));
-    }
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, c->out.p, ob * nframes, flags));
-    return finish(c, flags);
+    return xambg_entry(c, ref, srv, n, bt, range_bins, freq_bins, window, nullptr, 0, out, mem_kind, flags);
 }
 
 int prc_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
                    int filter_len, int peek, float reg, int range_bins, int freq_bins, const void* window,
                    prc_c64* out_maps, prc_c64* taps_out, prc_c64* cleaned_out, int mem_kind, int device, void* stream,
                    unsigned flags) {
-    if (!ref || !srv || !out_maps) return fail(PRC_E_INVALID, "ref/srv/out_maps must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
-    if (freq_bins < 1 || range_bins < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", freq_bins, range_bins);
+    Batch bt;
+    TRY(stack_args(ref, srv, out_maps, "ref/srv/out_maps", mem_kind, n, nframes, frame_stride, &bt, range_bins, freq_bins));
     if (filter_len < 0 || peek < 0 || filter_len + peek < 1)
         return fail(PRC_E_INVALID, "filter_len=%d peek=%d invalid", filter_len, peek);
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     const int M = filter_len + peek;
-    const size_t nb = (size_t)n * sizeof(float2);
+    // host taps are read from c->lstaps after the call, which holds every frame's taps on the FFT-domain path only
+    if (mem_kind == PRC_MEM_HOST && taps_out && nframes > 1 &&
+        !(ls_fft_plan(c, n, M, nframes).on && caf_fft_plan(n, range_bins, freq_bins, n / freq_bins + 1, n / freq_bins, true, M).on))
+        return fail(PRC_E_INVALID, "taps_out with host pointers and nframes > 1 needs the FFT-domain path");
+    const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
     const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2);
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dmap = reinterpret_cast<float2*>(out_maps);
-    float2* dtaps = reinterpret_cast<float2*>(taps_out);
-    float2* dclean = reinterpret_cast<float2*>(cleaned_out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb * nframes));
-        TRY(c->srv.ensure(nb * nframes));
-        TRY(c->out.ensure(ob * nframes));
-        if (cleaned_out) TRY(c->clean.ensure(nb * nframes));
-        for (int fr = 0; fr < nframes; ++fr) {
-            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
-            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
-        }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dmap = c->out.as<float2>();
-        dtaps = nullptr;
-        dclean = cleaned_out ? c->clean.as<float2>() : nullptr;
-        bt.stride = n;
-    }
+    const size_t tb = (size_t)nframes * M * sizeof(float2);
+    const float2 *dref, *dsrv;
+    float2 *dmap, *dclean;
+    TRY(stage_in(c, ref, mem_kind, nframes, nb, sb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, nframes, nb, sb, c->srv, flags, &dsrv));
+    TRY(stage_out(out_maps, mem_kind, ob * nframes, c->out, &dmap));
+    TRY(stage_out(cleaned_out, mem_kind, nb * nframes, c->clean, &dclean));
+    float2* dtaps = mem_kind == PRC_MEM_DEVICE ? reinterpret_cast<float2*>(taps_out) : nullptr;   // host: from c->lstaps
+    if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     const float* win32;
     TRY(stage_window(c, window, n, mem_kind, flags, &win32));
     TRY(frame_device(c, dref, dsrv, n, bt, filter_len, peek, (double)reg, range_bins, freq_bins, win32, dmap, dtaps, dclean));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, out_maps, c->out.p, ob * nframes, flags));
-        if (taps_out) {
-            if (nframes > 1 && !(ls_fft_plan(c, n, M, nframes).on && caf_fft_plan(n, range_bins, freq_bins, n / freq_bins + 1, n / freq_bins, true, M).on))
-                return fail(PRC_E_INVALID, "taps_out with host pointers and nframes > 1 needs the FFT-domain path");
-            TRY(d2h(c, taps_out, c->lstaps.p, (size_t)nframes * M * sizeof(float2), flags));
-        }
-        if (cleaned_out) {
-            const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
-            for (int fr = 0; fr < nframes; ++fr)
-                TRY(d2h(c, cleaned_out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
-        }
-    }
+    TRY(unstage(c, out_maps, dmap, mem_kind, 1, ob * nframes, ob * nframes, flags));
+    TRY(unstage(c, taps_out, c->lstaps.p, mem_kind, 1, tb, tb, flags));
+    TRY(unstage(c, cleaned_out, dclean, mem_kind, nframes, nb, sb, flags));
     TRY(check_ls_status(c, flags, nframes));
     return finish(c, flags);
 }
@@ -2328,111 +2258,59 @@ int prc_get_option(const char* name, int* value) {
 
 int prc_ls_toeplitz_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int filter_len, int peek,
                         prc_c64* out, prc_c64* taps, int mem_kind, int device, void* stream, unsigned flags) {
-    const double bin0 = 0.0;
-    (void)bin0;
     return prc_ls_multiple_c64(ref, srv, n, filter_len, peek, 1.0, nullptr, 1, out, taps, mem_kind, device, stream, flags);
 }
 
 int prc_ls_multiple_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int filter_len, int peek,
                         double sample_rate, const double* doppler_bins, int nbins, prc_c64* out, prc_c64* taps_last,
                         int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, 1, n, nullptr));
     if (nbins < 1) return fail(PRC_E_INVALID, "nbins=%d invalid", nbins);
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t nb = (size_t)n * sizeof(float2);
-    const int M = filter_len + peek;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dtaps = reinterpret_cast<float2*>(taps_last);
-    TRY(c->clean.ensure(nb));
-    TRY(c->clean2.ensure(nb));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb));
-        TRY(c->srv.ensure(nb));
-        TRY(h2d(c, c->ref.p, ref, nb, flags));
-        TRY(h2d(c, c->srv.p, srv, nb, flags));
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dtaps = nullptr;
-    }
-    // bins are applied one after the other on the running residual (clutter_removal.py:178-187)
-    const float2* cur = dsrv;
-    float2* ping[2] = {c->clean.as<float2>(), c->clean2.as<float2>()};
-    for (int b = 0; b < nbins; ++b) {
-        const double fc = doppler_bins ? doppler_bins[b] : 0.0;
-        const bool last = (b == nbins - 1);
-        float2* dst = (last && mem_kind == PRC_MEM_DEVICE) ? dout : ping[b & 1];
-        TRY(ls_toeplitz_device(c, dref, cur, n, filter_len, peek, fc != 0.0, fc, sample_rate, dst, last ? dtaps : nullptr));
-        if (!(flags & PRC_FLAG_ASYNC)) TRY(check_ls_status(c, 0));      // singular systems are reported per bin
-        cur = dst;
-    }
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, out, cur, nb, flags));
-        if (taps_last) TRY(d2h(c, taps_last, c->lstaps.p, (size_t)M * sizeof(float2), flags));
-    }
+    const size_t nb = (size_t)n * sizeof(float2), mb = (size_t)(filter_len + peek) * sizeof(float2);
+    const float2 *dref, *dsrv;
+    float2* dout;
+    TRY(stage_in(c, ref, mem_kind, 1, nb, nb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, 1, nb, nb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, nb, c->out, &dout));
+    float2* dtaps = mem_kind == PRC_MEM_DEVICE ? reinterpret_cast<float2*>(taps_last) : nullptr;   // host: from c->lstaps
+    TRY(ls_bins(c, dref, dsrv, n, Batch{}, filter_len, peek, sample_rate, doppler_bins, nbins, dout, dtaps, flags));
+    TRY(unstage(c, out, dout, mem_kind, 1, nb, nb, flags));
+    TRY(unstage(c, taps_last, c->lstaps.p, mem_kind, 1, mb, mb, flags));
     return finish(c, flags);
 }
 
 int prc_ls_multiple_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
                                int filter_len, int peek, double sample_rate, const double* doppler_bins, int nbins,
                                prc_c64* out, int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
     if (mem_kind != PRC_MEM_DEVICE) return fail(PRC_E_INVALID, "prc_ls_multiple_frames_c64 takes device pointers (mem_kind=%d)", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
     if (nframes < 1 || nbins < 1) return fail(PRC_E_INVALID, "nframes=%d nbins=%d invalid", nframes, nbins);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, nframes, frame_stride, &bt));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const size_t span = ((size_t)(nframes - 1) * bt.stride + n) * sizeof(float2);
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* cur = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (nbins > 1) TRY(c->clean.ensure(span));
-    if (nbins > 2) TRY(c->clean2.ensure(span));
-    // bins are applied one after the other on the running residual (clutter_removal.py:178-187); the last one
-    // writes the caller's buffer
-    for (int b = 0; b < nbins; ++b) {
-        const double fc = doppler_bins ? doppler_bins[b] : 0.0;
-        const bool last = (b == nbins - 1);
-        float2* dst = last ? dout : (((nbins - 1 - b) & 1) ? c->clean.as<float2>() : c->clean2.as<float2>());
-        TRY(ls_toeplitz_device(c, dref, cur, n, filter_len, peek, fc != 0.0, fc, sample_rate, dst, nullptr, bt));
-        if (!(flags & PRC_FLAG_ASYNC)) TRY(check_ls_status(c, 0, nframes));
-        cur = dst;
-    }
+    TRY(ls_bins(c, reinterpret_cast<const float2*>(ref), reinterpret_cast<const float2*>(srv), n, bt, filter_len, peek,
+                sample_rate, doppler_bins, nbins, reinterpret_cast<float2*>(out), nullptr, flags));
     return finish(c, flags);
 }
 
 int prc_iq_mix_c64(const void* in, int in_kind, int64_t n, int mode, double fc, double fs, double phase_offset,
                    prc_c64* out, int mem_kind, int device, void* stream, unsigned flags) {
     if (!in || !out) return fail(PRC_E_INVALID, "in/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (in_kind < IQ_C64 || in_kind > IQ_I16) return fail(PRC_E_INVALID, "in_kind=%d invalid", in_kind);
-    if (mode < MIX_NONE || mode > MIX_FS64) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
-    if (mode != MIX_NONE && !(fs != 0.0)) return fail(PRC_E_INVALID, "fs must not be 0");
+    TRY(frontend_args(mem_kind, n, in_kind, mode, fs));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const void* din = in;
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->fe_in.ensure(iq_bytes(in_kind, n)));
-        TRY(c->fe_out.ensure((size_t)n * sizeof(float2)));
-        TRY(h2d(c, c->fe_in.p, in, iq_bytes(in_kind, n), flags));
-        din = c->fe_in.p;
-        dout = c->fe_out.as<float2>();
-    }
+    const size_t ib = iq_bytes(in_kind, n), ob = (size_t)n * sizeof(float2);
+    const void* din;
+    float2* dout;
+    TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
+    TRY(stage_out(out, mem_kind, ob, c->fe_out, &dout));
     TRY(mix_device(c, make_mix(din, in_kind, n, mode, fc, fs, phase_offset), dout));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, (size_t)n * sizeof(float2), flags));
+    TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
@@ -2448,29 +2326,21 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
                      int up, int down, const double* h, int nh, prc_c64* out, int64_t out_capacity,
                      int mem_kind, int device, void* stream, unsigned flags) {
     if (!in || !out || !h) return fail(PRC_E_INVALID, "in/out/h must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
-    if (in_kind < IQ_C64 || in_kind > IQ_I16) return fail(PRC_E_INVALID, "in_kind=%d invalid", in_kind);
-    if (mode < MIX_NONE || mode > MIX_FS64) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
-    if (mode != MIX_NONE && !(fs != 0.0)) return fail(PRC_E_INVALID, "fs must not be 0");
+    TRY(frontend_args(mem_kind, n, in_kind, mode, fs));
     ResampleGeo g;
     TRY(resample_geo(n, up, down, nh, &g));
     if (out_capacity < g.n_out) return fail(PRC_E_INVALID, "out holds %lld samples, %lld needed", (long long)out_capacity, g.n_out);
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const void* din = in;
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->fe_in.ensure(iq_bytes(in_kind, n)));
-        TRY(c->fe_out.ensure((size_t)g.n_out * sizeof(float2)));
-        TRY(h2d(c, c->fe_in.p, in, iq_bytes(in_kind, n), flags));
-        din = c->fe_in.p;
-        dout = c->fe_out.as<float2>();
-    }
+    const size_t ib = iq_bytes(in_kind, n);
+    const void* din;
+    float2* dout;
+    TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
+    TRY(stage_out(out, mem_kind, (size_t)g.n_out * sizeof(float2), c->fe_out, &dout));
     long long n_out = 0;
     TRY(resample_device(c, make_mix(din, in_kind, n, mode, fc, fs, phase_offset), up, down, h, nh, dout, &n_out));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, (size_t)n_out * sizeof(float2), flags));
+    TRY(unstage(c, out, dout, mem_kind, 1, (size_t)n_out * sizeof(float2), (size_t)n_out * sizeof(float2), flags));
     return finish(c, flags);
 }
 
@@ -2479,13 +2349,9 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
                             prc_c64* out, int64_t out_stride, int64_t out_capacity, int mem_kind, int device,
                             void* stream, unsigned flags) {
     if (!in || !out || !h || !phase_offsets) return fail(PRC_E_INVALID, "in/out/h/phase_offsets must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    TRY(frontend_args(mem_kind, n, in_kind, mode, fs));
     if (nchunks < 1 || nchunks > 65535) return fail(PRC_E_INVALID, "nchunks=%d outside [1, 65535]", nchunks);
     if (nchunks > 1 && chunk_stride < 0) return fail(PRC_E_INVALID, "chunk_stride=%lld invalid", (long long)chunk_stride);
-    if (in_kind < IQ_C64 || in_kind > IQ_I16) return fail(PRC_E_INVALID, "in_kind=%d invalid", in_kind);
-    if (mode < MIX_NONE || mode > MIX_FS64) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
-    if (mode != MIX_NONE && !(fs != 0.0)) return fail(PRC_E_INVALID, "fs must not be 0");
     ResampleGeo g;
     TRY(resample_geo(n, up, down, nh, &g));
     if (nchunks > 1 && out_stride < g.n_out)
@@ -2497,32 +2363,16 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const void* din = in;
-    float2* dout = reinterpret_cast<float2*>(out);
-    long long dstride = ostride;
-    if (mem_kind == PRC_MEM_HOST) {
-        const size_t in_bytes = iq_bytes(in_kind, (long long)(nchunks - 1) * cstride + n);
-        TRY(c->fe_in.ensure(in_bytes));
-        TRY(c->fe_out.ensure((size_t)nchunks * g.n_out * sizeof(float2)));
-        TRY(h2d(c, c->fe_in.p, in, in_bytes, flags));
-        din = c->fe_in.p;
-        dout = c->fe_out.as<float2>();
-        dstride = g.n_out;
-    }
-    // copied out of the caller's memory before the call returns: the transfer below is from pageable memory this
-    // function owns, which the runtime stages before cudaMemcpyAsync returns, so it is safe under PRC_FLAG_ASYNC even
-    // when the caller's array is page-locked and goes away right after the call
-    const std::vector<double> po(phase_offsets, phase_offsets + nchunks);
-    TRY(c->fe_po.ensure((size_t)nchunks * sizeof(double)));
-    CU(cudaMemcpyAsync(c->fe_po.p, po.data(), (size_t)nchunks * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    const size_t ib = iq_bytes(in_kind, (long long)(nchunks - 1) * cstride + n), cb = (size_t)g.n_out * sizeof(float2);
+    const void* din;
+    float2* dout;
+    TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
+    TRY(stage_out(out, mem_kind, nchunks * cb, c->fe_out, &dout));
+    const long long dstride = mem_kind == PRC_MEM_HOST ? g.n_out : ostride;      // staged chunks are packed
+    TRY(copy_params(c, phase_offsets, nchunks, c->fe_po));
     TRY(frontend_chunks_device(c, make_mix(din, in_kind, n, mode, fc, fs, 0.0), nchunks, cstride, c->fe_po.as<double>(),
                                up, down, h, nh, dout, dstride));
-    if (mem_kind == PRC_MEM_HOST) {
-        if (ostride == g.n_out) TRY(d2h(c, out, dout, (size_t)nchunks * g.n_out * sizeof(float2), flags));
-        else
-            for (int b = 0; b < nchunks; ++b)
-                TRY(d2h(c, out + (size_t)b * ostride, dout + (size_t)b * g.n_out, (size_t)g.n_out * sizeof(float2), flags));
-    }
+    TRY(unstage(c, out, dout, mem_kind, nchunks, cb, (size_t)ostride * sizeof(float2), flags));
     return finish(c, flags);
 }
 
@@ -2536,23 +2386,16 @@ int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const floa
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t cells = (size_t)rows * cols;
-    const void* dx = x;
-    float* dcr = cr_out;
-    uint8_t* ddet = det_out;
-    if (mem_kind == PRC_MEM_HOST) {
-        const size_t inb = cells * (cplx ? sizeof(float2) : sizeof(float));
-        TRY(c->cf_in.ensure(inb));
-        TRY(h2d(c, c->cf_in.p, x, inb, flags));
-        dx = c->cf_in.p;
-        if (cr_out) { TRY(c->cf_cr.ensure(cells * sizeof(float))); dcr = c->cf_cr.as<float>(); }
-        if (det_out) { TRY(c->cf_det.ensure(cells)); ddet = c->cf_det.as<uint8_t>(); }
-    }
+    const size_t cells = (size_t)rows * cols, inb = cells * (cplx ? sizeof(float2) : sizeof(float));
+    const void* dx;
+    float* dcr;
+    uint8_t* ddet;
+    TRY(stage_in(c, x, mem_kind, 1, inb, inb, c->cf_in, flags, &dx));
+    TRY(stage_out(cr_out, mem_kind, cells * sizeof(float), c->cf_cr, &dcr));
+    TRY(stage_out(det_out, mem_kind, cells, c->cf_det, &ddet));
     TRY(cfar_device(c, dx, cplx, rows, cols, fw, gw, thresh, dcr, ddet));
-    if (mem_kind == PRC_MEM_HOST) {
-        if (cr_out) TRY(d2h(c, cr_out, dcr, cells * sizeof(float), flags));
-        if (det_out) TRY(d2h(c, det_out, ddet, cells, flags));
-    }
+    TRY(unstage(c, cr_out, dcr, mem_kind, 1, cells * sizeof(float), cells * sizeof(float), flags));
+    TRY(unstage(c, det_out, ddet, mem_kind, 1, cells, cells, flags));
     return finish(c, flags);
 }
 
@@ -2573,30 +2416,15 @@ int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t fr
     std::lock_guard<std::mutex> lk(c->mu);
     if (nframes == 0) return finish(c, flags);
     const size_t ine = cplx ? sizeof(float2) : sizeof(float), oute = f64 ? sizeof(double) : sizeof(float);
-    f.p.x = x;
+    const long long xs = nframes > 1 ? frame_stride : cells, os = nframes > 1 ? cr_stride : cells;
+    TRY(stage_in(c, x, mem_kind, nframes, cells * ine, xs * ine, c->rd_in, flags, &f.p.x));
+    TRY(stage_out(cr_out, mem_kind, (size_t)nframes * cells * oute, c->rd_out, &f.cr));
     f.p.is_complex = cplx ? 1 : 0;
-    f.frame_stride = nframes > 1 ? frame_stride : cells;
-    f.cr = cr_out;
-    f.cr_stride = nframes > 1 ? cr_stride : cells;
+    f.frame_stride = mem_kind == PRC_MEM_HOST ? cells : xs;      // staged frames are packed
+    f.cr_stride = mem_kind == PRC_MEM_HOST ? cells : os;
     f.cr_f64 = f64 ? 1 : 0;
-    if (mem_kind == PRC_MEM_HOST) {            // staged frame after frame, compact
-        TRY(c->rd_in.ensure((size_t)nframes * cells * ine));
-        TRY(c->rd_out.ensure((size_t)nframes * cells * oute));
-        for (int b = 0; b < nframes; ++b)
-            TRY(h2d(c, c->rd_in.as<char>() + (size_t)b * cells * ine,
-                    static_cast<const char*>(x) + (size_t)b * f.frame_stride * ine, cells * ine, flags));
-        f.p.x = c->rd_in.p;
-        f.frame_stride = cells;
-        f.cr = c->rd_out.p;
-        f.cr_stride = cells;
-    }
     TRY(cfar_frames_device(c, f, nframes));
-    if (mem_kind == PRC_MEM_HOST) {
-        const long long os = nframes > 1 ? cr_stride : cells;
-        for (int b = 0; b < nframes; ++b)
-            TRY(d2h(c, static_cast<char*>(cr_out) + (size_t)b * os * oute, c->rd_out.as<char>() + (size_t)b * cells * oute,
-                    cells * oute, flags));
-    }
+    TRY(unstage(c, cr_out, f.cr, mem_kind, nframes, cells * oute, os * oute, flags));
     return finish(c, flags);
 }
 
@@ -2621,40 +2449,26 @@ int prc_persistence_frames(const void* x, int rows, int cols, int nframes, int64
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     if (nframes == 0) return finish(c, flags);
-    // the weights a call uses (min(hold, frames)) are copied out of the caller's memory before the call returns, as
-    // prc_frontend_chunks_c64 does with its phase offsets
-    const int nw = std::min(hold, total);
-    const std::vector<double> w(weights, weights + nw);
-    TRY(c->rd_w.ensure((size_t)nw * sizeof(double)));
-    CU(cudaMemcpyAsync(c->rd_w.p, w.data(), (size_t)nw * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    TRY(copy_params(c, weights, std::min(hold, total), c->rd_w));      // the weights the call uses
     rdr::PersistParams p{};
     const size_t ine = f64 ? sizeof(double) : sizeof(float);
-    p.x = x;
-    p.frame_stride = total > 1 ? frame_stride : cells;
+    const long long xs = total > 1 ? frame_stride : cells;
+    const size_t ob = (size_t)nframes * cells * sizeof(double);
+    TRY(stage_in(c, x, mem_kind, total, cells * ine, xs * ine, c->rd_in, flags, &p.x));
+    TRY(stage_out(out, mem_kind, ob, c->rd_out, &p.out));
+    p.frame_stride = mem_kind == PRC_MEM_HOST ? cells : xs;      // staged frames are packed
     p.f64 = f64 ? 1 : 0;
     p.f32prod = prod32 ? 1 : 0;
     p.oriented = (flags & PRC_FLAG_ORIENT) ? 1 : 0;
     p.rows = rows; p.cols = cols;
     p.n_carry = n_carry; p.nframes = nframes; p.hold = hold;
     p.w = c->rd_w.as<double>();
-    p.out = out;
-    const size_t ob = (size_t)nframes * cells * sizeof(double);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->rd_in.ensure((size_t)total * cells * ine));
-        TRY(c->rd_out.ensure(ob));
-        for (int b = 0; b < total; ++b)
-            TRY(h2d(c, c->rd_in.as<char>() + (size_t)b * cells * ine,
-                    static_cast<const char*>(x) + (size_t)b * p.frame_stride * ine, cells * ine, flags));
-        p.x = c->rd_in.p;
-        p.frame_stride = cells;
-        p.out = c->rd_out.as<double>();
-    }
     {
         ProfScope ps(c, K_PERSISTENCE);
         rdr::launch_persistence(p, c->stream);
     }
     TRY(check_launch("pst_kernel"));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, p.out, ob, flags));
+    TRY(unstage(c, out, p.out, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
@@ -2690,55 +2504,36 @@ int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t fram
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     if (nframes == 0) return finish(c, flags);
-    p.x = x;
-    p.frame_stride = nframes > 1 ? frame_stride : n;
-    p.out = out;
+    const long long xs = nframes > 1 ? frame_stride : n;
     const size_t ob = (size_t)nframes * nq * sizeof(double);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->rd_in.ensure((size_t)nframes * n * sizeof(double)));
-        TRY(c->rd_out.ensure(ob));
-        for (int b = 0; b < nframes; ++b)
-            TRY(h2d(c, c->rd_in.as<double>() + (size_t)b * n, x + (size_t)b * p.frame_stride, (size_t)n * sizeof(double),
-                    flags));
-        p.x = c->rd_in.as<double>();
-        p.frame_stride = n;
-        p.out = c->rd_out.as<double>();
-    }
+    TRY(stage_in(c, x, mem_kind, nframes, (size_t)n * sizeof(double), xs * sizeof(double), c->rd_in, flags, &p.x));
+    TRY(stage_out(out, mem_kind, ob, c->rd_out, &p.out));
+    p.frame_stride = mem_kind == PRC_MEM_HOST ? n : xs;      // staged frames are packed
     {
         ProfScope ps(c, K_PERCENTILE);
         rdr::launch_percentiles(p, nframes, c->stream);
     }
     TRY(check_launch("pct_kernel"));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, p.out, ob, flags));
+    TRY(unstage(c, out, p.out, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
 int prc_direct_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int range_bins, int freq_bins,
                          double sample_rate, prc_c64* out, int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (n <= 0) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, 1, n, nullptr));
     if (range_bins < 0 || freq_bins < 1) return fail(PRC_E_INVALID, "range_bins=%d freq_bins=%d invalid", range_bins, freq_bins);
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     const size_t nb = (size_t)n * sizeof(float2);
     const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2);
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb));
-        TRY(c->srv.ensure(nb));
-        TRY(c->out.ensure(ob));
-        TRY(h2d(c, c->ref.p, ref, nb, flags));
-        TRY(h2d(c, c->srv.p, srv, nb, flags));
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->out.as<float2>();
-    }
+    const float2 *dref, *dsrv;
+    float2* dout;
+    TRY(stage_in(c, ref, mem_kind, 1, nb, nb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, 1, nb, nb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, ob, c->out, &dout));
     TRY(direct_xambg_device(c, dref, dsrv, n, range_bins, freq_bins, sample_rate, dout));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, ob, flags));
+    TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
@@ -2761,22 +2556,14 @@ int prc_get_measurements_frames(const void* maps, int rows, int cols, int nseq, 
     TRY(c->trk_stats.ensure(nfr * 2 * sizeof(double)));
     mp.mean = c->trk_stats.as<double>();
     mp.thr = mp.mean + nfr;
-    mp.count = counts;
-    mp.out = meas;
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->trk_cnt.ensure(nfr * sizeof(int)));
-        TRY(c->trk_out.ensure(ob));
-        mp.count = c->trk_cnt.as<int>();
-        mp.out = c->trk_out.as<double>();
-    }
+    TRY(stage_out(counts, mem_kind, nfr * sizeof(int), c->trk_cnt, &mp.count));
+    TRY(stage_out(meas, mem_kind, ob, c->trk_out, &mp.out));
     mp.f0 = 0;
     mp.out_cap = meas_capacity;
     mp.out_nf = nframes;
     TRY(trk_meas_launch(c, mp, (flags & PRC_FLAG_MAP_F64) != 0, TRK_MODE_MEAS, nframes, nseq));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, counts, mp.count, nfr * sizeof(int), flags));
-        if (ob) TRY(d2h(c, meas, mp.out, ob, flags));
-    }
+    TRY(unstage(c, counts, mp.count, mem_kind, 1, nfr * sizeof(int), nfr * sizeof(int), flags));
+    TRY(unstage(c, ob ? meas : nullptr, mp.out, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
@@ -2808,11 +2595,8 @@ int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq,
     mp.out_cap = mp.cap;
     mp.out_nf = fc;
     const size_t hb = nfr * n_tracks * sizeof(prc_track);
-    prc_track* dh = history;
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->trk_out.ensure(hb));
-        dh = c->trk_out.as<prc_track>();
-    }
+    prc_track* dh;
+    TRY(stage_out(history, mem_kind, hb, c->trk_out, &dh));
     for (int f0 = 0; f0 < nframes; f0 += fc) {
         const int nf = std::min(fc, nframes - f0);
         mp.f0 = f0;
@@ -2832,7 +2616,7 @@ int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq,
         }
         TRY(check_launch("track_multi_kernel"));
     }
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, history, dh, hb, flags));
+    TRY(unstage(c, history, dh, mem_kind, 1, hb, hb, flags));
     return finish(c, flags);
 }
 
@@ -2852,11 +2636,8 @@ int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int 
     mp.mean = c->trk_stats.as<double>();
     TRY(trk_meas_launch(c, mp, f64, TRK_MODE_MEAN, nframes, nseq));
     const size_t hb = nfr * sizeof(prc_track_simple);
-    prc_track_simple* dh = history;
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->trk_out.ensure(hb));
-        dh = c->trk_out.as<prc_track_simple>();
-    }
+    prc_track_simple* dh;
+    TRY(stage_out(history, mem_kind, hb, c->trk_out, &dh));
     TrkSimpleParams sp{};
     sp.m = mp;
     sp.hist = dh;
@@ -2869,7 +2650,7 @@ int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int 
         else track_simple_kernel<float><<<nseq, TRK_SIMPLE_THREADS, 0, c->stream>>>(sp);
     }
     TRY(check_launch("track_simple_kernel"));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, history, dh, hb, flags));
+    TRY(unstage(c, history, dh, mem_kind, 1, hb, hb, flags));
     return finish(c, flags);
 }
 
@@ -2902,12 +2683,9 @@ int prc_channel_offset(const void* s1, int dtype1, int64_t n1, const void* s2, i
     double* xc = xc_abs;
     if (xc_abs && mem_kind == PRC_MEM_HOST) TRY(ws.get(&xc, (size_t)nvalid * sizeof(double)));
     TRY(chanoff_device(c, ws, s1, dtype1, n1, s2, dtype2, n2, f, nd, nl, nl, chanoff::ARG_ABS, xc, res));
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(d2h(c, offset, res + 1, sizeof(long long), flags));
-        if (xc_abs) TRY(d2h(c, xc_abs, xc, (size_t)nvalid * sizeof(double), flags));
-    } else {
-        CU(cudaMemcpyAsync(offset, res + 1, sizeof(long long), cudaMemcpyDeviceToDevice, c->stream));
-    }
+    if (mem_kind == PRC_MEM_DEVICE) CU(cudaMemcpyAsync(offset, res + 1, sizeof(long long), cudaMemcpyDeviceToDevice, c->stream));
+    TRY(unstage(c, offset, res + 1, mem_kind, 1, sizeof(long long), sizeof(long long), flags));
+    TRY(unstage(c, xc_abs, xc, mem_kind, 1, (size_t)nvalid * sizeof(double), (size_t)nvalid * sizeof(double), flags));
     return finish(c, flags);
 }
 
@@ -2929,57 +2707,39 @@ int prc_xcorr(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2
     if (mem_kind == PRC_MEM_HOST) TRY(ws.get(&dout, ob));
     TRY(chanoff_device(c, ws, s1, dtype1, n1, s2, dtype2, n2, nullptr, 1, nlag, nlead,
                        cplx ? chanoff::ARG_COMPLEX : chanoff::ARG_REAL, dout, nullptr));
-    if (mem_kind == PRC_MEM_HOST) TRY(d2h(c, out, dout, ob, flags));
+    TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
 
 int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
                           int filter_len, int peek, prc_c64* out, prc_c64* taps_out, int* rank_out,
                           int mem_kind, int device, void* stream, unsigned flags) {
-    if (!ref || !srv || !out) return fail(PRC_E_INVALID, "ref/srv/out must not be NULL");
-    if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
-    if (nframes > 1 && frame_stride < n) return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
     TRY(ls_svd_check(n, filter_len, peek));             // before any CUDA call
+    Batch bt;
+    TRY(stack_args(ref, srv, out, "ref/srv/out", mem_kind, n, nframes, frame_stride, &bt));
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     const int M = filter_len + peek;
-    const size_t nb = (size_t)n * sizeof(float2), mb = (size_t)M * sizeof(float2) * nframes;
-    Batch bt;
-    bt.nf = nframes;
-    bt.stride = nframes > 1 ? frame_stride : n;
-    const float2* dref = reinterpret_cast<const float2*>(ref);
-    const float2* dsrv = reinterpret_cast<const float2*>(srv);
-    float2* dout = reinterpret_cast<float2*>(out);
-    float2* dtaps = reinterpret_cast<float2*>(taps_out);
-    int* drank = rank_out;
-    if (mem_kind == PRC_MEM_HOST) {
-        TRY(c->ref.ensure(nb * nframes));
-        TRY(c->srv.ensure(nb * nframes));
-        TRY(c->clean.ensure(nb * nframes));
-        for (int fr = 0; fr < nframes; ++fr) {
-            TRY(h2d(c, c->ref.as<float2>() + (size_t)fr * n, ref + (size_t)fr * bt.stride, nb, flags));
-            TRY(h2d(c, c->srv.as<float2>() + (size_t)fr * n, srv + (size_t)fr * bt.stride, nb, flags));
-        }
-        if (taps_out) { TRY(c->lstaps.ensure(mb)); dtaps = c->lstaps.as<float2>(); }
-        dref = c->ref.as<float2>();
-        dsrv = c->srv.as<float2>();
-        dout = c->clean.as<float2>();
-        bt.stride = n;
-    }
-    if (mem_kind == PRC_MEM_HOST || !rank_out) {
-        TRY(c->svd_rank.ensure((size_t)nframes * sizeof(int)));
+    const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
+    const size_t mb = (size_t)M * sizeof(float2) * nframes, rb = (size_t)nframes * sizeof(int);
+    const float2 *dref, *dsrv;
+    float2 *dout, *dtaps;
+    TRY(stage_in(c, ref, mem_kind, nframes, nb, sb, c->ref, flags, &dref));
+    TRY(stage_in(c, srv, mem_kind, nframes, nb, sb, c->srv, flags, &dsrv));
+    TRY(stage_out(out, mem_kind, nb * nframes, c->clean, &dout));
+    TRY(stage_out(taps_out, mem_kind, mb, c->lstaps, &dtaps));
+    int* drank;
+    TRY(stage_out(rank_out, mem_kind, rb, c->svd_rank, &drank));
+    if (!rank_out) {
+        TRY(c->svd_rank.ensure(rb));
         drank = c->svd_rank.as<int>();
     }
+    if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     TRY(ls_svd_device(c, dref, dsrv, n, bt, filter_len, peek, dout, dtaps, drank));
-    if (mem_kind == PRC_MEM_HOST) {
-        const size_t fs = (size_t)(nframes > 1 ? frame_stride : n);
-        for (int fr = 0; fr < nframes; ++fr)
-            TRY(d2h(c, out + fr * fs, c->clean.as<float2>() + (size_t)fr * n, nb, flags));
-        if (taps_out) TRY(d2h(c, taps_out, c->lstaps.p, mb, flags));
-        if (rank_out) TRY(d2h(c, rank_out, drank, (size_t)nframes * sizeof(int), flags));
-    }
+    TRY(unstage(c, out, dout, mem_kind, nframes, nb, sb, flags));
+    TRY(unstage(c, taps_out, dtaps, mem_kind, 1, mb, mb, flags));
+    TRY(unstage(c, rank_out, drank, mem_kind, 1, rb, rb, flags));
     return finish(c, flags);
 }
 
