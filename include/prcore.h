@@ -264,6 +264,8 @@ int prc_direct_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
  *           reference's float32 phase ramp; PRC_MIX_C64 = phase_offset is a Python scalar (complex64
  *           arithmetic throughout), PRC_MIX_C128 = phase_offset is a NumPy float64 (main.py:127-130;
  *           the exponential is then evaluated in float64).  Results are complex64 either way.
+ * in      : I and Q are read as scalars, so `in` may sit at any raw element, odd ones included (a raw array
+ *           sliced by a channel offset, main.py:87-92).
  * prc_frontend_c64 additionally applies resample() = scipy.signal.resample_poly(x, up, down,
  * padtype='line') (signal_utils.py:15-17) in the same pass: h = the nh = 2*half_len+1 low-pass taps
  * ALREADY multiplied by up (what resample_poly hands to upfirdn; host doubles, designed by the caller
@@ -287,8 +289,8 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
                      int up, int down, const double* h, int nh, prc_c64* out, int64_t out_capacity,
                      int mem_kind, int device, void* stream, unsigned flags);
 /* prc_frontend_chunks_c64: prc_frontend_c64 on nchunks chunks of n complex samples in one launch, what main.py:105-166
- * does to every chunk of a recording.  Chunk b starts at complex sample b * chunk_stride of `in` (any element: I and Q
- * are read as scalars, so `in` itself may sit at an odd raw element), is mixed with phase_offsets[b] and resampled
+ * does to every chunk of a recording.  Chunk b starts at complex sample b * chunk_stride of `in` (which may sit at
+ * any raw element, as above), is mixed with phase_offsets[b] and resampled
  * with the line extension of its own end points.  phase_offsets is nchunks doubles in host memory whatever mem_kind
  * is; they are copied before the call returns, also with PRC_FLAG_ASYNC.  Its prc_resample_out_len() samples go to
  * out + b * out_stride (out_stride >= that length when nchunks > 1).  out_capacity counts complex samples from `out`.

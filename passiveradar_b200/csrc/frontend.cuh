@@ -1,9 +1,10 @@
-// frontend.cuh -- the per-chunk front end that feeds the hot path (SURVEY.md section 8(f).2):
+// frontend.cuh -- the arithmetic of the front end that feeds the hot path (SURVEY.md section 8(f).2):
 //   deinterleave_IQ  (reference passiveRadar/signal_utils.py:19-22)
 //   frequency_shift  (signal_utils.py:24-27, float32 phase ramp reproduced)
 //   resample         (signal_utils.py:15-17: scipy resample_poly(x, up, dn, padtype='line'))
-// and the CFAR detector behind it (detect.cuh).  All of it is bandwidth-bound element-wise / short-FIR
-// work: one pass over the raw samples, coalesced 128-bit loads, shared-memory staging of the FIR window.
+// Its one set of kernels, which run one chunk (prc_iq_mix_c64, prc_frontend_c64) or many (prc_frontend_chunks_c64),
+// is in recording.cuh, and the CFAR detector behind it in detect.cuh.  All of it is bandwidth-bound element-wise /
+// short-FIR work: one pass over the raw samples, shared-memory staging of the FIR window.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,18 +25,6 @@ struct MixParams {
     double po;           // phase offset (MIX_C64: rounded to float32 first, like numpy's weak scalar)
     double B64, rFs64;   // MIX_F64 / MIX_FS64: the same in float64 (fc or Fs was a NumPy float64 scalar)
 };
-
-__device__ __forceinline__ float2 iq_load(const void* in, int kind, long long i) {
-    if (kind == IQ_I8) {
-        const char2 v = reinterpret_cast<const char2*>(in)[i];
-        return make_float2((float)v.x, (float)v.y);
-    }
-    if (kind == IQ_I16) {
-        const short2 v = reinterpret_cast<const short2*>(in)[i];
-        return make_float2((float)v.x, (float)v.y);
-    }
-    return reinterpret_cast<const float2*>(in)[i];
-}
 
 // x[i] * exp(1j * theta_i) with numpy's evaluation order:
 //   theta32 = fl32(fl32(B * fl32(i)) * fl32(1/Fs))                                  (complex64 arange, weak python scalars)
@@ -61,71 +50,32 @@ __device__ __forceinline__ float2 mix_sample(const MixParams& p, float2 v, long 
     return make_float2(__fmaf_rn(v.x, cs, -__fmul_rn(v.y, sn)), __fmaf_rn(v.x, sn, __fmul_rn(v.y, cs)));
 }
 
-__global__ void iq_mix_kernel(const __grid_constant__ MixParams p, float2* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= p.n) return;
-    out[i] = mix_sample(p, iq_load(p.in, p.kind, i), i);
-}
-
 // ---------------------------------------------------------------------------------------------------
 // resample_poly(x, up, down, padtype='line') as one polyphase pass.
 //   y[m] = sum_k hpad[k] * xup[(m + n_pre_remove) * down - k],   xup[i * up] = xext[i]
 // hpad = n_pre_pad zeros + h (already scaled by up), xext = x extended by a line through its end points
 // (scipy _upfirdn_apply.pyx MODE_LINE: x[0] + idx * slope on the left, x[n-1] + (idx - n + 1) * slope on
 // the right, slope = (x[n-1] - x[0]) / (n - 1)).  One thread per output sample; a CTA stages the
-// polyphase taps [phase][j] and its window of (optionally mixed, optionally deinterleaved) input samples
-// in shared memory, so the raw samples are read from HBM exactly once.
+// polyphase taps [phase][j] and its window of mixed, deinterleaved input samples in shared memory, so the raw
+// samples are read from HBM exactly once.
 // ---------------------------------------------------------------------------------------------------
 struct ResampleParams {
-    MixParams mix;        // input description (mode MIX_NONE for plain resample)
+    MixParams mix;        // input description of chunk 0 (mode MIX_NONE for plain resample)
     int up, down;
-    int nh;               // taps in h (2 * half_len + 1)
     int n_pre_pad, n_pre_remove;
     int tpp;              // taps per phase = ceil((n_pre_pad + nh) / up), made odd (table row stride)
     long long n_out;
     const float* hp;      // polyphase table [up][tpp]: hp[ph][j] = hpad[ph + j * up]
-    float2 x0, x1;        // mixed end points x[0], x[n-1] (line extension); filled by resample_ends_kernel
-    const float2* ends;   // device copy of {x0, x1}
     int span;             // input samples staged per CTA
 };
 
 constexpr int RS_THREADS = 256;
 
-__global__ void resample_ends_kernel(const __grid_constant__ MixParams p, float2* __restrict__ ends) {
-    if (threadIdx.x == 0 && blockIdx.x == 0) {
-        ends[0] = mix_sample(p, iq_load(p.in, p.kind, 0), 0);
-        ends[1] = mix_sample(p, iq_load(p.in, p.kind, p.n - 1), p.n - 1);
-    }
+__device__ __forceinline__ size_t rs_table_bytes(const ResampleParams& p) {
+    return ((size_t)p.up * p.tpp * 4 + 15) & ~(size_t)15;
 }
 
-// The two halves of a resample CTA, shared by resample_kernel and the per-chunk front end (recording.cuh) so that
-// both compute every output with the same instructions.
-// rs_stage: the polyphase table and the CTA's window xext[i_lo, i_lo + span) into shared memory; returns i_lo.
-// load(i) gives the (mixed) input sample i for 0 <= i < n; x0, x1 are load(0), load(n - 1).
-template <class Load>
-__device__ __forceinline__ long long rs_stage(const ResampleParams& p, long long n, const float2* ends, float* hp,
-                                              float2* xs, Load load) {
-    const long long m0 = (long long)blockIdx.x * RS_THREADS;
-    // input index range of this CTA: output m uses i = floor(T / up) - j, j = 0 .. tpp-1, T = (m + npr) * down
-    const long long Tlo = (m0 + p.n_pre_remove) * (long long)p.down;
-    const long long i_hi0 = Tlo / p.up;                      // largest index of the first output
-    const long long i_lo = i_hi0 - (p.tpp - 1);              // smallest index any output of the CTA needs
-    for (int q = threadIdx.x; q < p.up * p.tpp; q += RS_THREADS) hp[q] = p.hp[q];
-    const float2 x0 = ends[0], x1 = ends[1];
-    // n == 1 gives 0/0 = NaN, and every output NaN, as scipy's padtype='line' does
-    const float2 slope = make_float2((x1.x - x0.x) / (float)(n - 1), (x1.y - x0.y) / (float)(n - 1));
-    for (int q = threadIdx.x; q < p.span; q += RS_THREADS) {
-        const long long i = i_lo + q;
-        float2 v;
-        if (i < 0) v = make_float2(x0.x + (float)i * slope.x, x0.y + (float)i * slope.y);
-        else if (i >= n) v = make_float2(x1.x + (float)(i - n + 1) * slope.x, x1.y + (float)(i - n + 1) * slope.y);
-        else v = load(i);
-        xs[q] = v;
-    }
-    return i_lo;
-}
-
-// rs_sum: output m of the CTA whose window rs_stage staged at i_lo
+// output m of the CTA whose window of xext starts at i_lo
 __device__ __forceinline__ float2 rs_sum(const ResampleParams& p, const float* hp, const float2* xs, long long i_lo,
                                          long long m) {
     const long long T = (m + p.n_pre_remove) * (long long)p.down;
@@ -147,22 +97,6 @@ __device__ __forceinline__ float2 rs_sum(const ResampleParams& p, const float* h
         ar = fmaf(h0, v0.x, ar); ai = fmaf(h0, v0.y, ai);
     }
     return make_float2(ar + br, ai + bi);
-}
-
-__device__ __forceinline__ size_t rs_table_bytes(const ResampleParams& p) {
-    return ((size_t)p.up * p.tpp * 4 + 15) & ~(size_t)15;
-}
-
-__global__ void __launch_bounds__(RS_THREADS) resample_kernel(const __grid_constant__ ResampleParams p, float2* __restrict__ out) {
-    extern __shared__ __align__(16) unsigned char rs_smem[];
-    float* hp = reinterpret_cast<float*>(rs_smem);                               // [up][tpp]
-    float2* xs = reinterpret_cast<float2*>(rs_smem + rs_table_bytes(p));
-    const long long i_lo = rs_stage(p, p.mix.n, p.ends, hp, xs,
-                                    [&p](long long i) { return mix_sample(p.mix, iq_load(p.mix.in, p.mix.kind, i), i); });
-    __syncthreads();
-    const long long m = (long long)blockIdx.x * RS_THREADS + threadIdx.x;
-    if (m >= p.n_out) return;
-    out[m] = rs_sum(p, hp, xs, i_lo, m);
 }
 
 }  // namespace prc

@@ -124,10 +124,10 @@ struct Ctx {
     bool own_stream = false;
     int nsm = 148;
     std::mutex mu;
-    DBuf fe_in, fe_out, fe_hp, fe_ends;            // front end: raw IQ, resampled, polyphase taps, end points
-    DBuf fe_po, fe_cends;                          // front end over chunks: phase offsets, end points of every chunk
-    DBuf cf_in, cf_cr, cf_det, cf_part;            // CFAR_2D
-    DBuf rd_in, rd_out, rd_part, rd_w;             // frame chain of range_doppler_plot.py: maps, results, CFAR partial sums, weights
+    DBuf fe_in, fe_out, fe_hp;                     // front end: raw IQ, resampled, polyphase taps
+    DBuf fe_po, fe_cends;                          // front end: phase offsets, end points of every chunk
+    DBuf rd_in, rd_out, rd_det, rd_part, rd_w;     // CFAR_2D and the frame chain of range_doppler_plot.py: maps, results,
+                                                   // detections, CFAR partial sums, weights
     uint64_t fe_hp_key = 0;                        // which taps fe_hp holds
     DBuf rs, clean2;          // LS_Filter_Toeplitz: rolled / frequency-shifted reference, ping-pong output
     DBuf refw, ref, srv, out, clean, partial, win32, win64, dtaps32, dtaps64, lstaps, tw, pbuf, status,
@@ -154,8 +154,8 @@ struct Ctx {
         for (DBuf& b : fft_tw) b.release();
         for (bool& r : fft_tw_ready) r = false;
         for (DBuf* b : {&wp_fir, &wp_caf, &fftP, &fpacc}) b->release();
-        for (DBuf* b : {&fe_in, &fe_out, &fe_hp, &fe_ends, &fe_po, &fe_cends, &cf_in, &cf_cr, &cf_det, &cf_part,
-                        &rd_in, &rd_out, &rd_part, &rd_w}) b->release();
+        for (DBuf* b : {&fe_in, &fe_out, &fe_hp, &fe_po, &fe_cends, &rd_in, &rd_out, &rd_det, &rd_part, &rd_w})
+            b->release();
         for (DBuf* b : {&refw, &ref, &srv, &out, &clean, &partial, &win32, &win64, &dtaps32, &dtaps64, &lstaps,
                         &tw, &pbuf, &status, &nl_init, &nl_taps, &gal_k, &gal_h, &trk_map, &trk_plan, &trk_stats,
                         &trk_slots, &trk_out, &trk_cnt, &svd_part, &svd_cr, &svd_ws, &svd_taps, &svd_rank})
@@ -909,12 +909,6 @@ MixParams make_mix(const void* in, int kind, long long n, int mode, double fc, d
     return m;
 }
 
-int mix_device(Ctx* c, const MixParams& m, float2* out) {
-    ProfScope ps(c, K_MISC);
-    iq_mix_kernel<<<ceil_div(m.n, 256), 256, 0, c->stream>>>(m, out);
-    return check_launch("iq_mix_kernel");
-}
-
 // scipy.signal.resample_poly(x, up, down, padtype='line') geometry (scipy/signal/_signaltools.py, resample_poly)
 struct ResampleGeo { int up, down, n_pre_pad, n_pre_remove, tpp; long long n_out; };
 
@@ -933,11 +927,11 @@ int resample_geo(long long n_in, int up, int down, int nh, ResampleGeo* g) {
     return PRC_OK;
 }
 
-// The geometry, shared-memory check and polyphase table of one resample CTA (resample_kernel and
-// rec_resample_kernel).  h: host doubles (already multiplied by `up`, as resample_poly does before upfirdn).
+// The geometry, shared-memory check and polyphase table of one resample CTA.  h: host doubles (already multiplied by
+// `up`, as resample_poly does before upfirdn).
 int resample_table(Ctx* c, const ResampleGeo& g, const double* h, int nh, ResampleParams* out, size_t* smem_out) {
     ResampleParams& rp = *out;
-    rp.up = g.up; rp.down = g.down; rp.nh = nh;
+    rp.up = g.up; rp.down = g.down;
     rp.n_pre_pad = g.n_pre_pad; rp.n_pre_remove = g.n_pre_remove; rp.tpp = g.tpp;
     rp.n_out = g.n_out;
     rp.span = (int)(((long long)(RS_THREADS - 1) * g.down) / g.up) + 2 + g.tpp;
@@ -968,136 +962,76 @@ int resample_table(Ctx* c, const ResampleGeo& g, const double* h, int nh, Resamp
     return PRC_OK;
 }
 
-int resample_device(Ctx* c, const MixParams& mix, int up_in, int down_in, const double* h, int nh, float2* out,
-                    long long* n_out) {
-    ResampleGeo g;
-    TRY(resample_geo(mix.n, up_in, down_in, nh, &g));
-    if (mix.n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", mix.n);
-    if (n_out) *n_out = g.n_out;
-    if (g.up == 1 && g.down == 1) {           // resample_poly returns a copy
-        return mix_device(c, mix, out);
-    }
-    ResampleParams rp{};
-    size_t smem = 0;
-    TRY(resample_table(c, g, h, nh, &rp, &smem));
-    rp.mix = mix;
-    TRY(c->fe_ends.ensure(2 * sizeof(float2)));
-    rp.ends = c->fe_ends.as<float2>();
-    static std::atomic<bool> attr_set[64];
-    if (!attr_set[c->device].exchange(true))
-        CU(cudaFuncSetAttribute(resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT));
-    {
-        ProfScope ps(c, K_MISC);
-        resample_ends_kernel<<<1, 32, 0, c->stream>>>(mix, c->fe_ends.as<float2>());
-        resample_kernel<<<ceil_div(g.n_out, RS_THREADS), RS_THREADS, smem, c->stream>>>(rp, out);
-    }
-    return check_launch("resample_kernel");
-}
-
-// resample_device on nchunks chunks of mix.n samples each, chunk b at raw sample b * chunk_stride of mix.in, mixed
-// with phase offset po[b] (device doubles), its output at out + b * out_stride (recording.cuh)
-int frontend_chunks_device(Ctx* c, const MixParams& mix, int nchunks, long long chunk_stride, const double* po,
-                           int up_in, int down_in, const double* h, int nh, float2* out, long long out_stride) {
-    ResampleGeo g;
-    TRY(resample_geo(mix.n, up_in, down_in, nh, &g));
+// nchunks chunks of mix.n samples each, chunk b at raw sample b * chunk_stride of mix.in, mixed with phase offset po[b]
+// (device doubles; NULL: mix.po, for a single chunk), its output at out + b * out_stride (recording.cuh)
+rec::ChunkParams chunk_params(const MixParams& mix, int nchunks, long long chunk_stride, const double* po, long long out_stride) {
     rec::ChunkParams p{};
     p.rs.mix = mix;
-    p.rs.n_out = g.n_out;
     p.chunk_bytes = (long long)iq_bytes(mix.kind, chunk_stride);
     p.out_stride = out_stride;
     p.po = po;
     p.nchunks = nchunks;
-    if (g.up == 1 && g.down == 1) {           // resample_poly returns a copy
-        ProfScope ps(c, K_FRONTEND_CHUNKS);
-        rec::launch_mix(p, out, c->stream);
-        return check_launch("rec_mix_kernel");
-    }
+    return p;
+}
+
+// deinterleave_IQ + frequency_shift of the chunks: all of the front end when up == down == 1 (resample_poly returns a
+// copy), and all a mix alone needs (no taps)
+int mix_chunks_device(Ctx* c, KernelId kid, const rec::ChunkParams& p, float2* out) {
+    ProfScope ps(c, kid);
+    rec::launch_mix(p, out, c->stream);
+    return check_launch("rec_mix_kernel");
+}
+
+int frontend_device(Ctx* c, KernelId kid, rec::ChunkParams p, const ResampleGeo& g, const double* h, int nh, float2* out) {
+    if (g.up == 1 && g.down == 1) return mix_chunks_device(c, kid, p, out);
     size_t smem = 0;
     TRY(resample_table(c, g, h, nh, &p.rs, &smem));
-    TRY(c->fe_cends.ensure((size_t)nchunks * 2 * sizeof(float2)));
+    TRY(c->fe_cends.ensure((size_t)p.nchunks * 2 * sizeof(float2)));
     p.ends = c->fe_cends.as<float2>();
     static std::atomic<bool> attr_set[64];
     if (!attr_set[c->device].exchange(true)) CU(rec::allow_smem((int)SMEM_LIMIT));
     {
-        ProfScope ps(c, K_FRONTEND_CHUNKS);
+        ProfScope ps(c, kid);
         rec::launch_resample(p, smem, out, c->stream);
     }
     return check_launch("rec_resample_kernel");
 }
 
 // ---- CFAR_2D (detect.cuh) -----------------------------------------------------------------------
-int cfar_device(Ctx* c, const void* x, bool is_complex, int rows, int cols, int fw, int gw, const float* thresh,
-                float* cr, uint8_t* det) {
+// CFAR_2D's limits, messages and window geometry
+int cfar_window(int rows, int cols, int fw, int gw, CfarParams* p) {
     if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
     if (rows > CFAR_MAX_ROWS)          // one CTA row of tiles per gridDim.y index
         return fail(PRC_E_INVALID, "rows=%d exceed the CFAR maximum of %d rows", rows, CFAR_MAX_ROWS);
     if (fw < 1 || fw > CFAR_MAX_FW) return fail(PRC_E_INVALID, "fw=%d outside [1, %d]", fw, CFAR_MAX_FW);
     if (gw < 0 || fw * fw - gw * gw == 0) return fail(PRC_E_INVALID, "fw=%d gw=%d: fw^2 - gw^2 must not be 0", fw, gw);
-    TRY(c->cf_part.ensure(CFAR_MEAN_CTAS * sizeof(double)));
-    CfarParams p{};
-    p.x = x; p.is_complex = is_complex ? 1 : 0; p.rows = rows; p.cols = cols;
-    p.fw = fw;
+    *p = CfarParams{};
+    p->rows = rows; p->cols = cols; p->fw = fw;
     // python: e1 = (fw - gw) // 2 (floor), e2 = fw - e1 + 1; slices clip to [0, fw]
     int e1 = (fw - gw) >= 0 ? (fw - gw) / 2 : -((gw - fw + 1) / 2);
     int e2 = fw - e1 + 1;
     if (e1 < 0) e1 = std::max(0, e1 + fw);     // negative slice start counts from the end
-    p.e1 = std::min(e1, fw); p.e2 = std::min(std::max(e2, 0), fw);
-    p.c = (fw - 1) / 2;
-    p.scale = 1.0 / ((double)fw * fw - (double)gw * gw);
-    p.has_thresh = thresh ? 1 : 0;
-    p.thresh = thresh ? *thresh : 0.f;
-    p.partial = c->cf_part.as<double>();
-    p.cr = cr; p.det = det;
-    ProfScope ps(c, K_MISC);
-    cfar_abssum_kernel<<<CFAR_MEAN_CTAS, 256, 0, c->stream>>>(p, c->cf_part.as<double>());
-    const size_t smem = (size_t)(CFAR_TX + fw - 1) * (CFAR_TY + fw - 1) * sizeof(double);   // 53 960 B at fw = 64
-    {   // under a lock: a concurrent first call must not launch before the attribute is set
-        static std::mutex attr_mu;
-        static bool attr_set[64];
-        std::lock_guard<std::mutex> g(attr_mu);
-        if (!attr_set[c->device]) {
-            CU(cudaFuncSetAttribute(cfar2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_LIMIT));
-            attr_set[c->device] = true;
-        }
-    }
-    cfar2d_kernel<<<dim3(ceil_div(cols, CFAR_TX), ceil_div(rows, CFAR_TY)), dim3(CFAR_TX, CFAR_TY), smem, c->stream>>>(p);
-    return check_launch("cfar2d_kernel");
-}
-
-// ---- frame chain of range_doppler_plot.py:45-85 (render.cuh) --------------------------------------------------------
-// CFAR_2D's limits, messages and window geometry, as cfar_device sets them
-int cfar_window(int rows, int cols, int fw, int gw, CfarParams* p) {
-    if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
-    if (rows > CFAR_MAX_ROWS)
-        return fail(PRC_E_INVALID, "rows=%d exceed the CFAR maximum of %d rows", rows, CFAR_MAX_ROWS);
-    if (fw < 1 || fw > CFAR_MAX_FW) return fail(PRC_E_INVALID, "fw=%d outside [1, %d]", fw, CFAR_MAX_FW);
-    if (gw < 0 || fw * fw - gw * gw == 0) return fail(PRC_E_INVALID, "fw=%d gw=%d: fw^2 - gw^2 must not be 0", fw, gw);
-    *p = CfarParams{};
-    p->rows = rows; p->cols = cols; p->fw = fw;
-    int e1 = (fw - gw) >= 0 ? (fw - gw) / 2 : -((gw - fw + 1) / 2);
-    int e2 = fw - e1 + 1;
-    if (e1 < 0) e1 = std::max(0, e1 + fw);
     p->e1 = std::min(e1, fw); p->e2 = std::min(std::max(e2, 0), fw);
     p->c = (fw - 1) / 2;
     p->scale = 1.0 / ((double)fw * fw - (double)gw * gw);
     return PRC_OK;
 }
 
-int cfar_frames_device(Ctx* c, rdr::CfarFramesParams& f, int nframes) {
+int cfar_frames_device(Ctx* c, KernelId kid, CfarParams& p, int nframes) {
     TRY(c->rd_part.ensure((size_t)nframes * CFAR_MEAN_CTAS * sizeof(double)));
-    f.partial = c->rd_part.as<double>();
+    p.partial = c->rd_part.as<double>();
     {   // under a lock: a concurrent first call must not launch before the attribute is set
         static std::mutex attr_mu;
         static bool attr_set[64];
         std::lock_guard<std::mutex> g(attr_mu);
         if (!attr_set[c->device]) {
-            CU(rdr::allow_smem((int)SMEM_LIMIT));
+            CU(allow_cfar_smem((int)SMEM_LIMIT));
             attr_set[c->device] = true;
         }
     }
     {
-        ProfScope ps(c, K_CFAR_FRAMES);
-        rdr::launch_cfar(f, nframes, c->stream);
+        ProfScope ps(c, kid);
+        launch_cfar(p, nframes, c->stream);
     }
     return check_launch("cfar_frames_kernel");
 }
@@ -1117,7 +1051,7 @@ int direct_xambg_device(Ctx* c, const float2* ref, const float2* srv, long long 
     for (int f = 0; f < F; ++f) {
         const double df = ((double)f - 0.5 * (double)F) / cpi;
         const MixParams m = make_mix(ref, IQ_C64, n, MIX_C64, df, fs, 0.0);
-        TRY(mix_device(c, m, c->rs.as<float2>()));
+        TRY(mix_chunks_device(c, K_MISC, chunk_params(m, 1, 0, nullptr, 0), c->rs.as<float2>()));
         LagStreamParams sp{};
         sp.x = c->rs.as<float2>();
         sp.s[0] = srv; sp.s[1] = srv;
@@ -2309,7 +2243,8 @@ int prc_iq_mix_c64(const void* in, int in_kind, int64_t n, int mode, double fc, 
     float2* dout;
     TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
     TRY(stage_out(out, mem_kind, ob, c->fe_out, &dout));
-    TRY(mix_device(c, make_mix(din, in_kind, n, mode, fc, fs, phase_offset), dout));
+    TRY(mix_chunks_device(c, K_MISC, chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset), 1, 0, nullptr, 0),
+                          dout));
     TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
 }
@@ -2338,9 +2273,9 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
     float2* dout;
     TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
     TRY(stage_out(out, mem_kind, (size_t)g.n_out * sizeof(float2), c->fe_out, &dout));
-    long long n_out = 0;
-    TRY(resample_device(c, make_mix(din, in_kind, n, mode, fc, fs, phase_offset), up, down, h, nh, dout, &n_out));
-    TRY(unstage(c, out, dout, mem_kind, 1, (size_t)n_out * sizeof(float2), (size_t)n_out * sizeof(float2), flags));
+    TRY(frontend_device(c, K_MISC, chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset), 1, 0, nullptr, 0), g,
+                        h, nh, dout));
+    TRY(unstage(c, out, dout, mem_kind, 1, (size_t)g.n_out * sizeof(float2), (size_t)g.n_out * sizeof(float2), flags));
     return finish(c, flags);
 }
 
@@ -2370,8 +2305,10 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
     TRY(stage_out(out, mem_kind, nchunks * cb, c->fe_out, &dout));
     const long long dstride = mem_kind == PRC_MEM_HOST ? g.n_out : ostride;      // staged chunks are packed
     TRY(copy_params(c, phase_offsets, nchunks, c->fe_po));
-    TRY(frontend_chunks_device(c, make_mix(din, in_kind, n, mode, fc, fs, 0.0), nchunks, cstride, c->fe_po.as<double>(),
-                               up, down, h, nh, dout, dstride));
+    TRY(frontend_device(c, K_FRONTEND_CHUNKS,
+                        chunk_params(make_mix(din, in_kind, n, mode, fc, fs, 0.0), nchunks, cstride, c->fe_po.as<double>(),
+                                     dstride),
+                        g, h, nh, dout));
     TRY(unstage(c, out, dout, mem_kind, nchunks, cb, (size_t)ostride * sizeof(float2), flags));
     return finish(c, flags);
 }
@@ -2381,21 +2318,21 @@ int prc_cfar2d_f32(const void* x, int rows, int cols, int fw, int gw, const floa
     if (!x || (!cr_out && !det_out)) return fail(PRC_E_INVALID, "x and one of cr_out/det_out must not be NULL");
     if (det_out && !thresh) return fail(PRC_E_INVALID, "det_out needs a threshold");
     if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    if (rows < 1 || cols < 1) return fail(PRC_E_INVALID, "rows=%d cols=%d invalid", rows, cols);
+    CfarParams p;
+    TRY(cfar_window(rows, cols, fw, gw, &p));
     const bool cplx = (flags & PRC_FLAG_ABS_C64) != 0;
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     const size_t cells = (size_t)rows * cols, inb = cells * (cplx ? sizeof(float2) : sizeof(float));
-    const void* dx;
-    float* dcr;
-    uint8_t* ddet;
-    TRY(stage_in(c, x, mem_kind, 1, inb, inb, c->cf_in, flags, &dx));
-    TRY(stage_out(cr_out, mem_kind, cells * sizeof(float), c->cf_cr, &dcr));
-    TRY(stage_out(det_out, mem_kind, cells, c->cf_det, &ddet));
-    TRY(cfar_device(c, dx, cplx, rows, cols, fw, gw, thresh, dcr, ddet));
-    TRY(unstage(c, cr_out, dcr, mem_kind, 1, cells * sizeof(float), cells * sizeof(float), flags));
-    TRY(unstage(c, det_out, ddet, mem_kind, 1, cells, cells, flags));
+    TRY(stage_in(c, x, mem_kind, 1, inb, inb, c->rd_in, flags, &p.x));
+    TRY(stage_out(cr_out, mem_kind, cells * sizeof(float), c->rd_out, &p.cr));
+    TRY(stage_out(det_out, mem_kind, cells, c->rd_det, &p.det));
+    p.is_complex = cplx ? 1 : 0;
+    p.thresh = thresh ? *thresh : 0.f;
+    TRY(cfar_frames_device(c, K_MISC, p, 1));
+    TRY(unstage(c, cr_out, p.cr, mem_kind, 1, cells * sizeof(float), cells * sizeof(float), flags));
+    TRY(unstage(c, det_out, p.det, mem_kind, 1, cells, cells, flags));
     return finish(c, flags);
 }
 
@@ -2403,8 +2340,8 @@ int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t fr
                       void* cr_out, int64_t cr_stride, int mem_kind, int device, void* stream, unsigned flags) {
     if (!x || !cr_out) return fail(PRC_E_INVALID, "x and cr_out must not be NULL");
     if (bad_mem_kind(mem_kind)) return fail(PRC_E_INVALID, "mem_kind=%d invalid", mem_kind);
-    rdr::CfarFramesParams f{};
-    TRY(cfar_window(rows, cols, fw, gw, &f.p));
+    CfarParams p;
+    TRY(cfar_window(rows, cols, fw, gw, &p));
     if (nframes < 0 || nframes > 65535) return fail(PRC_E_INVALID, "nframes=%d outside [0, 65535]", nframes);
     const long long cells = (long long)rows * cols;
     if (nframes > 1 && (frame_stride < cells || cr_stride < cells))
@@ -2417,14 +2354,14 @@ int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t fr
     if (nframes == 0) return finish(c, flags);
     const size_t ine = cplx ? sizeof(float2) : sizeof(float), oute = f64 ? sizeof(double) : sizeof(float);
     const long long xs = nframes > 1 ? frame_stride : cells, os = nframes > 1 ? cr_stride : cells;
-    TRY(stage_in(c, x, mem_kind, nframes, cells * ine, xs * ine, c->rd_in, flags, &f.p.x));
-    TRY(stage_out(cr_out, mem_kind, (size_t)nframes * cells * oute, c->rd_out, &f.cr));
-    f.p.is_complex = cplx ? 1 : 0;
-    f.frame_stride = mem_kind == PRC_MEM_HOST ? cells : xs;      // staged frames are packed
-    f.cr_stride = mem_kind == PRC_MEM_HOST ? cells : os;
-    f.cr_f64 = f64 ? 1 : 0;
-    TRY(cfar_frames_device(c, f, nframes));
-    TRY(unstage(c, cr_out, f.cr, mem_kind, nframes, cells * oute, os * oute, flags));
+    TRY(stage_in(c, x, mem_kind, nframes, cells * ine, xs * ine, c->rd_in, flags, &p.x));
+    TRY(stage_out(cr_out, mem_kind, (size_t)nframes * cells * oute, c->rd_out, &p.cr));
+    p.is_complex = cplx ? 1 : 0;
+    p.frame_stride = mem_kind == PRC_MEM_HOST ? cells : xs;      // staged frames are packed
+    p.out_stride = mem_kind == PRC_MEM_HOST ? cells : os;
+    p.cr_f64 = f64 ? 1 : 0;
+    TRY(cfar_frames_device(c, K_CFAR_FRAMES, p, nframes));
+    TRY(unstage(c, cr_out, p.cr, mem_kind, nframes, cells * oute, os * oute, flags));
     return finish(c, flags);
 }
 

@@ -1,10 +1,7 @@
-// render.cuh -- the frame chain of range_doppler_plot.py:45-85 (DESIGN.md section 15): CFAR_2D of every frame of a
-// stack, the reference's persistence (passiveRadar/plotting_tools.py:9-30) along the frame axis, and the two
+// render.cuh -- the frame chain of range_doppler_plot.py:45-85 (DESIGN.md section 15) after CFAR_2D of every frame
+// (detect.cuh): the reference's persistence (passiveRadar/plotting_tools.py:9-30) along the frame axis, and the two
 // per-frame percentiles that set the colour limits.
 //
-// cfar_frames_*: detect.cuh's CFAR_2D with the frame on a grid dimension.  Each frame is summed over the same 64-CTA
-//   partition and tiled with the same window order as cfar_abssum_kernel / cfar2d_kernel, so its float32 CR is bit-
-//   identical to a prc_cfar2d_f32 call on that frame; the float64 CR the division forms can be written instead.
 // pst_kernel: out[k] = sum_{i < min(k + 1, hold)} X[k - i] * w[i], summed from +0.0 in the order i = 0, 1, ... with
 //   separate multiplies and adds (no contraction), the products in float32 when NumPy's promotion makes them so.  One
 //   thread per cell walks the frames in order and keeps the last PST_RING inputs of its cell in shared memory, so an
@@ -16,104 +13,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#include "detect.cuh"
 #include "track.cuh"
 
 namespace prc {
 namespace rdr {
-
-// ---- batched CFAR_2D ---------------------------------------------------------------------------------------------
-struct CfarFramesParams {
-    CfarParams p;              // frame 0: p.x and the window; p.partial, p.cr, p.det and the threshold are unused
-    long long frame_stride;    // elements (float, or float2 with p.is_complex) from one frame's map to the next
-    double* partial;           // [nframes][CFAR_MEAN_CTAS] partial sums of |x|
-    void* cr;                  // float, or double with cr_f64
-    long long cr_stride;       // elements from one frame's CR to the next
-    int cr_f64;
-};
-
-__device__ __forceinline__ CfarParams cfar_frame(const CfarFramesParams& f, int b) {
-    CfarParams q = f.p;
-    q.x = static_cast<const char*>(f.p.x) + (size_t)b * f.frame_stride * (f.p.is_complex ? sizeof(float2) : sizeof(float));
-    return q;
-}
-
-// cfar_abssum_kernel on frame blockIdx.y
-__global__ void cfar_frames_abssum_kernel(const __grid_constant__ CfarFramesParams f) {
-    __shared__ double red[256];
-    const CfarParams p = cfar_frame(f, blockIdx.y);
-    const long long total = (long long)p.rows * p.cols;
-    const long long per = (total + gridDim.x - 1) / gridDim.x;
-    const long long lo = blockIdx.x * per;
-    long long hi = lo + per;
-    if (hi > total) hi = total;
-    double s = 0.0;
-    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-        float v;
-        if (p.is_complex) {
-            const float2 z = reinterpret_cast<const float2*>(p.x)[i];
-            v = hypotf(z.x, z.y);
-        } else {
-            v = fabsf(reinterpret_cast<const float*>(p.x)[i]);
-        }
-        s += (double)v;
-    }
-    red[threadIdx.x] = s;
-    __syncthreads();
-    for (int w = blockDim.x / 2; w > 0; w >>= 1) {
-        if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) f.partial[(size_t)blockIdx.y * CFAR_MEAN_CTAS + blockIdx.x] = red[0];
-}
-
-// cfar2d_kernel on frame blockIdx.z
-__global__ void __launch_bounds__(CFAR_TX * CFAR_TY) cfar_frames_kernel(const __grid_constant__ CfarFramesParams f) {
-    extern __shared__ double rdr_tile[];               // [(TY + fw - 1)][(TX + fw - 1)]
-    __shared__ double s_inv_mean;
-    const int b = blockIdx.z;
-    const CfarParams p = cfar_frame(f, b);
-    const int fw = p.fw;
-    const int tw = CFAR_TX + fw - 1, th = CFAR_TY + fw - 1;
-    const int i0 = blockIdx.y * CFAR_TY, j0 = blockIdx.x * CFAR_TX;
-    const int tid = threadIdx.y * CFAR_TX + threadIdx.x;
-    if (tid == 0) {
-        const double* part = f.partial + (size_t)b * CFAR_MEAN_CTAS;
-        double s = 0.0;
-        for (int q = 0; q < CFAR_MEAN_CTAS; ++q) s += part[q];
-        s_inv_mean = (double)p.rows * (double)p.cols / s;
-    }
-    const int rbase = i0 + p.c - (fw - 1), cbase = j0 + p.c - (fw - 1);
-    for (int q = tid; q < tw * th; q += CFAR_TX * CFAR_TY) {
-        const int tr = q / tw, tc = q - tr * tw;
-        int r = (rbase + tr) % p.rows;
-        if (r < 0) r += p.rows;
-        int cc = (cbase + tc) % p.cols;
-        if (cc < 0) cc += p.cols;
-        rdr_tile[q] = cfar_load(p, r, cc);
-    }
-    __syncthreads();
-    const int i = i0 + threadIdx.y, j = j0 + threadIdx.x;
-    if (i >= p.rows || j >= p.cols) return;
-    double acc = 0.0;
-    for (int a = 0; a < fw; ++a) {
-        const double* row = rdr_tile + (threadIdx.y + fw - 1 - a) * tw + threadIdx.x + fw - 1;
-        const bool hole_row = a >= p.e1 && a < p.e2;
-        double racc = 0.0;
-        for (int bb = 0; bb < fw; ++bb) {
-            if (hole_row && bb >= p.e1 && bb < p.e2) continue;
-            racc += row[-bb];
-        }
-        acc += racc;
-    }
-    const double xv = rdr_tile[(threadIdx.y + fw - 1 - p.c) * tw + threadIdx.x + fw - 1 - p.c];
-    double num = xv;
-    if (!p.is_complex) num = reinterpret_cast<const float*>(p.x)[(size_t)i * p.cols + j];
-    const double cr = (num * s_inv_mean) / (acc * p.scale + 1e-10);
-    const size_t o = (size_t)b * f.cr_stride + (size_t)i * p.cols + j;
-    if (f.cr_f64) static_cast<double*>(f.cr)[o] = cr;
-    else static_cast<float*>(f.cr)[o] = (float)cr;
-}
 
 // ---- persistence -------------------------------------------------------------------------------------------------
 constexpr int PST_TX = 32, PST_TY = 8;
@@ -299,18 +202,6 @@ __global__ void __launch_bounds__(PCT_THREADS) pct_kernel(const __grid_constant_
 }
 
 // ---- launches (host side; prcore.cu brackets them with its profiling scope and checks the launch) ----------------
-inline cudaError_t allow_smem(int bytes) {
-    return cudaFuncSetAttribute(cfar_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-}
-
-inline void launch_cfar(const CfarFramesParams& f, int nframes, cudaStream_t st) {
-    cfar_frames_abssum_kernel<<<dim3(CFAR_MEAN_CTAS, (unsigned)nframes), 256, 0, st>>>(f);
-    const size_t smem = (size_t)(CFAR_TX + f.p.fw - 1) * (CFAR_TY + f.p.fw - 1) * sizeof(double);
-    const dim3 grid((unsigned)((f.p.cols + CFAR_TX - 1) / CFAR_TX), (unsigned)((f.p.rows + CFAR_TY - 1) / CFAR_TY),
-                    (unsigned)nframes);
-    cfar_frames_kernel<<<grid, dim3(CFAR_TX, CFAR_TY), smem, st>>>(f);
-}
-
 inline void launch_persistence(const PersistParams& p, cudaStream_t st) {
     const dim3 grid((unsigned)((p.cols + PST_TX - 1) / PST_TX), (unsigned)((p.rows + PST_TY - 1) / PST_TY));
     pst_kernel<<<grid, dim3(PST_TX, PST_TY), 0, st>>>(p);

@@ -53,29 +53,34 @@ def main():
         pass
     res = {"hbm_peak_GBps": hbm}
 
-    # ---- front end: one main.py chunk, int8 IQ -> mix -> 13/119 resample
+    # ---- front end: one main.py chunk, IQ -> mix -> 13/119 resample, and the mix alone; int8 is what main.py reads,
+    # int16 and float32 load I and Q as wider scalars
     n = 9_600_000
-    iq = torch.from_numpy(synth.raw_iq(n, "int8", 1)).to(dev)
     h = _resample_taps(13, 119, False)
     n_out = (n * 13 + 118) // 119
     out = torch.empty(n_out, dtype=torch.complex64, device=dev)
-
-    def fe():
-        _lib.check(lib.prc_frontend_c64(iq.data_ptr(), _lib.IQ_I8, n, _lib.MIX_C128, 300e3, 2.4e6, 0.7, 13, 119,
-                                        h.ctypes.data, h.shape[0], out.data_ptr(), n_out, _lib.MEM_DEVICE, 0, st, _lib.FLAG_ASYNC))
-    us = timeit(fe, args.reps)
-    alg = 2 * n + 8 * n_out
-    res["frontend_int8_9.6M"] = {"us": round(us, 1), "alg_bytes": alg, "alg_GBps": round(alg / us / 1e3, 1),
-                                 "frac_hbm": round(alg / us / 1e3 / hbm, 4), "Msamples_in_per_s": round(n / us, 1)}
     x64 = torch.empty(n, dtype=torch.complex64, device=dev)
+    for name, kind, ib in (("int8", _lib.IQ_I8, 2), ("int16", _lib.IQ_I16, 4), ("float32", _lib.IQ_C64, 8)):
+        iq = torch.from_numpy(synth.raw_iq(n, name, 1)).to(dev)
 
-    def mix():
-        _lib.check(lib.prc_iq_mix_c64(iq.data_ptr(), _lib.IQ_I8, n, _lib.MIX_C128, 300e3, 2.4e6, 0.7, x64.data_ptr(),
-                                      _lib.MEM_DEVICE, 0, st, _lib.FLAG_ASYNC))
-    us = timeit(mix, args.reps)
-    alg = 2 * n + 8 * n
-    res["iq_mix_int8_9.6M"] = {"us": round(us, 1), "alg_bytes": alg, "alg_GBps": round(alg / us / 1e3, 1),
-                               "frac_hbm": round(alg / us / 1e3 / hbm, 4)}
+        def fe():
+            _lib.check(lib.prc_frontend_c64(iq.data_ptr(), kind, n, _lib.MIX_C128, 300e3, 2.4e6, 0.7, 13, 119,
+                                            h.ctypes.data, h.shape[0], out.data_ptr(), n_out, _lib.MEM_DEVICE, 0, st,
+                                            _lib.FLAG_ASYNC))
+        us = timeit(fe, args.reps)
+        alg = ib * n + 8 * n_out
+        res[f"frontend_{name}_9.6M"] = {"us": round(us, 1), "alg_bytes": alg, "alg_GBps": round(alg / us / 1e3, 1),
+                                        "frac_hbm": round(alg / us / 1e3 / hbm, 4),
+                                        "Msamples_in_per_s": round(n / us, 1)}
+
+        def mix():
+            _lib.check(lib.prc_iq_mix_c64(iq.data_ptr(), kind, n, _lib.MIX_C128, 300e3, 2.4e6, 0.7, x64.data_ptr(),
+                                          _lib.MEM_DEVICE, 0, st, _lib.FLAG_ASYNC))
+        us = timeit(mix, args.reps)
+        alg = ib * n + 8 * n
+        res[f"iq_mix_{name}_9.6M"] = {"us": round(us, 1), "alg_bytes": alg, "alg_GBps": round(alg / us / 1e3, 1),
+                                      "frac_hbm": round(alg / us / 1e3 / hbm, 4)}
+        del iq
 
     # ---- CFAR on a config-2 map
     rows, cols = 256, 301

@@ -484,6 +484,8 @@ def test_caf_wave_grid_is_bit_identical(n, F, R):
 
 # ------------------------------------------------------------------ CPU guard: every launch site is covered
 # (host function, kernel<template arguments>) of every launch in prcore.cu -> [(test id, variant, what it reaches)].
+# The launches in the headers' own launchers are covered where those headers are tested: the front end's in
+# tests/test_recording.py, CFAR_2D's and the frame chain's in tests/test_render.py.
 # Variant: "default" (shipped configuration), "fft" / "direct" (the both_paths fixture), or a VARIANTS child.
 # A row is checked against the source, not the other way round: read the dispatch code before adding one.
 PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/test_kernel_variants.py::"
@@ -550,26 +552,6 @@ COVERAGE = {
                                                     (VARIANT_TEST, "default", "ls_big, frame at config 2")],
     "ls_toeplitz_device: shift_roll_kernel": [(VARIANT_TEST, "default", "toep"),
                                               (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins")],
-    "mix_device: iq_mix_kernel": [
-        (FE + "test_frequency_shift_follows_numpy_promotion", "default", ""),
-        (RS + "test_frequency_shift_and_frontend_past_2_24_samples", "default", "2^25 + 12345 samples, MIX_C64 and MIX_C128"),
-        (RS + "test_direct_xambg_shapes", "default", "one mix per Doppler bin, F = 1 .. 32")],
-    "resample_device: resample_ends_kernel": [(FE + "test_resample_matches_reference_golden", "default", ""),
-                                              (RS + "test_resample_short_inputs", "default", "n = 1 (NaN as SciPy), 2, 3, 27")],
-    "resample_device: resample_kernel": [
-        (FE + "test_resample_matches_reference_golden", "default", ""),
-        (RS + "test_resample_ratio_grid", "default", "42 ratios of {1, 2, 3, 5, 7, 13, 119}; complex64, complex128, float64"),
-        (RS + "test_resample_cta_boundaries", "default", "n_out = 255 .. 513 at 13/119 and 3/2"),
-        (RS + "test_resample_shared_memory_limit", "default", "1/89 and 2/171 fit, 1/90 and 2/173 are refused"),
-        (RS + "test_frontend_mix_modes", "default", "int8 / int16 / float32 IQ in MIX_F64, MIX_FS64, MIX_C64, MIX_C128")],
-    "cfar_device: cfar_abssum_kernel": [(FE + "test_cfar_matches_reference_golden", "default", ""),
-                                        (RS + "test_cfar_map_contents_match_oracle", "default", "real maps and |x| of complex maps")],
-    "cfar_device: cfar2d_kernel": [
-        (FE + "test_cfar_matches_reference_golden", "default", ""),
-        (RS + "test_cfar_fw_gw_grid_matches_oracle", "default", "fw = 1 .. 64, gw below, at and above fw"),
-        (RS + "test_cfar_map_sizes_match_oracle", "default", "1 x 1 .. 2048 x 301, maps smaller than the tile and than fw"),
-        (RS + "test_cfar_map_contents_match_oracle", "default", "signed, float64, complex (PRC_FLAG_ABS_C64), zero plateaus"),
-        (RS + "test_cfar_row_limit", "default", "the tallest map, 524 280 rows")],
     "direct_xambg_device: piece_sum_kernel": [
         (FE + "test_direct_xambg_matches_reference_golden", "default", ""),
         (RS + "test_direct_xambg_shapes", "default", "R >= n, F = 1, odd F, n = 2^18"),
@@ -633,9 +615,9 @@ def _is_gpu_test(test_id):
     return re.search(r"^pytestmark = pytest\.mark\.gpu$", src, re.M) is not None or "@pytest.mark.gpu" in decorators
 
 
-def test_every_launch_site_has_a_covering_gpu_test():
+def test_every_prcore_launch_site_has_a_covering_gpu_test():
     sites = launch_sites()
-    assert len(sites) == 46
+    assert len(sites) == 41
     missing = sorted(set(sites) - set(COVERAGE))
     stale = sorted(set(COVERAGE) - set(sites))
     assert not missing, "launch sites of prcore.cu without a covering test in COVERAGE: " + \

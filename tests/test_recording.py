@@ -137,25 +137,41 @@ def test_recording_kernels_build_for_sm90a_without_spills():
         assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in blk
 
 
-# every launch in recording.cuh -> the GPU tests that reach it
+# every launch in recording.cuh -> the GPU tests that reach it (a test of this file, or "tests/<file>::<test>")
+FE, RS = "tests/test_gpu_frontend.py::", "tests/test_rows_sweep.py::"
 COVERAGE = {
-    "rec_ends_kernel": ["test_frontend_chunks_bit_identical_to_per_chunk_calls", "test_pipeline_matches_oracle_chain"],
+    "rec_ends_kernel": ["test_frontend_chunks_bit_identical_to_per_chunk_calls", "test_pipeline_matches_oracle_chain",
+                        FE + "test_resample_matches_reference_golden",
+                        RS + "test_resample_short_inputs"],                      # n = 1 (NaN as SciPy), 2, 3, 27
     "rec_resample_kernel": ["test_frontend_chunks_bit_identical_to_per_chunk_calls",
-                            "test_pipeline_matches_oracle_chain"],
-    "rec_mix_kernel": ["test_frontend_chunks_bit_identical_to_per_chunk_calls"],
+                            "test_pipeline_matches_oracle_chain",
+                            FE + "test_resample_matches_reference_golden",
+                            RS + "test_resample_ratio_grid",                   # 42 ratios; complex64, complex128, float64
+                            RS + "test_resample_cta_boundaries",               # n_out = 255 .. 513 at 13/119 and 3/2
+                            RS + "test_resample_shared_memory_limit",          # 1/89 and 2/171 fit, 1/90 and 2/173 not
+                            RS + "test_frontend_mix_modes"],                   # int8 / int16 / float32 IQ, every mode
+    "rec_mix_kernel": ["test_frontend_chunks_bit_identical_to_per_chunk_calls",
+                       FE + "test_frequency_shift_follows_numpy_promotion",
+                       RS + "test_frequency_shift_and_frontend_past_2_24_samples",   # 2^25 + 12345 samples
+                       RS + "test_direct_xambg_shapes"],                       # one mix per Doppler bin, F = 1 .. 32
 }
+
+
+def _is_gpu_test(test_id):
+    path, _, name = test_id.rpartition("::")
+    src = open(os.path.join(ROOT, path) if path else os.path.abspath(__file__)).read()
+    i = src.index(f"\ndef {name}(")
+    decorators = src[src.rindex("\n\n", 0, i):i]
+    return "@pytest.mark.gpu" in decorators or re.search(r"^pytestmark = pytest\.mark\.gpu$", src, re.M) is not None
 
 
 def test_every_recording_launch_has_a_covering_gpu_test():
     src = open(RECORDING).read()
     sites = {m.group(1) + (m.group(2) or "") for m in re.finditer(r"([A-Za-z_]\w*)\s*(<[^<>;()]*>)?\s*<<<", src)}
     assert sites == set(COVERAGE), f"launch sites {sites} vs COVERAGE {set(COVERAGE)}"
-    this = open(os.path.abspath(__file__)).read()
     for tests in COVERAGE.values():
         for t in tests:
-            i = this.index(f"\ndef {t}(")
-            decorators = this[this.rindex("\n\n", 0, i):i]
-            assert "@pytest.mark.gpu" in decorators, f"{t} is not a GPU test"
+            assert _is_gpu_test(t), f"{t} is not a GPU test"
 
 
 # ------------------------------------------------------------------ GPU
@@ -205,6 +221,22 @@ def test_frontend_chunks_bit_identical_to_per_chunk_calls():
     for b in range(nchunks):
         want = prb.frontend(raw[off + 2 * b * n:off + 2 * (b + 1) * n], 100000, 2400000, np.array([po[b]]), 13, 119)
         np.testing.assert_array_equal(got[b].view(np.uint64), want.view(np.uint64))
+    # so do prc_iq_mix_c64 and prc_frontend_c64: a device pointer at an odd raw element gives the host call's bits
+    lib = _lib.load()
+    for dtype, kind in ((np.int8, _lib.IQ_I8), (np.int16, _lib.IQ_I16)):
+        iq = synth.raw_iq(n + 8, dtype.__name__, seed=4)
+        host, iq_d = np.ascontiguousarray(iq[off:off + 2 * n]), torch.from_numpy(iq).cuda()
+        mix, fe = np.empty(n, np.complex64), np.empty(n_out, np.complex64)
+        mix_d = torch.empty(n, dtype=torch.complex64, device="cuda")
+        fe_d = torch.empty(n_out, dtype=torch.complex64, device="cuda")
+        for src, m, f, mem in ((host.ctypes.data, mix.ctypes.data, fe.ctypes.data, _lib.MEM_HOST),
+                               (iq_d.data_ptr() + off * iq.itemsize, mix_d.data_ptr(), fe_d.data_ptr(), _lib.MEM_DEVICE)):
+            _lib.check(lib.prc_iq_mix_c64(src, kind, n, _lib.MIX_C128, 100000.0, 2400000.0, 0.3, m, mem, 0, None, 0))
+            _lib.check(lib.prc_frontend_c64(src, kind, n, _lib.MIX_C128, 100000.0, 2400000.0, 0.3, 13, 119, h.ctypes.data,
+                                            h.shape[0], f, n_out, mem, 0, None, 0))
+        torch.cuda.synchronize()
+        np.testing.assert_array_equal(mix_d.cpu().numpy().view(np.uint64), mix.view(np.uint64), err_msg=dtype.__name__)
+        np.testing.assert_array_equal(fe_d.cpu().numpy().view(np.uint64), fe.view(np.uint64), err_msg=dtype.__name__)
     # the resampler's shared-memory refusal and message are prc_frontend_c64's
     h = _resample_taps(17, 1245, False)
     o = np.empty(64, np.complex64)

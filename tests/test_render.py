@@ -17,6 +17,7 @@ from passiveradar_b200 import _lib, synth
 from passiveradar_b200.plotting_tools import RenderPipeline, persistence, persistence_frames
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+DETECT = os.path.join(ROOT, "passiveradar_b200", "csrc", "detect.cuh")
 RENDER = os.path.join(ROOT, "passiveradar_b200", "csrc", "render.cuh")
 GOLDEN = os.path.join(ROOT, "tests", "golden")
 ENTRIES = ("prc_cfar2d_frames", "prc_persistence_frames", "prc_percentiles_frames")
@@ -59,35 +60,49 @@ def test_abi_entries_are_declared():
     assert prb.persistence_frames is persistence_frames
 
 
-# every launch in render.cuh -> the GPU tests that reach it
+# every launch in detect.cuh and render.cuh -> the GPU tests that reach it (a test of this file, or
+# "tests/<file>::<test>")
+FE, RS = "tests/test_gpu_frontend.py::", "tests/test_rows_sweep.py::"
 COVERAGE = {
-    "cfar_frames_abssum_kernel": ["test_cfar_frames_bit_identical_to_per_frame_calls", "test_chain_matches_oracle"],
-    "cfar_frames_kernel": ["test_cfar_frames_bit_identical_to_per_frame_calls", "test_chain_matches_oracle"],
+    "cfar_frames_abssum_kernel": ["test_cfar_frames_bit_identical_to_per_frame_calls", "test_chain_matches_oracle",
+                                  FE + "test_cfar_matches_reference_golden",
+                                  RS + "test_cfar_map_contents_match_oracle"],       # real maps and |x| of complex maps
+    "cfar_frames_kernel": ["test_cfar_frames_bit_identical_to_per_frame_calls", "test_chain_matches_oracle",
+                           FE + "test_cfar_matches_reference_golden",
+                           RS + "test_cfar_fw_gw_grid_matches_oracle",      # fw = 1 .. 64, gw below, at and above fw
+                           RS + "test_cfar_map_sizes_match_oracle",         # 1 x 1 .. 2048 x 301, smaller than tile and fw
+                           RS + "test_cfar_map_contents_match_oracle",      # signed, float64, complex, zero plateaus
+                           RS + "test_cfar_row_limit"],                     # the tallest map, 524 280 rows
     "pst_kernel": ["test_persistence_matches_reference_goldens", "test_chain_matches_oracle"],
     "pct_kernel": ["test_percentiles_bit_identical_to_numpy", "test_chain_matches_oracle"],
 }
 
 
-def test_every_render_launch_has_a_covering_gpu_test():
-    src = open(RENDER).read()
+def _is_gpu_test(test_id):
+    path, _, name = test_id.rpartition("::")
+    src = open(os.path.join(ROOT, path) if path else os.path.abspath(__file__)).read()
+    i = src.index(f"\ndef {name}(")
+    decorators = src[src.rindex("\n\n", 0, i):i]
+    return "@pytest.mark.gpu" in decorators or re.search(r"^pytestmark = pytest\.mark\.gpu$", src, re.M) is not None
+
+
+def test_every_cfar_and_render_launch_has_a_covering_gpu_test():
+    src = open(DETECT).read() + open(RENDER).read()
     sites = {m.group(1) + (m.group(2) or "") for m in re.finditer(r"([A-Za-z_]\w*)\s*(<[^<>;()]*>)?\s*<<<", src)}
     assert sites == set(COVERAGE), f"launch sites {sites} vs COVERAGE {set(COVERAGE)}"
-    this = open(os.path.abspath(__file__)).read()
     for tests in COVERAGE.values():
         for t in tests:
-            i = this.index(f"\ndef {t}(")
-            decorators = this[this.rindex("\n\n", 0, i):i]
-            assert "@pytest.mark.gpu" in decorators, f"{t} is not a GPU test"
+            assert _is_gpu_test(t), f"{t} is not a GPU test"
 
 
-def test_render_kernels_build_for_sm90a_without_spills():
+def test_cfar_and_render_kernels_build_for_sm90a_without_spills():
     from passiveradar_b200 import build as b
     b.build(force=False)
     log = os.path.join(b.PKG, "libprcore.ptxas.log")
     if not os.path.exists(log):
         pytest.skip("the library was built elsewhere (no ptxas log in this tree)")
     blocks = [blk for blk in open(log).read().split("Compiling entry function")[1:]
-              if "3prc3rdr" in blk.split("\n")[0]]
+              if "3prc3rdr" in blk.split("\n")[0] or "cfar_frames" in blk.split("\n")[0]]
     assert len(blocks) == 4, "cfar abssum, cfar, persistence, percentile"
     for blk in blocks:
         assert "'sm_90a'" in blk.split("\n")[0]

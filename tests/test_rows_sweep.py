@@ -8,7 +8,7 @@ Criteria (SURVEY.md 8d): E = max|gpu - x| / max|x| <= 1e-5.  Where the reference
 GPU-vs-truth <= 1e-5 and GPU-vs-reference <= 1e-5 + 1.2 x (reference-vs-truth).  Figures go to
 $PRC_PARITY_DIR/parity.json (conftest.record_parity).
 
-The one CPU test states cfar2d_kernel's summation order in NumPy, with the accumulator type read from
+The one CPU test states cfar_frames_kernel's summation order in NumPy, with the accumulator type read from
 csrc/detect.cuh, and holds it to the float64 oracle on non-negative and signed maps."""
 import ctypes as C
 import math
@@ -77,9 +77,9 @@ def cfar_cells(gpu, want):
 
 # ------------------------------------------------------------------ CPU: the kernel's summation order
 def _acc_dtype():
-    """The accumulator cfar2d_kernel declares for its window sums."""
+    """The accumulator cfar_frames_kernel declares for its window sums."""
     src = open(DETECT).read()
-    kern = src[src.index("cfar2d_kernel("):src.index("piece_sum_kernel")]
+    kern = src[src.index("cfar_frames_kernel("):src.index("piece_sum_kernel")]
     acc = re.search(r"\b(float|double) acc = ", kern).group(1)
     racc = re.search(r"\b(float|double) racc = ", kern).group(1)
     assert acc == racc
@@ -87,7 +87,7 @@ def _acc_dtype():
 
 
 def cfar_model(X, fw, gw, acc):
-    """cfar2d_kernel in NumPy: X read as float32; for a = 0 .. fw-1 the row a of the window is summed over b = 0 .. fw-1
+    """cfar_frames_kernel in NumPy: X read as float32; for a = 0 .. fw-1 the row a of the window is summed over b = 0 .. fw-1
     (the guard hole skipped) into racc, and racc into acc, both of type ``acc``; the cell is X[(i + c - a) mod rows,
     (j + c - b) mod cols] with c = (fw - 1) // 2; CR = X * (1 / mean|X|) / (acc * scale + 1e-10) in ``acc``."""
     X = np.asarray(X, dtype=np.float32)
@@ -111,7 +111,7 @@ def cfar_model(X, fw, gw, acc):
     return ((X.astype(acc) * inv_mean) / (total * scale + acc(1e-10))).astype(np.float32)
 
 
-def test_cfar_summation_model_matches_float64_oracle():
+def test_cfar_frames_summation_model_matches_float64_oracle():
     acc = _acc_dtype()
     cases = [("rayleigh_256x301", rayleigh(256, 301, 1), 18, 4), ("rayleigh_256x301", rayleigh(256, 301, 1), 64, 10),
              ("ridge_256x301", clutter_ridge(256, 301, 2), 18, 4), ("ridge_256x301", clutter_ridge(256, 301, 2), 64, 3),
@@ -338,7 +338,7 @@ RS_SMEM_LIMIT = 200 * 1024          # SMEM_LIMIT of csrc/prcore.cu
 
 
 def _resample_smem(up, dn):
-    """Shared memory resample_device asks for (csrc/prcore.cu: resample_geo, resample_device), reduced ratio."""
+    """Shared memory the resampler asks for (csrc/prcore.cu: resample_geo, resample_table), reduced ratio."""
     g = math.gcd(up, dn)
     up, dn = up // g, dn // g
     half_len = 10 * max(up, dn)
