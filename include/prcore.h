@@ -428,6 +428,26 @@ int prc_channel_offset(const void* s1, int dtype1, int64_t n1, const void* s2, i
 int prc_xcorr(const void* s1, int dtype1, int64_t n1, const void* s2, int dtype2, int64_t n2, int64_t nlead, int64_t nlag,
               void* out, int mem_kind, int device, void* stream, unsigned flags);
 
+/* ---- Welch power spectral density -----------------------------------------------------------------
+ * prc_psd_frames computes matplotlib.mlab.psd (what plt.psd plots, signal_preview.py:52-72) of nframes frames of n
+ * samples, frame f at element f * frame_stride of x (dtype PRC_DT_F32, PRC_DT_F64, PRC_DT_C64 or PRC_DT_C128, widened
+ * on load).  Per frame: segments of nfft samples at a step of nfft - noverlap, (n - noverlap) / (nfft - noverlap) of
+ * them (a ragged tail is dropped; a frame shorter than nfft is zero-padded to one segment); each segment times
+ * window[0 .. nfft), zero-padded to pad_to points and transformed; |X|^2 summed over the segments, times scale, divided
+ * by the segment count.  onesided = 0: pad_to bins rotated so that bin 0 is -Fs/2 (mlab's freqcenter = pad_to / 2);
+ * onesided = 1: bins 0 .. pad_to/2, every bin but DC doubled, the pad_to/2 bin only when nfft is odd (mlab's rule).
+ * Frame f's bins go to out + f * out_stride.  All arithmetic is float64 / complex128.  A frame's result does not
+ * depend on nframes or on the device: a frame of a batch is bit-identical to the same frame computed alone.
+ *
+ * x, window and out are DEVICE pointers (the call has no mem_kind; callers stage host arrays themselves).
+ * Limits (PRC_E_INVALID): pad_to a power of two in [16, 8192]; 1 <= nfft <= pad_to; 0 <= noverlap < nfft; n >= 1;
+ * nframes >= 1; frame_stride >= n; out_stride >= the output bins; onesided 0 or 1; x, window, out not NULL.
+ * Scratch memory is allocated stream-ordered on the call's stream and released before the call returns it.
+ */
+int prc_psd_frames(const void* x, int dtype, int64_t n, int nframes, int64_t frame_stride, int nfft, int noverlap,
+                   int pad_to, const double* window, double scale, int onesided, double* out, int64_t out_stride,
+                   int device, void* stream, unsigned flags);
+
 #ifdef __cplusplus
 }
 #endif

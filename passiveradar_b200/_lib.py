@@ -113,6 +113,9 @@ SIGNATURES = {
                                      C.c_uint]),
     "prc_xcorr": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_int64,
                             C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_psd_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                 C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                 C.c_uint]),
 }
 
 

@@ -34,6 +34,7 @@
 #include "framepass.cuh"
 #include "recording.cuh"
 #include "render.cuh"
+#include "spectrum.cuh"
 
 namespace {
 
@@ -53,13 +54,13 @@ std::atomic<uint64_t> g_launches{0};
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
                 K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_CFAR_FRAMES, K_PERSISTENCE,
-                K_PERCENTILE, K_COUNT };
+                K_PERCENTILE, K_PSD_SEGMENTS, K_PSD_FINISH, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
                                            "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
                                            "caf_combine", "frontend_chunks", "cfar_frames",
-                                           "persistence", "percentile"};
+                                           "persistence", "percentile", "psd_segments", "psd_finish"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -251,6 +252,7 @@ int set_kernel_attrs(int device) {
     PRC_FFT_ATTRS(16)
 #undef PRC_FFT_ATTRS
     CU(fftc::framepass_set_attrs(lim));
+    CU(spec::set_attrs(lim));
     g_attrs_set[device].store(true);
     return PRC_OK;
 }
@@ -1877,6 +1879,60 @@ int ls_bins(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt,
     return PRC_OK;
 }
 
+// ---- Welch PSD (spectrum.cuh) -----------------------------------------------------------------------------------
+constexpr size_t PSD_PART_BUDGET = 256u << 20;     // partial spectra of one launch; larger batches run in groups
+
+// nframes frames -> their spectra: twiddles once, then per group of frames the segment transforms and the finishing
+// sums.  The groups only bound the scratch: a frame's chunks and its finishing sum do not depend on them.
+int psd_device(Ctx* c, const void* x, int dt, long long n, int nframes, long long stride, int nfft, int noverlap, int m,
+               const double* win, double scale, int onesided, double* out, long long out_stride) {
+    using namespace spec;
+    const long long P = 1ll << m, step = nfft - noverlap;
+    const long long nseg = n < nfft ? 1 : (n - noverlap) / step;      // mlab zero-pads a short frame to one segment
+    const long long per_cta = segments_per_cta(nseg);
+    const int nchunk = (int)((nseg + per_cta - 1) / per_cta);
+    const size_t frame_part = (size_t)nchunk * P * sizeof(double);
+    const size_t fit = std::max<size_t>(1, PSD_PART_BUDGET / frame_part);
+    const int group = (int)std::min<size_t>(std::min<size_t>((size_t)nframes, 65535), fit);
+    AsyncScratch ws(c->stream);
+    double2* tw;
+    double* part;
+    TRY(ws.get(&tw, (size_t)(P / 2) * sizeof(double2)));
+    TRY(ws.get(&part, frame_part * group));
+    SegParams sp{};
+    sp.x = x; sp.dt = dt; sp.n = n; sp.stride = stride;
+    sp.nfft = nfft; sp.m = m; sp.step = step; sp.nseg = nseg; sp.per_cta = per_cta; sp.nchunk = nchunk;
+    sp.win = win; sp.tw = tw; sp.part = part;
+    FinParams fp{};
+    fp.part = part; fp.m = m; fp.nchunk = nchunk;
+    fp.nbins = onesided ? P / 2 + 1 : P;
+    fp.onesided = onesided;
+    fp.nyq_double = nfft & 1;
+    fp.scale = scale;
+    fp.inv_nseg = 1.0 / (double)nseg;
+    fp.out = out; fp.out_stride = out_stride;
+    {
+        ProfScope ps(c, K_PSD_SEGMENTS);
+        launch_twiddle(tw, m, c->stream);
+    }
+    TRY(check_launch("spec_twiddle_kernel"));
+    for (int f0 = 0; f0 < nframes; f0 += group) {
+        const int nf = std::min(group, nframes - f0);
+        sp.f0 = fp.f0 = f0;
+        {
+            ProfScope ps(c, K_PSD_SEGMENTS);
+            launch_segments(sp, nf, c->stream);
+        }
+        TRY(check_launch("spec_segments_kernel"));
+        {
+            ProfScope ps(c, K_PSD_FINISH);
+            launch_finish(fp, nf, c->stream);
+        }
+        TRY(check_launch("spec_finish_kernel"));
+    }
+    return PRC_OK;
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2677,6 +2733,33 @@ int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int
     TRY(unstage(c, out, dout, mem_kind, nframes, nb, sb, flags));
     TRY(unstage(c, taps_out, dtaps, mem_kind, 1, mb, mb, flags));
     TRY(unstage(c, rank_out, drank, mem_kind, 1, rb, rb, flags));
+    return finish(c, flags);
+}
+
+int prc_psd_frames(const void* x, int dtype, int64_t n, int nframes, int64_t frame_stride, int nfft, int noverlap,
+                   int pad_to, const double* window, double scale, int onesided, double* out, int64_t out_stride,
+                   int device, void* stream, unsigned flags) {
+    if (!x || !window || !out) return fail(PRC_E_INVALID, "x/window/out must not be NULL");
+    if (!spec::dt_ok(dtype))
+        return fail(PRC_E_INVALID, "dtype=%d invalid: PRC_DT_F32, PRC_DT_F64, PRC_DT_C64 or PRC_DT_C128", dtype);
+    if (pad_to < (1 << spec::MIN_LOG2) || pad_to > (1 << spec::MAX_LOG2) || (pad_to & (pad_to - 1)))
+        return fail(PRC_E_INVALID, "pad_to=%d must be a power of two in [%d, %d]", pad_to, 1 << spec::MIN_LOG2,
+                    1 << spec::MAX_LOG2);
+    if (nfft < 1 || nfft > pad_to) return fail(PRC_E_INVALID, "nfft=%d outside [1, pad_to=%d]", nfft, pad_to);
+    if (noverlap < 0 || noverlap >= nfft) return fail(PRC_E_INVALID, "noverlap=%d outside [0, nfft=%d)", noverlap, nfft);
+    if (n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    if (nframes < 1) return fail(PRC_E_INVALID, "nframes=%d invalid", nframes);
+    if (frame_stride < n)
+        return fail(PRC_E_INVALID, "frame_stride=%lld smaller than n=%lld", (long long)frame_stride, (long long)n);
+    if (onesided != 0 && onesided != 1) return fail(PRC_E_INVALID, "onesided=%d must be 0 or 1", onesided);
+    const long long nbins = onesided ? pad_to / 2 + 1 : pad_to;
+    if (out_stride < nbins)
+        return fail(PRC_E_INVALID, "out_stride=%lld smaller than the %lld output bins", (long long)out_stride, nbins);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    TRY(psd_device(c, x, dtype, n, nframes, frame_stride, nfft, noverlap, ilog2(pad_to), window, scale, onesided, out,
+                   out_stride));
     return finish(c, flags);
 }
 

@@ -203,3 +203,13 @@ def recording_for(config, nchunks, channel_delay=0, clutter=True, seed=1):
     ref, srv = recording(n, config["input_sample_rate"], config["offset_freq"], up, dn, delay=3 * up, fd=fd,
                          channel_delay=channel_delay, clutter=clutter, seed=seed)
     return ref, srv, 3 * up, 40
+
+
+def interleave_channels(ref, srv):
+    """One raw source of two channels' interleaved IQ (``ref``, ``srv`` as ``recording`` returns them): complex
+    samples alternate between the channels, ``[ref_I[0], ref_Q[0], srv_I[0], srv_Q[0], ref_I[1], ...]``, the layout
+    PRconfig.yaml's ``interleaved_input_channels: True`` describes."""
+    out = np.empty(ref.shape[0] + srv.shape[0], dtype=ref.dtype)
+    out.reshape(-1, 4)[:, 0:2] = ref.reshape(-1, 2)
+    out.reshape(-1, 4)[:, 2:4] = srv.reshape(-1, 2)
+    return out
