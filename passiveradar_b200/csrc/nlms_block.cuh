@@ -131,6 +131,20 @@ __global__ void __launch_bounds__(NT, NT == 512 ? 3 : 1) nlms_block_kernel(const
             // ---- phase A2: Gram lags delta = warp, warp + NWARP, ...: g(m, m + delta), m = lane
             for (int delta = warp; delta < 32; delta += NWARP) {
                 const float2* t0 = tile + kk0;
+                if (M < NB_L) {
+                    // windows shorter than the block: the sliding increments below would telescope a window of a
+                    // few samples out of differences of other samples' products, and a small p_m (one or two
+                    // samples near zero) would be mostly their rounding.  Sum every window directly (< 32 MACs).
+                    float gr = 0.f, gi = 0.f;
+                    for (int q = 0; q < M; ++q) {
+                        const float2 a = t0[lane + q], b = t0[lane + q + delta];
+                        gr = fmaf(a.x, b.x, gr); gr = fmaf(a.y, b.y, gr);
+                        gi = fmaf(a.x, b.y, gi); gi = fmaf(-a.y, b.x, gi);
+                    }
+                    Gs[lane * (NB_L + 1) + delta] = make_float2(gr, gi);
+                    if (delta == 0) invp[lane] = p.mu / gr;
+                    continue;
+                }
                 float cr = 0.f, ci = 0.f;
                 for (int q = lane; q < M; q += 32) {                      // direct sum for m = 0
                     const float2 a = t0[q], b = t0[q + delta];

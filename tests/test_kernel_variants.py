@@ -492,10 +492,12 @@ PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/t
 FE, GAL, TRK = "tests/test_gpu_frontend.py::", "tests/test_gal_jpe.py::", "tests/test_tracking.py::"
 RS = "tests/test_rows_sweep.py::"
 PS = "tests/test_path_sweep.py::"
+DS = "tests/test_direct_sweep.py::"
 VARIANT_TEST = KV + "test_variant_matches_truth_and_reference"
 COVERAGE = {
     "launch_lagstream: lagstream_kernel<TILE_I, TILE_D>": [(PAR + "test_ls_matches_live_oracle", "direct", "LS, n <= 20000"),
-                                                           (VARIANT_TEST, "default", "ls_big, caf_big, frame: LS and CAF at config 2")],
+                                                           (VARIANT_TEST, "default", "ls_big, caf_big, frame: LS and CAF at config 2"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "default", "CAF: G = 1 at H = 512, G = 32, blocks over >= 3 CTAs, CTAs over >= 3 blocks"), (DS + "test_ls_direct_form_at_the_planner_edges", "default", "LS lag sums, M = 1 .. 2048")],
     "fft_twiddles: fft::fft_twiddle_kernel<R3>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 (n = 200000) and 8 (n = 10**6)"),
         (PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "R3 = 16")],
@@ -529,41 +531,59 @@ COVERAGE = {
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16 (R = 1200)"),
         (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
     "xambg_device: weight_kernel": [(VARIANT_TEST, "default", "caf_big, frame"),
-                                    (PAR + "test_xambg_matches_live_oracle", "direct", "lagstream CAF with a window")],
+                                    (PAR + "test_xambg_matches_live_oracle", "direct", "lagstream CAF with a window"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "default", "windowed lagstream cases")],
     "xambg_device: lagcorr_kernel<TILE_I, TILE_D>": [
         (VARIANT_TEST, "default", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
-        (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps")],
+        (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "default", "D = 1, ntaps 32 / 63, tap-weighted at G = 32, H = 512 and the nchunk loop")],
     "xambg_device: twiddle_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "every fast_xambg")],
     "xambg_device: doppler_fft_pow2_kernel<8>": [
         (KV + "test_caf_wave_grid_is_bit_identical", "default", "5 frames x 38 column groups >= SM count"),
-        (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "direct", "R = 1200, F = 64")],
+        (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "direct", "R = 1200, F = 64"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "default", "R = 1100, 3073, 5119")],
     "xambg_device: doppler_fft_pow2_kernel<2>": [(PAR + "test_xambg_matches_live_oracle", "direct", "F <= 4096"),
-                                                 (KV + "test_doppler_stage_at_large_F", "fft", "F = 4096")],
-    "xambg_device: doppler_fft_pow2_kernel<1>": [(KV + "test_doppler_stage_at_large_F", "fft", "F = 8192")],
+                                                 (KV + "test_doppler_stage_at_large_F", "fft", "F = 4096"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 2 .. 4096")],
+    "xambg_device: doppler_fft_pow2_kernel<1>": [(KV + "test_doppler_stage_at_large_F", "fft", "F = 8192"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 8192")],
     "xambg_device: chunk_sum_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
-                                       (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
+                                       (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 1, 100, 200, 1500, 16384")],
     "xambg_device: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
-                                         (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384")],
+                                         (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384"),
+        (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 1, 100, 200, 1500, 16384")],
     "ls_device: levinson_kernel<1>": [(VARIANT_TEST, "default", "ls_big, ls_small"),
-                                      (PAR + "test_ls_matches_live_oracle", "direct", "")],
+                                      (PAR + "test_ls_matches_live_oracle", "direct", ""),
+        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1 .. 1024")],
     "ls_device: levinson_kernel<4>": [(VARIANT_TEST, "default", "ls_wide"),
-                                      (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", "")],
+                                      (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", ""),
+        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1025, 2048")],
     "ls_device: fir_apply_kernel<TILE_I, TILE_D>": [(VARIANT_TEST, "default", "ls_small, ls_wide, toep"),
-                                                    (VARIANT_TEST, "default", "ls_big, frame at config 2")],
+                                                    (VARIANT_TEST, "default", "ls_big, frame at config 2"),
+        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "Mpad = 10 .. 2050, circular and linear")],
     "ls_toeplitz_device: shift_roll_kernel": [(VARIANT_TEST, "default", "toep"),
-                                              (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins")],
+                                              (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins"),
+        (DS + "test_toeplitz_direct_form_with_peek_past_half_the_frame", "default", "peek >= n / 2")],
     "direct_xambg_device: piece_sum_kernel": [
         (FE + "test_direct_xambg_matches_reference_golden", "default", ""),
         (RS + "test_direct_xambg_shapes", "default", "R >= n, F = 1, odd F, n = 2^18"),
         (RS + "test_direct_xambg_lag_limit", "default", "R + 1 = the lag limit")],
-    "nlms_device: nlms_block_kernel<1, 512>": [(FFT + "test_nlms_large_batch_uses_the_half_size_ctas_and_matches", "default", "M = 410")],
-    "nlms_device: nlms_block_kernel<2, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 1000")],
-    "nlms_device: nlms_block_kernel<4, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 2000")],
+    "nlms_device: nlms_block_kernel<1, 512>": [(FFT + "test_nlms_large_batch_uses_the_half_size_ctas_and_matches", "default", "M = 410"),
+        (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 512")],
+    "nlms_device: nlms_block_kernel<2, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 1000"),
+        (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 513")],
+    "nlms_device: nlms_block_kernel<4, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 2000"),
+        (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 1025, 2048")],
     "nlms_device: nlms_block_kernel<1>": [(PAR + "test_nlms_matches_reference_golden", "default", ""),
-                                          (VARIANT_TEST, "default", "nlms M = 410")],
-    "nlms_device: nlms_block_kernel<2>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 1110")],
+                                          (VARIANT_TEST, "default", "nlms M = 410"),
+        (DS + "test_nlms_at_the_tiling_edges", "default", "M = 1 .. 1024, every last-tile length")],
+    "nlms_device: nlms_block_kernel<2>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 1110"),
+        (DS + "test_nlms_at_the_tiling_edges", "default", "M = 1025, 2048")],
     "nlms_device: nlms_block_kernel<4>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 3010"),
-                                          (KV + "test_nlms_accepts_4096_taps_and_names_the_limit_above", "default", "M = 4096")],
+                                          (KV + "test_nlms_accepts_4096_taps_and_names_the_limit_above", "default", "M = 4096"),
+        (DS + "test_nlms_at_the_tiling_edges", "default", "M = 2049, 4096 with initial taps"),
+        (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 2049: more frames than SMs, 1024-thread CTAs")],
     "gal_device: gal_jpe_kernel<1, false>": [(GAL + "test_gal_edge_cases", "default", "D = 1")],
     "gal_device: gal_jpe_kernel<2, false>": [(GAL + "test_gal_edge_cases", "default", "D = 40")],
     "gal_device: gal_jpe_kernel<4, false>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 77")],
