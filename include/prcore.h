@@ -231,17 +231,14 @@ int prc_ls_svd_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int
  *   "fft"        1 (default): LS correlations, clutter FIR and CAF block sums as FFT-domain block correlations
  *                (csrc/fftcorr.cuh);  0: FP32 direct form (csrc/lagstream.cuh, kernels.cuh)
  *   "fft_min_n"  smallest channel length the FFT-domain path takes (default 8192)
- *   "caf_wave"   1: the FFT-domain CAF kernel runs one wave of CTAs, each walking several Doppler blocks (default 0)
  *   "frame_onepass"  1 (default): prc_frames_c64 / prc_frame_c64 on the FFT-domain path form the LS lag sums and the
  *                CAF's per-block spectra in one pass over the channels (csrc/framepass.cuh) where the plan allows it
  *                (L = 2048, filter_len >= 1, fewer transforms than two passes);  0: lscorr_fft_kernel, then the fused
  *                caf_fft_kernel.  Acceptance and results within float32 round-off are the same either way.
- * Read-only (prc_get_option only; prc_set_option returns PRC_E_INVALID): the environment switches of INTEGRATION.md
- * section 6, latched once per process, so a caller can check which kernel variants are in force:
- *   "tune_nchunk" (PRC_TUNE_NCHUNK, -1 = automatic), "tune_g" (PRC_TUNE_G, -1 = automatic);
- *   "fft_ctas_ls", "fft_ctas_fir", "fft_ctas_caf"  CTAs per SM of lscorr_fft_kernel, fir_fft_kernel and the fused
- *                 caf_fft_kernel at L = 2048 on the calling thread's current device, as the runtime's occupancy
- *                 calculator gives it for the launch configuration: the number their one-wave grids are sized from
+ * Read-only (prc_get_option only; prc_set_option returns PRC_E_INVALID):
+ *   "fft_ctas_ls", "fft_ctas_fir"  CTAs per SM of lscorr_fft_kernel and fir_fft_kernel at L = 2048 on the calling
+ *                 thread's current device, as the runtime's occupancy calculator gives it for the launch
+ *                 configuration: the number their one-wave grids are sized from
  *   "fft_ctas_frame"  the same for frame_pass_kernel (the one-pass frame; 2 on an H100)
  */
 int prc_set_option(const char* name, int value);

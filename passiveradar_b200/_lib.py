@@ -188,12 +188,11 @@ def check(status: int):
 
 
 def set_option(name: str, value: int):
-    """Run-time switch of the library (include/prcore.h: "fft", "fft_min_n", "caf_wave").
+    """Run-time switch of the library (include/prcore.h: "fft", "fft_min_n", "frame_onepass").
 
-    ``get_option`` also reads the environment switches the library latched when it started ("tune_nchunk",
-    "tune_g"), and "fft_ctas_ls", "fft_ctas_fir", "fft_ctas_caf": CTAs per SM of the
-    FFT-domain LS, FIR and fused CAF kernels at L = 2048 on the current device, which their one-wave grids are sized
-    from.  Those names are read-only: setting one raises PrcoreError."""
+    ``get_option`` also reads "fft_ctas_ls", "fft_ctas_fir" and "fft_ctas_frame": CTAs per SM of the FFT-domain LS
+    and FIR kernels at L = 2048 and of the one-pass frame kernel on the current device, which their one-wave grids are
+    sized from.  Those names are read-only: setting one raises PrcoreError."""
     check(load().prc_set_option(name.encode(), int(value)))
 
 

@@ -13,8 +13,8 @@
 //     the MAC loop: staging never leaves the math pipe idle;
 //   * the register accumulators hold one sub-chunk (<= steps*TI samples per thread); after each
 //     sub-chunk a thread folds them into its own slot of the reduction scratch with a compensated
-//     (Kahan) sum, so the FP32 error does not grow with the length of a piece (one CTA may walk a
-//     whole 2**20-sample channel: PRC_TUNE_NCHUNK=1); the cross-group reduction and the partial row
+//     (Kahan) sum, so the FP32 error does not grow with the length of a piece (a CTA's range can
+//     span a whole 2**20-sample channel); the cross-group reduction and the partial row
 //     are paid once per piece, not once per 1-2k samples.
 // x must already carry its weights (ref, or ref*window written by weight_kernel); the tap-weighted
 // decimator of fast_xambg(shortFilt=False) keeps using lagcorr_kernel.

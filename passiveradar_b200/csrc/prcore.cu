@@ -146,7 +146,7 @@ struct Ctx {
     DBuf fft_tw[3], wp_fir, wp_caf, fftP;     // FFT-domain path: twiddle tables (L = 1024 / 2048 / 4096), taps spectra, CAF block sums
     DBuf fpacc;                               // one-pass frame: AccP / AccQ spectra per Doppler block [nf][F][2][L]
     bool fft_tw_ready[3] = {false, false, false};
-    int fft_ctas[6][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
+    int fft_ctas[4][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
     std::vector<ProfRec> recs;
     void release() {
         cudaSetDevice(device);
@@ -176,10 +176,8 @@ std::map<std::pair<int, void*>, Ctx*> g_stream_ctx;   // (device, caller stream)
 std::vector<Ctx*> g_all_ctx;
 std::atomic<bool> g_attrs_set[64];
 std::atomic<uint64_t> g_epoch{1};                      // bumped by prc_shutdown
-int g_tune_nchunk = -1, g_tune_g = -1;
 std::atomic<int> g_fft{1};            // FFT-domain correlation / overlap-save kernels (fftcorr.cuh); PRC_FFT=0: FP32 direct form
 std::atomic<int> g_fft_min_n{8192};   // ... for channels of at least this many samples (PRC_FFT_MIN_N)
-std::atomic<int> g_caf_wave{0};       // 1: CAF kernel grid = one wave of CTAs walking several Doppler blocks instead of one CTA per block
 std::atomic<int> g_frame_onepass{1};  // FFT-domain frame: LS lag sums and CAF block spectra in one pass (framepass.cuh); 0: two passes
 std::once_flag g_env_once;
 
@@ -210,8 +208,6 @@ struct TlsCtx {
 thread_local TlsCtx g_tls;
 
 void read_env() {
-    if (const char* e = getenv("PRC_TUNE_NCHUNK")) g_tune_nchunk = atoi(e);
-    if (const char* e = getenv("PRC_TUNE_G")) g_tune_g = atoi(e);
     if (const char* e = getenv("PRC_FFT")) g_fft.store(atoi(e));
     if (const char* e = getenv("PRC_FFT_MIN_N")) g_fft_min_n.store(atoi(e));
 }
@@ -348,12 +344,10 @@ int choose_geo(int blk_len, long long outer, int nlag, int nsm, Geo* g) {
     g->HT = g->H * TD;
     if (g->H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
     int gmax = std::max(1, std::min(32, 256 / g->H));
-    if (g_tune_g > 0) gmax = std::max(1, std::min(g_tune_g, 512 / g->H));
     long long target = (long long)nsm * 8;
     long long nchunk = std::max<long long>(1, (target + outer - 1) / outer);
     const int min_chunk = TI * gmax * 2;
     nchunk = std::min<long long>(nchunk, std::max(1, blk_len / min_chunk));
-    if (g_tune_nchunk > 0) nchunk = std::min<long long>(g_tune_nchunk, blk_len);
     for (;;) {
         g->chunk_len = ceil_div(blk_len, nchunk);
         g->nchunk = ceil_div(blk_len, g->chunk_len);
@@ -382,10 +376,8 @@ int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo
     g->HT = g->H * TD;
     if (g->H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
     int G = std::max(1, std::min(32, 256 / g->H));
-    if (g_tune_g > 0) G = std::max(1, std::min(g_tune_g, 512 / g->H));
     g->total = (long long)nblk * blk_len;
     long long want = std::max(1, 2 * nsm / nprob);
-    if (g_tune_nchunk > 0) want = g_tune_nchunk;
     const long long min_per_cta = (long long)G * TI * 2;
     want = std::min<long long>(want, std::max<long long>(1, g->total / min_per_cta));
     g->per_cta = (g->total + want - 1) / want;
@@ -442,7 +434,7 @@ int fft_twiddles(Ctx* c, int r3, const float2** tw) {
 }
 
 // FFT-domain kernels whose grids are sized to one wave of CTAs for the whole batch
-enum FftKern { FK_LS = 0, FK_FIR = 1, FK_CAF = 2, FK_CAF_FUSED = 3, FK_FRAME = 4, FK_COMBINE = 5 };   // FRAME, COMBINE: R3 = 8 only
+enum FftKern { FK_LS = 0, FK_FIR = 1, FK_FRAME = 2, FK_COMBINE = 3 };   // FRAME, COMBINE: R3 = 8 only
 
 // CTAs of one instantiation an SM holds at once, at the block size and dynamic shared memory it is launched with:
 // registers (and the launch bounds that cap them) and shared memory decide it, so the grids follow the build rather
@@ -459,12 +451,6 @@ int fft_ctas_per_sm(Ctx* c, FftKern k, int r3) {
     } else if (k == FK_FIR) {
         PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::fir_fft_kernel<R3>, 16 * R3,
                                                                            fftc::fir_smem_float2<R3>() * sizeof(float2))));
-    } else if (k == FK_CAF) {
-        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, false>, 16 * R3,
-                                                                           fftc::caf_smem_float2<R3>() * sizeof(float2))));
-    } else if (k == FK_CAF_FUSED) {
-        PRC_R3_SWITCH(r3, (e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&v, fftc::caf_fft_kernel<R3, true>, 16 * R3,
-                                                                           fftc::caf_smem_float2<R3>() * sizeof(float2))));
     } else {
         v = k == FK_FRAME ? fftc::frame_pass_ctas_per_sm() : fftc::caf_combine_ctas_per_sm();
     }
@@ -613,15 +599,7 @@ int caf_fft(Ctx* c, const CafFftPlan& pl, const float2* ref, const float2* srv, 
     p.n = (int)n; p.R = R; p.F = F; p.M = M; p.peek = peek;
     p.D = D; p.c0 = c0; p.ntaps = (int)ntaps; p.Bmax = pl.Bmax;
     p.P = c->fftP.as<float2>(); p.HT = pl.HT; p.tw = tw;
-    // caf_wave: one wave of CTAs for the whole batch (R3 = 8: 3 resident per SM, shared memory bound): a CTA walks
-    // several Doppler blocks of its frame, so the twiddle tables are staged once per CTA and there is no partially
-    // filled last wave
-    int gx = F;
-    if (g_caf_wave.load()) {
-        const long long slots = (long long)fft_ctas_per_sm(c, wp ? FK_CAF_FUSED : FK_CAF, pl.r3) * c->nsm;
-        gx = (int)std::max<long long>(1, std::min<long long>(F, slots / bt.nf));
-    }
-    const dim3 grid(gx, bt.nf);
+    const dim3 grid(F, bt.nf);
     {
         ProfScope ps(c, K_LAGCORR_CAF);
         if (wp) { PRC_R3_SWITCH(pl.r3, (fftc::caf_fft_kernel<R3, true><<<grid, 16 * R3, fftc::caf_smem_float2<R3>() * sizeof(float2), c->stream>>>(p))); }
@@ -1589,21 +1567,11 @@ int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, 
     return check_launch("track_meas_kernel");
 }
 
-// switches latched from the environment once per process (read_env): readable by name (prc_get_option), never settable
-const int* env_switch(const std::string& k) {
-    static const std::pair<const char*, const int*> kSwitches[] = {
-        {"tune_nchunk", &g_tune_nchunk}, {"tune_g", &g_tune_g}};
-    for (const auto& s : kSwitches)
-        if (k == s.first) return s.second;
-    return nullptr;
-}
-
 // read-only names of the residency the one-wave grids are sized from (fft_ctas_per_sm, R3 = 8 -- the transform
 // length of up to 1024 LS taps and of the CAF at config 2): the FftKern they report, -1 for any other name
 int fft_ctas_option(const std::string& k) {
     if (k == "fft_ctas_ls") return FK_LS;
     if (k == "fft_ctas_fir") return FK_FIR;
-    if (k == "fft_ctas_caf") return FK_CAF_FUSED;
     if (k == "fft_ctas_frame") return FK_FRAME;
     return -1;
 }
@@ -2215,10 +2183,7 @@ int prc_set_option(const char* name, int value) {
     const std::string k(name);
     if (k == "fft") g_fft.store(value);
     else if (k == "fft_min_n") g_fft_min_n.store(value);
-    else if (k == "caf_wave") g_caf_wave.store(value);
     else if (k == "frame_onepass") g_frame_onepass.store(value);
-    else if (env_switch(k))
-        return fail(PRC_E_INVALID, "option '%s' is read-only (set from the environment when the library starts)", name);
     else if (fft_ctas_option(k) >= 0)
         return fail(PRC_E_INVALID, "option '%s' is read-only (CTAs per SM of the build's kernels on this device)", name);
     else return fail(PRC_E_INVALID, "unknown option '%s'", name);
@@ -2231,9 +2196,7 @@ int prc_get_option(const char* name, int* value) {
     const std::string k(name);
     if (k == "fft") *value = g_fft.load();
     else if (k == "fft_min_n") *value = g_fft_min_n.load();
-    else if (k == "caf_wave") *value = g_caf_wave.load();
     else if (k == "frame_onepass") *value = g_frame_onepass.load();
-    else if (const int* s = env_switch(k)) *value = *s;
     else if (fft_ctas_option(k) >= 0) {
         int dev = 0;
         CU(cudaGetDevice(&dev));

@@ -553,8 +553,6 @@ def _set_path(fft_min_n):
 
 def _nsm():
     import torch
-    if _lib.get_option("tune_g") > 0 or _lib.get_option("tune_nchunk") > 0:
-        pytest.skip("PRC_TUNE_G / PRC_TUNE_NCHUNK change the tiling the twin mirrors")
     return torch.cuda.get_device_properties(0).multi_processor_count
 
 

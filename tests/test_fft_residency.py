@@ -1,10 +1,10 @@
 """Residency of the FFT-domain correlation kernels (csrc/fftcorr.cuh) and the grids sized from it.
 
-lscorr_fft_kernel, fir_fft_kernel and (with caf_wave = 1) caf_fft_kernel launch one wave of CTAs for the whole batch,
-so their grids are only as good as the number of CTAs an SM really holds.  On the CPU that number is worked out from
-the build's ptxas log and the shared-memory layout of fftcorr.cuh against the H100's limits; on the GPU the library
-reports what it sized its grids from (prc_get_option "fft_ctas_*"), and the fused frame path is checked at Doppler
-block counts that leave a partial last group of blocks.
+lscorr_fft_kernel and fir_fft_kernel launch one wave of CTAs for the whole batch, so their grids are only as good as
+the number of CTAs an SM really holds.  On the CPU that number is worked out from the build's ptxas log and the
+shared-memory layout of fftcorr.cuh against the H100's limits, and caf_fft_kernel's (one CTA per Doppler block) is
+held to three per SM; on the GPU the library reports what it sized its grids from (prc_get_option "fft_ctas_*"), and
+the fused frame path is checked at Doppler block counts that leave a partial last group of blocks.
 """
 import os
 import re
@@ -62,8 +62,8 @@ def fftc_entries():
     return out
 
 
-def expected_ctas(entries, kernel, r3, fused=None):
-    regs, _ = entries[(kernel, r3, fused)]
+def expected_ctas(entries, kernel, r3):
+    regs, _ = entries[(kernel, r3, None)]
     return ctas_per_sm(regs, 16 * r3, smem_bytes(kernel, r3))
 
 
@@ -96,8 +96,7 @@ def test_residency_model_matches_the_known_h100_limits():
 
 
 # ------------------------------------------------------------------ GPU
-OPTIONS = {"fft_ctas_ls": ("lscorr_fft_kernel", None), "fft_ctas_fir": ("fir_fft_kernel", None),
-           "fft_ctas_caf": ("caf_fft_kernel", True)}
+OPTIONS = {"fft_ctas_ls": "lscorr_fft_kernel", "fft_ctas_fir": "fir_fft_kernel"}
 
 
 @pytest.mark.gpu
@@ -105,9 +104,9 @@ def test_residency_options_report_what_the_build_fits():
     from passiveradar_b200 import build as b
     have_log = os.path.exists(os.path.join(b.PKG, "libprcore.ptxas.log"))
     entries = fftc_entries() if have_log else None
-    for name, (kernel, fused) in OPTIONS.items():
+    for name, kernel in OPTIONS.items():
         got = _lib.get_option(name)
-        want = expected_ctas(entries, kernel, 8, fused) if entries else 3
+        want = expected_ctas(entries, kernel, 8) if entries else 3
         assert got == want, (name, got, want)
         with pytest.raises(_lib.PrcoreError):
             _lib.set_option(name, got)
@@ -128,28 +127,21 @@ def _fused_maps(n, F, R, fl, frames, batch):
 ])
 def test_fused_frames_at_small_and_odd_doppler_counts(n, F, R, fl, nf):
     """prc_frames_c64 on the FFT path (clutter filter fused into caf_fft_kernel) against the float64 LS filter
-    followed by the CAF oracle, with caf_wave 0 and 1 (one CTA per Doppler block, or one wave of CTAs walking them):
-    the two grids compute every block the same way and must agree bit for bit."""
+    followed by the CAF oracle, one frame per call and the whole batch in one call."""
     from oracle import clutter_oracle as co
     from oracle import xambg_oracle as xo
     frames = [synth.make_frame(n, "P0", frame=250 + i) for i in range(nf)]
-    old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"), _lib.get_option("caf_wave"))
-    res = {}
+    old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"))
     try:
         _lib.set_option("fft", 1)
         _lib.set_option("fft_min_n", 8192)
-        for wave in (0, 1):
-            _lib.set_option("caf_wave", wave)
-            res[wave] = [_fused_maps(n, F, R, fl, frames, batch) for batch in sorted({1, nf})]
+        res = [_fused_maps(n, F, R, fl, frames, batch) for batch in sorted({1, nf})]
     finally:
         _lib.set_option("fft", old[0])
         _lib.set_option("fft_min_n", old[1])
-        _lib.set_option("caf_wave", old[2])
-    for a, b in zip(res[0], res[1]):
-        assert np.array_equal(a, b)
     w = signal.get_window(("kaiser", 5.0), n)
     worst = 0.0
-    for maps in res[1]:
+    for maps in res:
         assert maps.shape[0] == nf
         for i, (ref, srv) in enumerate(frames):
             t_clean, _ = co.ls_filter_truth(ref, srv, fl, 1.0, 10)

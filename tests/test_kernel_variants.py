@@ -2,61 +2,166 @@
 
 Three parts:
 
-* Variant matrix (GPU).  The environment switches of INTEGRATION.md section 6 are latched once per process, so every
-  variant runs in a child process (tests/_variant_child.py) that saves its outputs; this process computes each oracle
-  once and makes every comparison.  A variant's outputs are held to the float64 truth (1e-5) and to the
-  reference-pinned oracle or golden (1e-5 + 1.2 x reference-vs-truth), as in tests/test_gpu_parity.py.  They are also
-  compared with the default child: the switches change the arithmetic and are held to 3e-6 on independent channels
-  (P0), the bound tests/test_gpu_fft.py uses between arithmetics.
-* In-process GPU cases for dispatches of the default configuration no other test reaches: NLMS with more than 1024
-  taps, the Doppler stage at F = 4096 .. 16384, the tap-weighted decimator at full size, and caf_wave = 1.
+* Direct-form cases (GPU).  LS, Toeplitz, CAF and whole-frame inputs at config 2 and below run on the FP32 direct form
+  ("fft" set to 0 for the test), and NLMS at 410 .. 3010 taps on its one path.  Outputs are held to the float64 truth
+  (1e-5) and to the reference-pinned oracle or golden (1e-5 + 1.2 x reference-vs-truth), as in
+  tests/test_gpu_parity.py.  Each oracle is computed once per module.
+* GPU cases for dispatches of the default configuration no other test reaches: NLMS with more than 1024 taps, the
+  Doppler stage at F = 4096 .. 16384, the tap-weighted decimator at full size, and 5-frame CAF batches.
 * A CPU guard: every kernel launch site of prcore.cu must appear in COVERAGE with the GPU tests that reach it.
 
-Per-variant figures go to $PRC_PARITY_DIR/parity.json (tests/conftest.py:record_parity).
+Per-case figures go to $PRC_PARITY_DIR/parity.json (tests/conftest.py:record_parity).
 """
-import json
 import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import scipy.signal as signal
 
 import _golden as G
-import _variant_child as VC
 from conftest import record_parity
 from passiveradar_b200 import _lib, synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-CHILD = os.path.join(HERE, "_variant_child.py")
 PRCORE = os.path.join(ROOT, "passiveradar_b200", "csrc", "prcore.cu")
 TOL = 1e-5
-XVAR = 3e-6           # between two arithmetics on independent channels (test_random_shapes_fft_path_matches_direct_path_and_oracle)
 
 DIRECT = ["ls_big", "ls_small", "ls_wide", "toep", "caf_big", "caf_small", "frame"]
-# variant -> (environment, cases it runs).  The switches only change the direct form.
-VARIANTS = {
-    "default": ({}, DIRECT + ["nlms"]),
-    "tune": ({"PRC_TUNE_NCHUNK": "1", "PRC_TUNE_G": "1"}, DIRECT),  # one chunk / group per problem
+
+
+# ------------------------------------------------------------------ case inputs
+# Output keys are "<case>.<item>.<profile>.<field>"; the profile is the channel model (P0: independent channels, P1:
+# strong clutter).
+KAISER = ("kaiser", 5.0)
+
+
+def ls_items(case):
+    """LS_Filter inputs: (item, profile, golden name or None, ref, srv, filter_len, reg, peek)."""
+    if case == "ls_big":          # n = 2**20, 310 taps: lagstream_kernel, levinson_kernel<1>, fir_apply_kernel
+        for name in ("ls_c2_p1", "frame_c2_p0"):
+            g = G.load(name)
+            ref, srv = G.inputs(g)
+            yield name, str(g["profile"]), name, ref, srv, 300, 1.0, 10
+    elif case == "ls_small":      # lagstream_kernel, fir_apply_kernel, levinson_kernel<1>
+        ref, srv = synth.make_frame(5000, "P0", frame=9)
+        yield "n5000", "P0", None, ref, srv, 20, 1.0, 10
+        for name in ("ls_small", "ls_small_peek0", "ls_small_reg0"):
+            g = G.load(name)
+            ref, srv = G.inputs(g)
+            yield name, str(g["profile"]), name, ref, srv, int(g["filter_len"]), float(g["reg"]), int(g["peek"])
+    elif case == "ls_wide":       # 1110 taps: levinson_kernel<4>
+        for profile in ("P1", "P0"):
+            ref, srv = synth.make_frame(2 ** 18, profile, frame=2)
+            yield f"n262144_{profile}", profile, None, ref, srv, 1100, 1.0, 10
+
+
+def toep_items():
+    for name in ("toep_small", "toep_mid"):
+        g = G.load(name)
+        ref, srv = G.inputs(g)
+        yield name, str(g["profile"]), g, ref, srv
+
+
+def caf_items(case):
+    """fast_xambg inputs: (item, profile, golden or None, ref, srv, R, F, input_len, window, short_filt)."""
+    if case == "caf_big":         # D = 4096: weight_kernel, lagstream_kernel (CAF)
+        n = 2 ** 20
+        ref, srv = synth.make_frame(n, "P0", frame=21)
+        yield "n1048576", "P0", None, ref, srv, 300, 256, n, signal.get_window(KAISER, n), True
+    elif case == "caf_small":     # Doppler blocks of < 64 taps and the tap-weighted decimator: lagcorr_kernel
+        ref, srv = synth.make_frame(1000, "P0", frame=3)
+        yield "n1000", "P0", None, ref, srv, 9, 16, None, None, True
+        g = G.load("xambg_longfilt")
+        ref, srv = G.inputs(g)
+        R, F, input_len, window, short = G.xambg_args(g)
+        yield "xambg_longfilt", str(g["profile"]), g, ref, srv, R, F, input_len, window, short
+
+
+FRAME = dict(name="frame_c2_p0", filter_len=300, reg=1.0, peek=10)
+
+
+def frame_inputs():
+    g = G.load(FRAME["name"])
+    ref, srv = G.inputs(g)
+    return g, ref, srv, int(g["n"]), int(g["R"]), int(g["F"])
+
+
+NLMS = dict(n=2 ** 15, profile="P1", frame=4, mu=0.05, peek=10)
+NLMS_FILTER_LENS = (400, 1100, 3000)       # M = 410, 1110, 3010: nlms_block_kernel<1>, <2>, <4>
+NLMS_BLOCK = dict(filter_len=1100, block_len=64)
+
+
+def nlms_inputs():
+    return synth.make_frame(NLMS["n"], NLMS["profile"], frame=NLMS["frame"])
+
+
+# ------------------------------------------------------------------ runners: each fills `res` with its case's outputs
+def run_ls(case, res):
+    import passiveradar_b200 as prb
+    for item, profile, _, ref, srv, fl, reg, peek in ls_items(case):
+        out, taps = prb.LS_Filter(ref, srv, fl, reg, peek, True)
+        res[f"{case}.{item}.{profile}.out"] = out
+        res[f"{case}.{item}.{profile}.taps"] = taps
+
+
+def run_toep(res):
+    import passiveradar_b200 as prb
+    for item, profile, g, ref, srv in toep_items():
+        out, taps = prb.LS_Filter_Toeplitz(ref, srv, int(g["filter_len"]), int(g["peek"]), True)
+        res[f"toep.{item}.{profile}.out"] = out
+        res[f"toep.{item}.{profile}.taps"] = taps
+
+
+def run_caf(case, res):
+    import passiveradar_b200 as prb
+    for item, profile, _, ref, srv, R, F, input_len, window, short in caf_items(case):
+        res[f"{case}.{item}.{profile}.map"] = prb.fast_xambg(ref, srv, R, F, input_len, window, short)
+
+
+def run_frame(res):
+    """One frame through prc_frame_c64 (the entry point of FramePipeline) on the direct form: the LS stage's kernels, then
+    the CAF of the cleaned channel against the reference weighted by weight_kernel."""
+    g, ref, srv, n, R, F = frame_inputs()
+    M = FRAME["filter_len"] + FRAME["peek"]
+    w = np.ascontiguousarray(signal.get_window(KAISER, n), dtype=np.float64)
+    maps = np.empty((F, R + 1), np.complex64)
+    taps = np.empty(M, np.complex64)
+    clean = np.empty(n, np.complex64)
+    lib = _lib.load()
+    _lib.check(lib.prc_frame_c64(ref.ctypes.data, srv.ctypes.data, n, FRAME["filter_len"], FRAME["peek"], FRAME["reg"], R, F,
+                                 w.ctypes.data, maps.ctypes.data, taps.ctypes.data, clean.ctypes.data, _lib.MEM_HOST,
+                                 _lib.current_device(), None, 0))
+    prof = str(g["profile"])
+    res[f"frame.{FRAME['name']}.{prof}.map"] = maps[:, :, None]
+    res[f"frame.{FRAME['name']}.{prof}.taps"] = taps
+    res[f"frame.{FRAME['name']}.{prof}.out"] = clean
+
+
+def run_nlms(res):
+    import passiveradar_b200 as prb
+    ref, srv = nlms_inputs()
+    p = NLMS["profile"]
+    for fl in NLMS_FILTER_LENS:
+        out, taps = prb.NLMS_filter(ref, srv, fl, NLMS["mu"], NLMS["peek"], None, True)
+        res[f"nlms.M{fl + NLMS['peek']}.{p}.out"] = out
+        res[f"nlms.M{fl + NLMS['peek']}.{p}.taps"] = taps
+    fl, B = NLMS_BLOCK["filter_len"], NLMS_BLOCK["block_len"]
+    out, taps = prb.block_NLMS(ref, srv, fl, NLMS["mu"], NLMS["peek"], B, None, True)
+    res[f"nlms.M{fl + NLMS['peek']}_B{B}.{p}.out"] = out
+    res[f"nlms.M{fl + NLMS['peek']}_B{B}.{p}.taps"] = taps
+
+
+RUNNERS = {
+    "ls_big": lambda res: run_ls("ls_big", res),
+    "ls_small": lambda res: run_ls("ls_small", res),
+    "ls_wide": lambda res: run_ls("ls_wide", res),
+    "toep": run_toep,
+    "caf_big": lambda res: run_caf("caf_big", res),
+    "caf_small": lambda res: run_caf("caf_small", res),
+    "frame": run_frame,
 }
-_ENV_NAMES = {var for var, _ in VC.SWITCHES.values()} | {"PRC_FFT", "PRC_FFT_MIN_N"}
-
-
-def _child_env(extra):
-    env = {k: v for k, v in os.environ.items() if k not in _ENV_NAMES}
-    env.update(extra)
-    env["PYTHONPATH"] = os.pathsep.join([HERE, ROOT] + ([os.environ["PYTHONPATH"]] if os.environ.get("PYTHONPATH") else []))
-    return env
-
-
-def _run_child(args, extra, timeout):
-    res = subprocess.run([sys.executable, CHILD] + args, env=_child_env(extra), capture_output=True, text=True,
-                         timeout=timeout)
-    assert res.returncode == 0, f"child {args} with {extra} failed:\n{res.stdout[-4000:]}\n{res.stderr[-4000:]}"
-    return res.stdout
 
 
 def _rel_columns(got, want_cols, lags, R, peak):
@@ -82,7 +187,7 @@ class Oracles:
         def make():
             from oracle import clutter_oracle as co
             d = {}
-            for item, profile, golden, ref, srv, fl, reg, peek in VC.ls_items(case):
+            for item, profile, golden, ref, srv, fl, reg, peek in ls_items(case):
                 t_out, t_taps = co.ls_filter_truth(ref, srv, fl, reg, peek)
                 den = float(np.abs(srv).max())
                 e = dict(truth=(t_out, t_taps), den=den, profile=profile, oracle=None)
@@ -103,7 +208,7 @@ class Oracles:
         def make():
             from oracle import clutter_oracle as co
             d = {}
-            for item, profile, g, ref, srv in VC.toep_items():
+            for item, profile, g, ref, srv in toep_items():
                 t_out, t_taps = co.ls_filter_toeplitz_oracle(ref, srv, int(g["filter_len"]), int(g["peek"]), True)
                 d[item] = dict(truth=(t_out, t_taps), golden=g, den=float(g["srv_absmax"]))
             return d
@@ -114,7 +219,7 @@ class Oracles:
         def make():
             from oracle import xambg_oracle as xo
             d = {}
-            for item, profile, golden, ref, srv, R, F, input_len, window, short in VC.caf_items(case):
+            for item, profile, golden, ref, srv, R, F, input_len, window, short in caf_items(case):
                 if case == "caf_big":
                     n = ref.shape[0]
                     lags = sorted({0, 1, R // 3, R // 2, R - 1, R})
@@ -132,22 +237,22 @@ class Oracles:
         def make():
             from oracle import clutter_oracle as co
             from oracle import xambg_oracle as xo
-            g, ref, srv, n, R, F = VC.frame_inputs()
-            t_clean, t_taps = co.ls_filter_truth(ref, srv, VC.FRAME["filter_len"], VC.FRAME["reg"], VC.FRAME["peek"])
-            t_map = xo.fast_xambg_truth(ref, t_clean, R, F, n, signal.get_window(VC.KAISER, n))
+            g, ref, srv, n, R, F = frame_inputs()
+            t_clean, t_taps = co.ls_filter_truth(ref, srv, FRAME["filter_len"], FRAME["reg"], FRAME["peek"])
+            t_map = xo.fast_xambg_truth(ref, t_clean, R, F, n, signal.get_window(KAISER, n))
             return dict(golden=g, t_clean=t_clean, t_taps=t_taps, t_map=t_map, den=float(np.abs(srv).max()))
         return self.get("frame", make)
 
     def nlms(self):
-        """key (as the child names it) -> (oracle out, oracle taps, truth out, truth taps) of the C oracle."""
+        """key (as run_nlms names it) ->(oracle out, oracle taps, truth out, truth taps) of the C oracle."""
         def make():
             from oracle import clutter_oracle as co
-            ref, srv = VC.nlms_inputs()
-            mu, peek = VC.NLMS["mu"], VC.NLMS["peek"]
+            ref, srv = nlms_inputs()
+            mu, peek = NLMS["mu"], NLMS["peek"]
             d = {}
-            for fl in VC.NLMS_FILTER_LENS:
+            for fl in NLMS_FILTER_LENS:
                 d[f"M{fl + peek}"] = co.block_nlms_oracle_c(ref, srv, fl, mu, peek, 1) + co.block_nlms_truth_c(ref, srv, fl, mu, peek, 1)
-            fl, B = VC.NLMS_BLOCK["filter_len"], VC.NLMS_BLOCK["block_len"]
+            fl, B = NLMS_BLOCK["filter_len"], NLMS_BLOCK["block_len"]
             d[f"M{fl + peek}_B{B}"] = co.block_nlms_oracle_c(ref, srv, fl, mu, peek, B) + co.block_nlms_truth_c(ref, srv, fl, mu, peek, B)
             return d
         return self.get("nlms", make)
@@ -158,20 +263,13 @@ def oracles():
     return Oracles()
 
 
-@pytest.fixture(scope="module")
-def variant_outputs(tmp_path_factory):
-    """variant -> its child's outputs; each child runs once per module, the first time a test asks for it."""
-    cache = {}
-
-    def get(name):
-        if name not in cache:
-            env, cases = VARIANTS[name]
-            path = tmp_path_factory.mktemp(f"variant_{name}") / "outputs.npz"
-            _run_child([str(path)] + cases, env, timeout=1200)
-            with np.load(path) as z:
-                cache[name] = {k: z[k] for k in z.files}
-        return cache[name]
-    return get
+@pytest.fixture
+def direct_form():
+    """Run a test on the FP32 direct-form kernels ("fft" = 0) and restore the library's "fft" option afterwards."""
+    old = _lib.get_option("fft")
+    _lib.set_option("fft", 0)
+    yield
+    _lib.set_option("fft", old)
 
 
 # ------------------------------------------------------------------ per-case checks against truth and oracle
@@ -228,7 +326,7 @@ def _check_caf(case, res, orc, fig):
 def _check_frame(res, orc, fig):
     e = orc.frame()
     g = e["golden"]
-    p = f"frame.{VC.FRAME['name']}.{g['profile']}"
+    p = f"frame.{FRAME['name']}.{g['profile']}"
     fig["map_vs_truth"] = em = G.rel_inf(res[p + ".map"], e["t_map"])
     fig["taps_vs_truth"] = et = G.rel_inf(res[p + ".taps"], e["t_taps"])
     fig["out_vs_truth"] = eo = G.rel_inf(res[p + ".out"], e["t_clean"], den=e["den"])
@@ -251,13 +349,13 @@ def _nlms_bounds(out, taps, want, ww, truth, tw, what):
 
 
 def _check_nlms(res, orc, fig):
-    prof = VC.NLMS["profile"]
+    prof = NLMS["profile"]
     for key, (want, ww, truth, tw) in orc.nlms().items():
         out, taps = res[f"nlms.{key}.{prof}.out"], res[f"nlms.{key}.{prof}.taps"]
         for k, v in _nlms_bounds(out, taps, want, ww, truth, tw, key).items():
             fig[f"{key}/{k}"] = v
-        fl = int(key[1:].split("_")[0]) - VC.NLMS["peek"]
-        assert not out[:fl].any() and not out[-VC.NLMS["peek"]:].any(), key
+        fl = int(key[1:].split("_")[0]) - NLMS["peek"]
+        assert not out[:fl].any() and not out[-NLMS["peek"]:].any(), key
 
 
 def _check(case, res, orc, fig):
@@ -274,59 +372,29 @@ def _check(case, res, orc, fig):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", list(VARIANTS))
-def test_variant_matches_truth_and_reference(variant, variant_outputs, oracles):
-    env, cases = VARIANTS[variant]
-    res = variant_outputs(variant)
-    assert list(res["cases"]) == cases
-    echo = dict(zip(VC.SWITCHES, res["switches"].tolist()))
-    assert echo == VC.expected_switches(env), echo
-    for case in cases:
-        fig = {}
-        _check(case, res, oracles, fig)
-        record_parity(f"variants/{variant}/{case}", **fig)
+@pytest.mark.parametrize("case", DIRECT)
+def test_direct_form_matches_truth_and_reference(case, direct_form, oracles):
+    res, fig = {}, {}
+    RUNNERS[case](res)
+    _check(case, res, oracles, fig)
+    record_parity(f"variants/default/{case}", **fig)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", [v for v in VARIANTS if v != "default"])
-def test_variant_matches_default_child(variant, variant_outputs):
-    res, base = variant_outputs(variant), variant_outputs("default")
-    keys = [k for k in res if k.count(".") == 3]
-    assert keys and all(k in base for k in keys)
-    worst = 0.0
-    for k in keys:
-        if k.split(".")[2] != "P0":
-            continue                     # strong clutter: what is left after ~55 dB of cancellation, held to the truth only
-        e = G.rel_inf(res[k], base[k])
-        worst = max(worst, e)
-        assert e <= XVAR, (k, e)
-    record_parity(f"variants/{variant}/vs_default", E=worst)
-
-
-# ------------------------------------------------------------------ switch echo (no GPU needed)
-def test_switch_echo_reports_the_environment():
-    env = {"PRC_TUNE_G": "2", "PRC_TUNE_NCHUNK": "3"}
-    got = json.loads(_run_child(["--switches"], env, timeout=300))
-    assert (got["tune_g"], got["tune_nchunk"]) == (2, 3)
-    assert got == VC.expected_switches(env)
-    defaults = json.loads(_run_child(["--switches"], {}, timeout=300))
-    assert defaults == {"tune_nchunk": -1, "tune_g": -1}
-
-
-@pytest.mark.parametrize("name", list(VC.SWITCHES))
-def test_environment_switches_are_read_only(name):
-    lib = _lib.load()
-    assert lib.prc_set_option(name.encode(), 1) == _lib.PRC_E_INVALID
-    assert b"read-only" in lib.prc_last_error()
-    assert _lib.get_option(name) == VC.expected_switches(os.environ)[name]
+def test_nlms_matches_truth_and_reference(oracles):
+    res, fig = {}, {}
+    run_nlms(res)
+    _check("nlms", res, oracles, fig)
+    record_parity("variants/default/nlms", **fig)
 
 
 @pytest.mark.parametrize("name", ["stream", "packed", "tile", "nlms_block", "tma", "tma_l2", "tc", "tc_caf", "tc_fir",
-                                  "tma_active"])
+                                  "tune_nchunk", "tune_g", "tma_active", "caf_wave", "fft_ctas_caf"])
 def test_retired_switches_are_unknown_options(name):
-    """The environment switches INTEGRATION.md section 6 lists as no longer read, and "tma_active", which reported the
-    loader the "tma" switch selected: their option names are unknown, not read-only, so a library that still kept one
-    of them fails here."""
+    """The switches INTEGRATION.md section 6 lists as no longer read ("tune_nchunk" and "tune_g" reported PRC_TUNE_NCHUNK
+    and PRC_TUNE_G) and the options it lists as removed ("tma_active" reported the loader the "tma" switch selected,
+    "fft_ctas_caf" the residency the "caf_wave" grid was sized from): their option names are unknown, not read-only,
+    so a library that still kept one of them fails here."""
     lib = _lib.load()
     with pytest.raises(_lib.PrcoreError):
         _lib.get_option(name)
@@ -341,8 +409,8 @@ def test_retired_switches_are_unknown_options(name):
 def test_nlms_with_more_than_1024_taps_matches_c_oracle(fl, oracles):
     """M = 1110 and 3010: nlms_block_kernel<2> and <4> (two and four taps per thread)."""
     import passiveradar_b200 as prb
-    ref, srv = VC.nlms_inputs()
-    mu, peek = VC.NLMS["mu"], VC.NLMS["peek"]
+    ref, srv = nlms_inputs()
+    mu, peek = NLMS["mu"], NLMS["peek"]
     got, gw = prb.NLMS_filter(ref, srv, fl, mu, peek, None, True)
     fig = _nlms_bounds(got, gw, *oracles.nlms()[f"M{fl + peek}"], fl)
     record_parity(f"nlms/n32768_M{fl + peek}", **fig)
@@ -406,7 +474,7 @@ def test_doppler_stage_at_large_F(n, F, both_paths, oracles):
     from oracle import xambg_oracle as xo
     R = 40
     ref, srv = synth.make_frame(n, "P1", frame=25)
-    w = signal.get_window(VC.KAISER, n)
+    w = signal.get_window(KAISER, n)
     lags = [0, 1, R // 2, R - 1, R]
     cols = oracles.get(("doppler", n, F), lambda: {d: xo.fast_xambg_oracle(ref, np.roll(srv, -d), 0, F, n, w)[:, 0, 0] for d in lags})
     got = prb.fast_xambg(ref, srv, R, F, n, w)
@@ -439,46 +507,33 @@ def test_tap_weighted_decimator_at_full_size(both_paths, oracles):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("n,F,R", [(2 ** 20, 256, 300), (2 ** 18, 1024, 100)])
-def test_caf_wave_grid_is_bit_identical(n, F, R):
-    """caf_wave = 1 walks the Doppler blocks of the FFT-domain CAF with one wave of CTAs; every block is computed the
-    same way, so single frames, 5-frame CAF batches and 5-frame fused batches are bit-identical to caf_wave = 0.  At
-    (2**20, 256, 300) the 5-frame batch also takes doppler_fft_pow2_kernel<8>, checked against the oracle."""
-    import passiveradar_b200 as prb
+def test_xambg_frames_batch_matches_oracle(n, F, R):
+    """A 5-frame prc_xambg_frames_c64 batch on the FFT-domain CAF (one CTA per Doppler block and frame), sampled range
+    columns of the first and last frame against the oracle.  At (2**20, 256, 300) the batch also takes
+    doppler_fft_pow2_kernel<8>."""
     from oracle import xambg_oracle as xo
     nf = 5
     frames = [synth.make_frame(n, "P0", frame=190 + i) for i in range(nf)]
     ref = np.ascontiguousarray(np.stack([f[0] for f in frames]))
     srv = np.ascontiguousarray(np.stack([f[1] for f in frames]))
-    w = np.ascontiguousarray(signal.get_window(VC.KAISER, n), dtype=np.float64)
+    w = np.ascontiguousarray(signal.get_window(KAISER, n), dtype=np.float64)
     lib = _lib.load()
-    old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"), _lib.get_option("caf_wave"))
-    res = {}
+    old = (_lib.get_option("fft"), _lib.get_option("fft_min_n"))
     try:
         _lib.set_option("fft", 1)
         _lib.set_option("fft_min_n", 8192)
-        for wave in (0, 1):
-            _lib.set_option("caf_wave", wave)
-            single = prb.fast_xambg(ref[0], srv[0], R, F, n, w)
-            xb = np.empty((nf, F, R + 1), np.complex64)
-            _lib.check(lib.prc_xambg_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nf, n, R, F, w.ctypes.data, xb.ctypes.data,
-                                                _lib.MEM_HOST, 0, None, 0))
-            fb = np.empty((nf, F, R + 1), np.complex64)
-            _lib.check(lib.prc_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nf, n, R, 10, 1.0, R, F, w.ctypes.data,
-                                          fb.ctypes.data, None, None, _lib.MEM_HOST, 0, None, 0))
-            res[wave] = (single, xb, fb)
+        xb = np.empty((nf, F, R + 1), np.complex64)
+        _lib.check(lib.prc_xambg_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nf, n, R, F, w.ctypes.data, xb.ctypes.data,
+                                            _lib.MEM_HOST, 0, None, 0))
     finally:
         _lib.set_option("fft", old[0])
         _lib.set_option("fft_min_n", old[1])
-        _lib.set_option("caf_wave", old[2])
-    for a, b, what in zip(res[0], res[1], ("fast_xambg", "prc_xambg_frames_c64", "prc_frames_c64")):
-        assert np.array_equal(a, b), what
-    xb = res[1][1]
     lags = sorted({0, 1, R // 2, R - 1, R})
     worst = 0.0
     for i in (0, nf - 1):
         cols = {d: xo.fast_xambg_oracle(ref[i], np.roll(srv[i], -d), 0, F, n, w)[:, 0, 0] for d in lags}
         worst = max(worst, _rel_columns(xb[i][:, :, None], cols, lags, R, float(np.abs(xb[i]).max())))
-    record_parity(f"xambg/caf_wave_n{n}_F{F}_R{R}", E_vs_oracle_sampled_columns=worst)
+    record_parity(f"xambg/frames_n{n}_F{F}_R{R}", E_vs_oracle_sampled_columns=worst)
     assert worst <= TOL, worst
 
 
@@ -486,17 +541,19 @@ def test_caf_wave_grid_is_bit_identical(n, F, R):
 # (host function, kernel<template arguments>) of every launch in prcore.cu -> [(test id, variant, what it reaches)].
 # The launches in the headers' own launchers are covered where those headers are tested: the front end's in
 # tests/test_recording.py, CFAR_2D's and the frame chain's in tests/test_render.py.
-# Variant: "default" (shipped configuration), "fft" / "direct" (the both_paths fixture), or a VARIANTS child.
+# Variant: "default" (shipped configuration), or "fft" / "direct" (the both_paths fixture; "direct" also marks the
+# direct_form fixture).
 # A row is checked against the source, not the other way round: read the dispatch code before adding one.
 PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/test_kernel_variants.py::"
 FE, GAL, TRK = "tests/test_gpu_frontend.py::", "tests/test_gal_jpe.py::", "tests/test_tracking.py::"
 RS = "tests/test_rows_sweep.py::"
 PS = "tests/test_path_sweep.py::"
 DS = "tests/test_direct_sweep.py::"
-VARIANT_TEST = KV + "test_variant_matches_truth_and_reference"
+DIRECT_TEST = KV + "test_direct_form_matches_truth_and_reference"
+NLMS_TEST = KV + "test_nlms_matches_truth_and_reference"
 COVERAGE = {
     "launch_lagstream: lagstream_kernel<TILE_I, TILE_D>": [(PAR + "test_ls_matches_live_oracle", "direct", "LS, n <= 20000"),
-                                                           (VARIANT_TEST, "default", "ls_big, caf_big, frame: LS and CAF at config 2"),
+                                                           (DIRECT_TEST, "direct", "ls_big, caf_big, frame: LS and CAF at config 2"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "CAF: G = 1 at H = 512, G = 32, blocks over >= 3 CTAs, CTAs over >= 3 blocks"), (DS + "test_ls_direct_form_at_the_planner_edges", "default", "LS lag sums, M = 1 .. 2048")],
     "fft_twiddles: fft::fft_twiddle_kernel<R3>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 (n = 200000) and 8 (n = 10**6)"),
@@ -521,7 +578,6 @@ COVERAGE = {
     "caf_fft: fftc::caf_fft_kernel<R3, true>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16"),
-        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid"),
         (PS + "test_fused_frame_at_the_planner_edges", "default",
          "R3 = 16 against the frame truth (R + M - 1 = 3072); filterLen = 0: the staging without reuse; peek = 0")],
     "caf_fft: fftc::caf_fft_kernel<R3, false>": [
@@ -529,17 +585,17 @@ COVERAGE = {
         (PAR + "test_xambg_matches_live_oracle", "fft", "R3 = 4"),
         (FFT + "test_xambg_large_shapes_sampled_columns", "fft", "R3 = 8 (F = 64, D >= 16384)"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "fft", "R3 = 16 (R = 1200)"),
-        (KV + "test_caf_wave_grid_is_bit_identical", "default", "caf_wave = 1 grid")],
-    "xambg_device: weight_kernel": [(VARIANT_TEST, "default", "caf_big, frame"),
+        (KV + "test_xambg_frames_batch_matches_oracle", "default", "5-frame batches, one CTA per Doppler block and frame")],
+    "xambg_device: weight_kernel": [(DIRECT_TEST, "direct", "caf_big, frame"),
                                     (PAR + "test_xambg_matches_live_oracle", "direct", "lagstream CAF with a window"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "windowed lagstream cases")],
     "xambg_device: lagcorr_kernel<TILE_I, TILE_D>": [
-        (VARIANT_TEST, "default", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
+        (DIRECT_TEST, "direct", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
         (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "D = 1, ntaps 32 / 63, tap-weighted at G = 32, H = 512 and the nchunk loop")],
     "xambg_device: twiddle_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "every fast_xambg")],
     "xambg_device: doppler_fft_pow2_kernel<8>": [
-        (KV + "test_caf_wave_grid_is_bit_identical", "default", "5 frames x 38 column groups >= SM count"),
+        (KV + "test_xambg_frames_batch_matches_oracle", "default", "5 frames x 38 column groups >= SM count"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "direct", "R = 1200, F = 64"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "R = 1100, 3073, 5119")],
     "xambg_device: doppler_fft_pow2_kernel<2>": [(PAR + "test_xambg_matches_live_oracle", "direct", "F <= 4096"),
@@ -553,16 +609,16 @@ COVERAGE = {
     "xambg_device: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
                                          (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 1, 100, 200, 1500, 16384")],
-    "ls_device: levinson_kernel<1>": [(VARIANT_TEST, "default", "ls_big, ls_small"),
+    "ls_device: levinson_kernel<1>": [(DIRECT_TEST, "direct", "ls_big, ls_small"),
                                       (PAR + "test_ls_matches_live_oracle", "direct", ""),
         (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1 .. 1024")],
-    "ls_device: levinson_kernel<4>": [(VARIANT_TEST, "default", "ls_wide"),
+    "ls_device: levinson_kernel<4>": [(DIRECT_TEST, "direct", "ls_wide"),
                                       (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", ""),
         (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1025, 2048")],
-    "ls_device: fir_apply_kernel<TILE_I, TILE_D>": [(VARIANT_TEST, "default", "ls_small, ls_wide, toep"),
-                                                    (VARIANT_TEST, "default", "ls_big, frame at config 2"),
+    "ls_device: fir_apply_kernel<TILE_I, TILE_D>": [(DIRECT_TEST, "direct", "ls_small, ls_wide, toep"),
+                                                    (DIRECT_TEST, "direct", "ls_big, frame at config 2"),
         (DS + "test_ls_direct_form_at_the_planner_edges", "default", "Mpad = 10 .. 2050, circular and linear")],
-    "ls_toeplitz_device: shift_roll_kernel": [(VARIANT_TEST, "default", "toep"),
+    "ls_toeplitz_device: shift_roll_kernel": [(DIRECT_TEST, "direct", "toep"),
                                               (PAR + "test_ls_multiple_matches_reference_golden", "direct", "shifted bins"),
         (DS + "test_toeplitz_direct_form_with_peek_past_half_the_frame", "default", "peek >= n / 2")],
     "direct_xambg_device: piece_sum_kernel": [
@@ -576,7 +632,7 @@ COVERAGE = {
     "nlms_device: nlms_block_kernel<4, 512>": [(KV + "test_nlms_frames_past_the_sm_count_with_many_taps", "default", "M = 2000"),
         (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 1025, 2048")],
     "nlms_device: nlms_block_kernel<1>": [(PAR + "test_nlms_matches_reference_golden", "default", ""),
-                                          (VARIANT_TEST, "default", "nlms M = 410"),
+                                          (NLMS_TEST, "default", "M = 410"),
         (DS + "test_nlms_at_the_tiling_edges", "default", "M = 1 .. 1024, every last-tile length")],
     "nlms_device: nlms_block_kernel<2>": [(KV + "test_nlms_with_more_than_1024_taps_matches_c_oracle", "default", "M = 1110"),
         (DS + "test_nlms_at_the_tiling_edges", "default", "M = 1025, 2048")],
@@ -647,9 +703,7 @@ def test_every_prcore_launch_site_has_a_covering_gpu_test():
         assert reached, f"{site}: no test"
         for test_id, variant, _ in reached:
             assert _is_gpu_test(test_id), f"{site}: {test_id} is not a GPU test"
-            assert variant in ("default", "fft", "direct") or variant in VARIANTS, f"{site}: unknown variant {variant}"
-            if test_id == VARIANT_TEST:
-                assert variant in VARIANTS
+            assert variant in ("default", "fft", "direct"), f"{site}: unknown variant {variant}"
 
 
 def test_coverage_guard_sees_a_new_launch(tmp_path):
