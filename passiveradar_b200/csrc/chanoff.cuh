@@ -265,8 +265,16 @@ struct ArgParams {
     long long* part_k;
 };
 
+// (v, k) ranks above (bv, bk) in np.argmax's order: NaN above every number, then the larger value, then among equal
+// values (NaNs included) the lower index
+__device__ __forceinline__ bool arg_above(double v, long long k, double bv, long long bk) {
+    const bool n = isnan(v), bn = isnan(bv);
+    if (n != bn) return n;
+    return v > bv || ((n || v == bv) && k < bk);
+}
+
 __device__ __forceinline__ void arg_take(double& bv, long long& bk, double v, long long k) {
-    if (v > bv || (v == bv && k < bk)) { bv = v; bk = k; }
+    if (arg_above(v, k, bv, bk)) { bv = v; bk = k; }
 }
 
 __device__ __forceinline__ void arg_block(double& bv, long long& bk) {
@@ -291,7 +299,8 @@ __global__ void __launch_bounds__(ARG_THREADS) chanoff_argmax_kernel(const ArgPa
         if (p.mode == ARG_ABS) {
             const double a = hypot(v.x, v.y);
             if (p.out) static_cast<double*>(p.out)[k] = a;
-            if (a > bv) { bv = a; bk = k; }                  // a thread's k increase: strict > keeps the first
+            // a thread's k increase, so the first maximum (or first NaN) stays: take a larger value, or a first NaN
+            if (a > bv || (isnan(a) && !isnan(bv))) { bv = a; bk = k; }
         } else if (p.mode == ARG_COMPLEX) {
             static_cast<double2*>(p.out)[k] = v;
         } else {

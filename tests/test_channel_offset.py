@@ -175,15 +175,31 @@ def test_chanoff_kernels_build_for_sm90a_without_spills():
         assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in blk
 
 
-# every launch in chanoff.cuh -> the GPU tests that reach it
+# every launch in chanoff.cuh -> the GPU tests that reach it ("module::test" for a test in another file)
+SWEEP = "test_offset_sweep::"
 COVERAGE = {
-    "chanoff_iir_kernel<CPLX, BACKWARD>": ["test_offsets_and_lags_match_goldens", "test_main_py_shapes"],
-    "chanoff_load_kernel": ["test_xcorr_dtypes_and_values"],
-    "chanoff_twiddle_kernel": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values"],
-    "chanoff_fft_kernel<true>": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values"],
-    "chanoff_fft_kernel<false>": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values"],
-    "chanoff_argmax_kernel": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values"],
-    "chanoff_argmax_final_kernel": ["test_offsets_and_lags_match_goldens"],
+    "chanoff_iir_kernel<CPLX, BACKWARD>": ["test_offsets_and_lags_match_goldens", "test_main_py_shapes",
+                                           SWEEP + "test_channel_offset_across_the_decimator"],
+    "chanoff_load_kernel": ["test_xcorr_dtypes_and_values", SWEEP + "test_xcorr_at_every_transform_size"],
+    "chanoff_twiddle_kernel": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values",
+                               SWEEP + "test_xcorr_at_every_transform_size",
+                               SWEEP + "test_channel_offset_across_the_decimator"],
+    "chanoff_fft_kernel<true>": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values",
+                                 SWEEP + "test_xcorr_at_every_transform_size",
+                                 SWEEP + "test_channel_offset_across_the_decimator"],
+    "chanoff_fft_kernel<false>": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values",
+                                  SWEEP + "test_xcorr_at_every_transform_size",
+                                  SWEEP + "test_channel_offset_across_the_decimator"],
+    "chanoff_argmax_kernel": ["test_offsets_and_lags_match_goldens", "test_xcorr_dtypes_and_values",
+                              SWEEP + "test_xcorr_at_every_transform_size",
+                              SWEEP + "test_channel_offset_across_the_decimator",
+                              SWEEP + "test_periodic_input_keeps_the_first_of_many_near_equal_peaks",
+                              SWEEP + "test_nan_and_inf_inputs_rank_as_numpy_argmax_does"],
+    "chanoff_argmax_final_kernel": ["test_offsets_and_lags_match_goldens",
+                                    SWEEP + "test_channel_offset_across_the_decimator",
+                                    SWEEP + "test_periodic_input_keeps_the_first_of_many_near_equal_peaks",
+                                    SWEEP + "test_all_zero_s1_gives_the_first_lag",
+                                    SWEEP + "test_nan_and_inf_inputs_rank_as_numpy_argmax_does"],
 }
 
 
@@ -191,9 +207,11 @@ def test_every_chanoff_launch_has_a_covering_gpu_test():
     src = open(CHANOFF).read()
     sites = {m.group(1) + (m.group(2) or "") for m in re.finditer(r"([A-Za-z_]\w*)\s*(<[^<>;()]*>)?\s*<<<", src)}
     assert sites == set(COVERAGE), f"launch sites {sites} vs COVERAGE {set(COVERAGE)}"
-    this = open(os.path.abspath(__file__)).read()
     for tests in COVERAGE.values():
         for t in tests:
+            module, _, t = t.rpartition("::")
+            path = os.path.join(ROOT, "tests", module + ".py") if module else os.path.abspath(__file__)
+            this = open(path).read()
             i = this.index(f"\ndef {t}(")
             decorators = this[this.rindex("\n\n", 0, i):i]
             assert "@pytest.mark.gpu" in decorators, f"{t} is not a GPU test"
@@ -272,7 +290,14 @@ def test_xcorr_dtypes_and_values(dt1, dt2, nlead, nlag):
         assert _rel(wide, truth, np.abs(truth).max()) <= 1e-12
         assert _rel(got, want, np.abs(want).max()) <= (1e-12 if got.dtype.itemsize >= 8 and got.dtype != np.complex64 else 1e-5)
     short = prb.xcorr(s2, s1, nlead, nlag)          # len(s1) < len(padded s2): SciPy's swapped operands
-    assert short.shape == oo.xcorr_oracle(s2, s1, nlead, nlag).shape
+    want = oo.xcorr_oracle(s2, s1, nlead, nlag)
+    assert short.dtype == want.dtype and short.shape == want.shape
+    if short.dtype.kind in "iu":
+        np.testing.assert_array_equal(short, want)
+    else:                                           # values and conjugation of the swapped result
+        truth = oo.xcorr_oracle(s2.astype(np.complex128), s1.astype(np.complex128), nlead, nlag)
+        wide = prb.xcorr(s2.astype(np.complex128), s1.astype(np.complex128), nlead, nlag)
+        assert _rel(wide, truth, np.abs(truth).max()) <= 1e-12
 
 
 @pytest.mark.gpu
