@@ -168,12 +168,15 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
             fetch_staged<G::T, true>(v, stg, t, G::L);
         }
         fft::fft_n2p<R3>(v, t, S, [&] { if (nu < u1 && !(nk == 2)) issue(nu, ng, nq, nk); });
-        if (ck == 0) {
+        // Ys', Yr', AccP and AccQ are updated by selects in place, not by assignments on separate branches: with
+        // branches ptxas kept each array in two register sets and copied it back and forth on every item
+        // (~100 MOV per item; without them the frame pass at C2 takes 8 % less time)
+        if (ck < 2) {
 #pragma unroll
-            for (int r = 0; r < 16; ++r) ys[r] = v[r];
-        } else if (ck == 1) {
-#pragma unroll
-            for (int r = 0; r < 16; ++r) yr[r] = v[r];
+            for (int r = 0; r < 16; ++r) {
+                ys[r] = ck == 0 ? v[r] : ys[r];
+                yr[r] = ck == 1 ? v[r] : yr[r];
+            }
         } else if (ck == 2) {
 #pragma unroll
             for (int r = 0; r < 16; ++r) {
@@ -189,14 +192,19 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
                 cmacc(accQ[r], v[r], yr[r]);                             // AccQ += X_caf conj(Yr')
                 cmacc(accP[r], v[r], ys[r]);                             // AccP += X_caf conj(Ys')
             }
-            if (cq + 1 == cg.nseg) {                                     // the block's last segment: write its sums
+            const bool last = cq + 1 == cg.nseg;                          // the block's last segment: write its sums
+            if (last) {
                 float2* dst = p.acc + ((size_t)blockIdx.y * p.F + cu) * 2 * G::L;
 #pragma unroll
                 for (int r = 0; r < 16; ++r) {
                     dst[r * G::T + t] = accP[r];
                     dst[G::L + r * G::T + t] = accQ[r];
-                    accP[r] = accQ[r] = make_float2(0.f, 0.f);
                 }
+            }
+#pragma unroll
+            for (int r = 0; r < 16; ++r) {
+                accP[r] = last ? make_float2(0.f, 0.f) : accP[r];
+                accQ[r] = last ? make_float2(0.f, 0.f) : accQ[r];
             }
         }
         if (nu != cu) cg = ng;
