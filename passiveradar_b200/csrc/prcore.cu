@@ -139,7 +139,6 @@ struct Ctx {
                                                                       // mean / thr / count, candidate slots, results
     int trk_plan_n = -1, trk_nnodes = 0, trk_nlevels = 0;             // map size trk_plan was built for, its shape
     int tw_F = 0;
-    int status_slot = 0;      // which int of `status` the direct-form Toeplitz solve reports to
     void* pin[2] = {nullptr, nullptr};      // page-locked bounce buffers for pageable host arrays (h2d / d2h below)
     cudaEvent_t pin_ev[2] = {nullptr, nullptr};
     bool pin_ready = false;
@@ -364,36 +363,41 @@ int choose_geo(int blk_len, long long outer, int nlag, int nsm, Geo* g) {
 }
 
 struct StreamGeo {
-    int H, HT, G, steps, threads, ncta, maxpieces;
-    long long per_cta, total;
+    int HT, threads, ncta;
     size_t smem;
+    LagStreamParams sp;   // the geometry's fields (blk_len, nblk, total .. maxpieces); operands, block starts and
+                          // s_linear are the caller's
 };
 
 // CTAs per problem: fill every SM with two co-resident CTAs, but keep >= 2 full steps per CTA
 int choose_stream(int blk_len, int nblk, int nprob, int nlag, int nsm, StreamGeo* g) {
     const int TI = TILE_I, TD = TILE_D;
-    g->H = ceil_div(nlag, TD);
-    g->HT = g->H * TD;
-    if (g->H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
-    int G = std::max(1, std::min(32, 256 / g->H));
-    g->total = (long long)nblk * blk_len;
+    LagStreamParams& s = g->sp;
+    s = LagStreamParams{};
+    s.blk_len = blk_len;
+    s.nblk = nblk;
+    s.H = ceil_div(nlag, TD);
+    g->HT = s.H * TD;
+    if (s.H > 512) return fail(PRC_E_INVALID, "%d lags exceed the supported maximum of %d", nlag, 512 * TD);
+    int G = std::max(1, std::min(32, 256 / s.H));
+    s.total = (long long)nblk * blk_len;
     long long want = std::max(1, 2 * nsm / nprob);
     const long long min_per_cta = (long long)G * TI * 2;
-    want = std::min<long long>(want, std::max<long long>(1, g->total / min_per_cta));
-    g->per_cta = (g->total + want - 1) / want;
-    g->ncta = (int)((g->total + g->per_cta - 1) / g->per_cta);
-    g->G = (int)std::max<long long>(1, std::min<long long>(G, (g->per_cta + TI - 1) / TI));
-    g->steps = std::max(2, 100 / TI);
-    while (g->steps > 1 && (long long)g->G * g->steps * TI > g->per_cta + g->G * TI) --g->steps;
+    want = std::min<long long>(want, std::max<long long>(1, s.total / min_per_cta));
+    s.per_cta = (s.total + want - 1) / want;
+    g->ncta = (int)((s.total + s.per_cta - 1) / s.per_cta);
+    s.G = (int)std::max<long long>(1, std::min<long long>(G, (s.per_cta + TI - 1) / TI));
+    s.steps = std::max(2, 100 / TI);
+    while (s.steps > 1 && (long long)s.G * s.steps * TI > s.per_cta + s.G * TI) --s.steps;
     for (;;) {
-        const size_t Lmax = (size_t)g->G * g->steps * TI;
-        g->smem = (2 * (2 * Lmax + g->HT) + 2 * (size_t)g->G * g->HT) * sizeof(float2);   // staging, sums, compensations
-        if (g->smem <= 100 * 1024 || g->steps == 1) break;
-        --g->steps;
+        const size_t Lmax = (size_t)s.G * s.steps * TI;
+        g->smem = (2 * (2 * Lmax + g->HT) + 2 * (size_t)s.G * g->HT) * sizeof(float2);   // staging, sums, compensations
+        if (g->smem <= 100 * 1024 || s.steps == 1) break;
+        --s.steps;
     }
     if (g->smem > SMEM_LIMIT) return fail(PRC_E_INVALID, "lag-correlation tile needs %zu B of shared memory", g->smem);
-    g->maxpieces = (int)std::min<long long>(g->ncta, (blk_len + g->per_cta - 2) / g->per_cta + 1);
-    g->threads = ((g->H * g->G + 31) / 32) * 32;
+    s.maxpieces = (int)std::min<long long>(g->ncta, (blk_len + s.per_cta - 2) / s.per_cta + 1);
+    g->threads = ((s.H * s.G + 31) / 32) * 32;
     return PRC_OK;
 }
 
@@ -505,20 +509,18 @@ int ls_fft_corr(Ctx* c, const LsFftPlan& pl, const float2* ref, const float2* sr
     return check_launch("lscorr_fft_kernel");
 }
 
-// (T + reg I) w = rhs for nf frames: taps -> c->lstaps [f0 + nf][M], status -> c->status [f0 + nf], from frame f0 on
-int levinson_launch(Ctx* c, int nchunk, int HT, int M, double reg, int nf, int f0 = 0) {
-    TRY(c->lstaps.ensure((size_t)(f0 + nf) * M * sizeof(float2)));
-    TRY(c->status.ensure((size_t)(f0 + nf) * sizeof(int)));
+// (T + reg I) w = rhs for nf frames from the lag sums in c->partial: taps -> taps [nf][M], status -> status [nf].
+// thr: threads of a levinson_kernel<1> CTA (M <= 1024); 0: one thread per unknown (a CTA of 1024 threads would own a
+// whole SM's registers and could not share it with the other slots' transform CTAs; the recursion only ever uses
+// ceil(M / 32) warps)
+int levinson_launch(Ctx* c, int nchunk, int HT, int M, double reg, int nf, float2* taps, int* status, int thr = 0) {
     LevinsonParams lp{};
     lp.partial = c->partial.as<float2>();
     lp.nchunk = nchunk; lp.HT = HT; lp.M = M; lp.reg = reg;
-    lp.taps = c->lstaps.as<float2>() + (size_t)f0 * M;
-    lp.status = c->status.as<int>() + f0;
+    lp.taps = taps; lp.status = status;
     {
         ProfScope ps(c, K_LEVINSON);
-        // one thread per unknown (a CTA of 1024 threads would own a whole SM's registers and could not share it
-        // with the other slots' transform CTAs; the recursion only ever uses ceil(M / 32) warps)
-        const int thr = std::max(64, (M + 31) & ~31);
+        if (!thr) thr = std::max(64, (M + 31) & ~31);
         if (M <= 1024) levinson_kernel<1><<<nf, thr, levinson_smem(M, thr), c->stream>>>(lp);
         else levinson_kernel<4><<<nf, 512, levinson_smem(M, 512), c->stream>>>(lp);
     }
@@ -563,15 +565,42 @@ int fir_fft(Ctx* c, int r3, const float2* ref, const float2* srv, float2* out, l
 }
 
 // ---- CAF block sums
+int decimator_offset(long long ntaps, long long D) {   // resample_poly alignment, up = 1
+    const long long half = (ntaps - 1) / 2;
+    const long long pre_pad = D - half % D;
+    const long long pre_remove = (half + pre_pad) / D;
+    return (int)(pre_remove * D - pre_pad);
+}
+
+// fast_xambg's decimator: factor D = int(n / F) and ntaps taps (taps: device float32; NULL: a boxcar of D + 1, or no
+// filter at all when D = 1).  Doppler block j covers samples j D + c0 - (ntaps - 1) .. j D + c0.
+struct Decimator {
+    long long D, ntaps;
+    int c0;
+    const float* taps;
+    bool boxcar() const { return taps == nullptr && ntaps == D + 1; }
+};
+
+// dtaps32: the tap-weighted decimator (ndtaps taps), or NULL.  No checks: D < 1 is the callers' to refuse.
+Decimator decimator(long long n, int F, const float* dtaps32, long long ndtaps) {
+    Decimator d{n / F, 1, 0, nullptr};
+    if (d.D <= 1) return d;   // resample_poly(x, 1, 1) returns x (scipy _signaltools.py:4028)
+    d.ntaps = dtaps32 ? ndtaps : d.D + 1;
+    d.c0 = decimator_offset(d.ntaps, d.D);
+    d.taps = dtaps32;
+    return d;
+}
+
 struct CafFftPlan {
     bool on = false;
     int r3 = 8, Bmax = 0, HT = 0;
 };
 
 // mfuse: taps of the clutter filter fused into the surveillance operand (0: none)
-CafFftPlan caf_fft_plan(long long n, int R, int F, long long ntaps, long long D, bool boxcar, int mfuse) {
+CafFftPlan caf_fft_plan(long long n, int R, int F, const Decimator& dm, int mfuse) {
     CafFftPlan pl;
-    if (!g_fft.load() || n < g_fft_min_n.load() || !boxcar || D < 32 || F < 1) return pl;
+    const long long ntaps = dm.ntaps;
+    if (!g_fft.load() || n < g_fft_min_n.load() || !dm.boxcar() || dm.D < 32 || F < 1) return pl;
     double best = 0.0;
     for (int r3 : {4, 8, 16}) {
         const int L = 256 * r3;
@@ -590,14 +619,14 @@ CafFftPlan caf_fft_plan(long long n, int R, int F, long long ntaps, long long D,
 // P[frame][j][d] -> c->fftP; wp == nullptr: plain CAF of (ref, srv); else srv is cleaned on the fly with the taps
 // spectrum wp ([nf][L], same r3)
 int caf_fft(Ctx* c, const CafFftPlan& pl, const float2* ref, const float2* srv, long long n, Batch bt, int R, int F,
-            const float* win32, long long D, int c0, long long ntaps, const float2* wp, int M, int peek) {
+            const float* win32, const Decimator& dm, const float2* wp, int M, int peek) {
     const float2* tw;
     TRY(fft_twiddles(c, pl.r3, &tw));
     TRY(c->fftP.ensure((size_t)bt.nf * F * pl.HT * sizeof(float2)));
     fftc::CafFftParams p{};
     p.ref = ref; p.srv = srv; p.frame_stride = bt.stride; p.win = win32; p.wp = wp;
     p.n = (int)n; p.R = R; p.F = F; p.M = M; p.peek = peek;
-    p.D = D; p.c0 = c0; p.ntaps = (int)ntaps; p.Bmax = pl.Bmax;
+    p.D = dm.D; p.c0 = dm.c0; p.ntaps = (int)dm.ntaps; p.Bmax = pl.Bmax;
     p.P = c->fftP.as<float2>(); p.HT = pl.HT; p.tw = tw;
     const dim3 grid(F, bt.nf);
     {
@@ -611,59 +640,84 @@ int caf_fft(Ctx* c, const CafFftPlan& pl, const float2* ref, const float2* srv, 
 // --------------------------------------------------------------------------- device pipelines
 // All pointers are device pointers; everything is enqueued on c->stream.
 
-int decimator_offset(long long ntaps, long long D) {   // resample_poly alignment, up = 1
-    const long long half = (ntaps - 1) / 2;
-    const long long pre_pad = D - half % D;
-    const long long pre_remove = (half + pre_pad) / D;
-    return (int)(pre_remove * D - pre_pad);
+// The CAF's block sums as the Doppler stage reads them: [nf][F][nchunk][HT] at src.  per_cta > 0: the lagstream
+// layout, block j holds stream_pieces(j, blk_len, per_cta) of its nchunk rows; 0: all nchunk rows.
+struct BlockSums {
+    const float2* src;
+    int nchunk, HT, blk_len;
+    long long per_cta;
+};
+
+// Doppler stage: the block sums of nf frames -> out [nf][F][R + 1]
+int doppler_stage(Ctx* c, const BlockSums& bs, int R, int F, int nf, float2* out) {
+    if (c->tw_F != F) {
+        TRY(c->tw.ensure((size_t)F * sizeof(float2)));
+        twiddle_kernel<<<ceil_div(F, 256), 256, 0, c->stream>>>(c->tw.as<float2>(), F);
+        TRY(check_launch("twiddle_kernel"));
+        c->tw_F = F;
+    }
+    DopplerParams d{};
+    d.partial = bs.src;
+    d.tw = c->tw.as<float2>();
+    d.out = out;
+    d.F = F; d.R = R; d.nchunk = bs.nchunk; d.HT = bs.HT;
+    d.partial_fstride = (long long)F * bs.nchunk * bs.HT;
+    d.out_fstride = (long long)F * (R + 1);
+    d.blk_len = bs.blk_len; d.per_cta = bs.per_cta;
+    int logF = 0;
+    while ((1 << logF) < F) ++logF;
+    d.logF = logF;
+    const bool pow2 = (1 << logF) == F && F >= 2;
+    ProfScope ps_doppler(c, K_DOPPLER);
+    if (pow2 && F <= 8192) {
+        if (F <= 1024 && (long long)ceil_div(R + 1, 8) * nf >= c->nsm) {
+            const size_t sm = (size_t)2 * F * 8 * sizeof(float2);
+            doppler_fft_pow2_kernel<8><<<dim3(ceil_div(R + 1, 8), nf), 256, sm, c->stream>>>(d);
+        } else if (F <= 4096) {     // also the small-grid case: 2 columns per CTA fill more SMs
+            const size_t sm = (size_t)2 * F * 2 * sizeof(float2);
+            doppler_fft_pow2_kernel<2><<<dim3(ceil_div(R + 1, 2), nf), 256, sm, c->stream>>>(d);
+        } else {
+            const size_t sm = (size_t)2 * F * sizeof(float2);
+            doppler_fft_pow2_kernel<1><<<dim3(R + 1, nf), 256, sm, c->stream>>>(d);
+        }
+        TRY(check_launch("doppler_fft_pow2_kernel"));
+    } else {
+        TRY(c->pbuf.ensure((size_t)F * (R + 1) * sizeof(float2)));
+        for (int fr = 0; fr < nf; ++fr) {      // any F: chunk sum + direct DFT, frame by frame
+            chunk_sum_kernel<<<ceil_div((long long)F * (R + 1), 256), 256, 0, c->stream>>>(
+                d.partial + (size_t)fr * d.partial_fstride, c->pbuf.as<float2>(), F, R, bs.nchunk, bs.HT, bs.blk_len, bs.per_cta, d);
+            TRY(check_launch("chunk_sum_kernel"));
+            doppler_dft_kernel<<<dim3(ceil_div(R + 1, 128), F), 128, 0, c->stream>>>(
+                c->pbuf.as<float2>(), c->tw.as<float2>(), out + (size_t)fr * d.out_fstride, F, R);
+            TRY(check_launch("doppler_dft_kernel"));
+        }
+    }
+    return PRC_OK;
 }
 
 // bt.nf > 1 (a batch of frames) and fuse_wp != nullptr (clutter filter applied inside the CAF kernel, taps spectrum
-// [nf][L] for the transform length of caf_fft_plan(..., fuse_M)) exist on the FFT-domain path only; p_ready: the block
-// sums are already in c->fftP (one-pass frame), only the Doppler stage runs
+// [nf][L] for the transform length of caf_fft_plan(..., fuse_M)) exist on the FFT-domain path only
 int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int R, int F,
                  const float* win32, const float* dtaps32, long long ndtaps, float2* out, Batch bt = Batch{},
-                 const float2* fuse_wp = nullptr, int fuse_M = 0, int fuse_peek = 0, bool p_ready = false) {
+                 const float2* fuse_wp = nullptr, int fuse_M = 0, int fuse_peek = 0) {
     if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
     if (F < 1 || R < 0) return fail(PRC_E_INVALID, "freq_bins=%d / range_bins=%d invalid", F, R);
-    const long long D = n / F;
-    if (D < 1) return fail(PRC_E_INVALID, "decimation factor int(n/freq_bins) is 0 (n=%lld, freq_bins=%d)", n, F);
-    long long ntaps;
-    int c0;
-    const float* taps = nullptr;
-    if (D == 1) {            // resample_poly(x, 1, 1) returns x (scipy _signaltools.py:4028)
-        ntaps = 1;
-        c0 = 0;
-    } else if (dtaps32 == nullptr) {
-        ntaps = D + 1;
-        c0 = decimator_offset(ntaps, D);
-    } else {
-        ntaps = ndtaps;
-        c0 = decimator_offset(ntaps, D);
-        taps = dtaps32;
-    }
-    if (ntaps > (1ll << 30)) return fail(PRC_E_INVALID, "decimator too long");
-    Geo g{};
-    long long d_per_cta = 0;
-    const float2* dop_src = nullptr;                // Doppler-stage input when it is not c->partial
-    const CafFftPlan fp = caf_fft_plan(n, R, F, ntaps, D, taps == nullptr && ntaps == D + 1, fuse_wp ? fuse_M : 0);
-    if ((bt.nf > 1 || fuse_wp) && !fp.on && !p_ready)
+    const Decimator dm = decimator(n, F, dtaps32, ndtaps);
+    if (dm.D < 1) return fail(PRC_E_INVALID, "decimation factor int(n/freq_bins) is 0 (n=%lld, freq_bins=%d)", n, F);
+    if (dm.ntaps > (1ll << 30)) return fail(PRC_E_INVALID, "decimator too long");
+    const int ntaps = (int)dm.ntaps;
+    const CafFftPlan fp = caf_fft_plan(n, R, F, dm, fuse_wp ? fuse_M : 0);
+    if ((bt.nf > 1 || fuse_wp) && !fp.on)
         return fail(PRC_E_INVALID, "batched / fused CAF needs the FFT-domain path (n=%lld, F=%d, R=%d not eligible)", n, F, R);
-    if (p_ready) {
-        // ---- block sums already in c->fftP ([nf][F][HT], the one-pass frame's caf_combine_kernel): Doppler stage only
-        g.nchunk = 1;
-        g.HT = (R + 2) & ~1;
-        dop_src = c->fftP.as<float2>();
-    } else if (fp.on) {
+    BlockSums bs;
+    if (fp.on) {
         // ---- FFT-domain block correlations (fftcorr.cuh): one CTA per Doppler block, P[j][d] straight from the channels
-        TRY(caf_fft(c, fp, ref, srv, n, bt, R, F, win32, D, c0, ntaps, fuse_wp, fuse_M, fuse_peek));
-        g.nchunk = 1;
-        g.HT = fp.HT;
-        dop_src = c->fftP.as<float2>();
-    } else if (taps == nullptr && ntaps >= 64) {   // tiny Doppler blocks: one flush per block would dominate
+        TRY(caf_fft(c, fp, ref, srv, n, bt, R, F, win32, dm, fuse_wp, fuse_M, fuse_peek));
+        bs = {c->fftP.as<float2>(), 1, fp.HT, ntaps, 0};
+    } else if (dm.taps == nullptr && ntaps >= 64) {   // tiny Doppler blocks: one flush per block would dominate
         StreamGeo sg;
-        TRY(choose_stream((int)ntaps, F, 1, R + 1, c->nsm, &sg));
-        TRY(c->partial.ensure((size_t)F * sg.maxpieces * sg.HT * sizeof(float2)));
+        TRY(choose_stream(ntaps, F, 1, R + 1, c->nsm, &sg));
+        TRY(c->partial.ensure((size_t)F * sg.sp.maxpieces * sg.HT * sizeof(float2)));
         const float2* xw = ref;
         if (win32) {
             TRY(c->refw.ensure((size_t)n * sizeof(float2)));
@@ -674,105 +728,54 @@ int xambg_device(Ctx* c, const float2* ref, const float2* srv, long long n, int 
             TRY(check_launch("weight_kernel"));
             xw = c->refw.as<float2>();
         }
-        LagStreamParams sp{};
+        LagStreamParams sp = sg.sp;
         sp.x = xw;
         sp.s[0] = srv; sp.s[1] = srv;
-        sp.dmin[0] = 0; sp.dmin[1] = 0;
         sp.n = (int)n;
-        sp.blk_first_lo = (long long)c0 - (ntaps - 1);
-        sp.blk_stride = D;
-        sp.blk_len = (int)ntaps;
-        sp.nblk = F;
-        sp.total = sg.total;
-        sp.per_cta = sg.per_cta;
-        sp.H = sg.H; sp.G = sg.G; sp.steps = sg.steps;
-        sp.maxpieces = sg.maxpieces;
+        sp.blk_first_lo = (long long)dm.c0 - (ntaps - 1);
+        sp.blk_stride = dm.D;
         sp.partial = c->partial.as<float2>();
         {
             ProfScope ps(c, K_LAGCORR_CAF);
             launch_lagstream(dim3(sg.ncta, 1), sg.threads, sg.smem, c->stream, sp);
         }
         TRY(check_launch("lagstream_kernel(caf)"));
-        g.nchunk = sg.maxpieces;
-        g.HT = sg.HT;
-        d_per_cta = sg.per_cta;
+        bs = {c->partial.as<float2>(), sp.maxpieces, sg.HT, ntaps, sp.per_cta};
     } else {
-    TRY(choose_geo((int)ntaps, F, R + 1, c->nsm, &g));
-    TRY(c->partial.ensure((size_t)F * g.nchunk * g.HT * sizeof(float2)));
-
-    LagCorrParams p{};
-    p.x = ref;
-    p.s[0] = srv; p.s[1] = srv;
-    p.dmin[0] = 0; p.dmin[1] = 0;
-    p.win = win32;
-    p.taps = taps;
-    p.n = (int)n;
-    p.blk_first_lo = (long long)c0 - (ntaps - 1);
-    p.blk_stride = D;
-    p.blk_len = (int)ntaps;
-    p.nblk = F;
-    p.nchunk = g.nchunk;
-    p.chunk_len = g.chunk_len;
-    p.H = g.H; p.G = g.G; p.steps = g.steps;
-    p.partial = c->partial.as<float2>();
-    {
-        ProfScope ps(c, K_LAGCORR_CAF);
-        const dim3 grid((unsigned)((long long)F * g.nchunk), 1);
-        lagcorr_kernel<TILE_I, TILE_D><<<grid, g.threads, g.smem, c->stream>>>(p);
-    }
-    TRY(check_launch("lagcorr_kernel(caf)"));
-    }
-
-    // Doppler stage
-    if (c->tw_F != F) {
-        TRY(c->tw.ensure((size_t)F * sizeof(float2)));
-        twiddle_kernel<<<ceil_div(F, 256), 256, 0, c->stream>>>(c->tw.as<float2>(), F);
-        TRY(check_launch("twiddle_kernel"));
-        c->tw_F = F;
-    }
-    DopplerParams d{};
-    d.partial = dop_src ? dop_src : c->partial.as<float2>();
-    d.tw = c->tw.as<float2>();
-    d.out = out;
-    d.F = F; d.R = R; d.nchunk = g.nchunk; d.HT = g.HT;
-    d.partial_fstride = (long long)F * g.nchunk * g.HT;
-    d.out_fstride = (long long)F * (R + 1);
-    d.blk_len = (int)ntaps; d.per_cta = d_per_cta;
-    int logF = 0;
-    while ((1 << logF) < F) ++logF;
-    d.logF = logF;
-    const bool pow2 = (1 << logF) == F && F >= 2;
-    ProfScope ps_doppler(c, K_DOPPLER);
-    if (pow2 && F <= 8192) {
-        if (F <= 1024 && (long long)ceil_div(R + 1, 8) * bt.nf >= c->nsm) {
-            const size_t sm = (size_t)2 * F * 8 * sizeof(float2);
-            doppler_fft_pow2_kernel<8><<<dim3(ceil_div(R + 1, 8), bt.nf), 256, sm, c->stream>>>(d);
-        } else if (F <= 4096) {     // also the small-grid case: 2 columns per CTA fill more SMs
-            const size_t sm = (size_t)2 * F * 2 * sizeof(float2);
-            doppler_fft_pow2_kernel<2><<<dim3(ceil_div(R + 1, 2), bt.nf), 256, sm, c->stream>>>(d);
-        } else {
-            const size_t sm = (size_t)2 * F * sizeof(float2);
-            doppler_fft_pow2_kernel<1><<<dim3(R + 1, bt.nf), 256, sm, c->stream>>>(d);
+        Geo g{};
+        TRY(choose_geo(ntaps, F, R + 1, c->nsm, &g));
+        TRY(c->partial.ensure((size_t)F * g.nchunk * g.HT * sizeof(float2)));
+        LagCorrParams p{};
+        p.x = ref;
+        p.s[0] = srv; p.s[1] = srv;
+        p.dmin[0] = 0; p.dmin[1] = 0;
+        p.win = win32;
+        p.taps = dm.taps;
+        p.n = (int)n;
+        p.blk_first_lo = (long long)dm.c0 - (ntaps - 1);
+        p.blk_stride = dm.D;
+        p.blk_len = ntaps;
+        p.nblk = F;
+        p.nchunk = g.nchunk;
+        p.chunk_len = g.chunk_len;
+        p.H = g.H; p.G = g.G; p.steps = g.steps;
+        p.partial = c->partial.as<float2>();
+        {
+            ProfScope ps(c, K_LAGCORR_CAF);
+            const dim3 grid((unsigned)((long long)F * g.nchunk), 1);
+            lagcorr_kernel<TILE_I, TILE_D><<<grid, g.threads, g.smem, c->stream>>>(p);
         }
-        TRY(check_launch("doppler_fft_pow2_kernel"));
-    } else {
-        TRY(c->pbuf.ensure((size_t)F * (R + 1) * sizeof(float2)));
-        for (int fr = 0; fr < bt.nf; ++fr) {      // any F: chunk sum + direct DFT, frame by frame
-            chunk_sum_kernel<<<ceil_div((long long)F * (R + 1), 256), 256, 0, c->stream>>>(
-                d.partial + (size_t)fr * d.partial_fstride, c->pbuf.as<float2>(), F, R, g.nchunk, g.HT, (int)ntaps, d_per_cta, d);
-            TRY(check_launch("chunk_sum_kernel"));
-            doppler_dft_kernel<<<dim3(ceil_div(R + 1, 128), F), 128, 0, c->stream>>>(
-                c->pbuf.as<float2>(), c->tw.as<float2>(), out + (size_t)fr * d.out_fstride, F, R);
-            TRY(check_launch("doppler_dft_kernel"));
-        }
+        TRY(check_launch("lagcorr_kernel(caf)"));
+        bs = {c->partial.as<float2>(), g.nchunk, g.HT, ntaps, 0};
     }
-    return PRC_OK;
+    return doppler_stage(c, bs, R, F, bt.nf, out);
 }
 
-// bt.nf > 1 (a batch of frames; taps_out then receives [nf][M]) and need_out == false (only the taps are wanted: the
-// caller applies them inside the CAF kernel) exist on the FFT-domain path only
+// bt.nf > 1 (a batch of frames; taps_out then receives [nf][M]) and out == nullptr (only the taps are wanted: the
+// caller applies them inside the CAF kernel) exist on the FFT-domain path only.  status_at: the int of c->status the
+// direct-form solve reports to.
 int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int filter_len, int peek,
-              double reg, float2* out, float2* taps_out, bool linear = false, Batch bt = Batch{}, bool need_out = true) {
+              double reg, float2* out, float2* taps_out, bool linear = false, Batch bt = Batch{}, int status_at = 0) {
     // linear: LS_Filter_Toeplitz semantics -- correlations and FIR treat ref/srv as zero outside [0, n)
     if (n <= 0 || n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
     if (filter_len < 0 || peek < 0 || filter_len + peek < 1)
@@ -780,35 +783,29 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
     const int M = filter_len + peek;
     if (M > 2048) return fail(PRC_E_INVALID, "%d taps exceed the Toeplitz solver's maximum of 2048", M);
     const LsFftPlan lf = ls_fft_plan(c, n, M, bt.nf);
-    if ((bt.nf > 1 || !need_out) && !lf.on)
+    if ((bt.nf > 1 || !out) && !lf.on)
         return fail(PRC_E_INVALID, "batched LS filter needs the FFT-domain path (n=%lld, %d taps not eligible)", n, M);
     if (lf.on) {
         // ---- FFT-domain path (fftcorr.cuh): block spectra -> lag sums -> float64 Toeplitz solve -> overlap-save FIR
         TRY(ls_fft_corr(c, lf, ref, srv, n, bt, M, peek, linear));
-        TRY(levinson_launch(c, lf.ncta, lf.HT, M, reg, bt.nf));
-        if (need_out) TRY(fir_fft(c, lf.r3, ref, srv, out, n, bt, M, peek, linear));
+        TRY(c->lstaps.ensure((size_t)bt.nf * M * sizeof(float2)));
+        TRY(c->status.ensure((size_t)bt.nf * sizeof(int)));
+        TRY(levinson_launch(c, lf.ncta, lf.HT, M, reg, bt.nf, c->lstaps.as<float2>(), c->status.as<int>()));
+        if (out) TRY(fir_fft(c, lf.r3, ref, srv, out, n, bt, M, peek, linear));
         if (taps_out)
             CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)bt.nf * M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
         return PRC_OK;
     }
     TRY(c->lstaps.ensure((size_t)M * sizeof(float2)));
-    TRY(c->status.ensure(sizeof(int)));
+    TRY(c->status.ensure((size_t)(status_at + 1) * sizeof(int)));
     StreamGeo sg;
     TRY(choose_stream((int)n, 1, 2, M, c->nsm, &sg));
-    TRY(c->partial.ensure((size_t)2 * sg.maxpieces * sg.HT * sizeof(float2)));
-    LagStreamParams sp{};
+    TRY(c->partial.ensure((size_t)2 * sg.sp.maxpieces * sg.HT * sizeof(float2)));
+    LagStreamParams sp = sg.sp;
     sp.x = ref;
     sp.s[0] = ref; sp.s[1] = srv;
-    sp.dmin[0] = 0; sp.dmin[1] = -peek;
+    sp.dmin[1] = -peek;
     sp.n = (int)n;
-    sp.blk_first_lo = 0;
-    sp.blk_stride = 0;
-    sp.blk_len = (int)n;
-    sp.nblk = 1;
-    sp.total = sg.total;
-    sp.per_cta = sg.per_cta;
-    sp.H = sg.H; sp.G = sg.G; sp.steps = sg.steps;
-    sp.maxpieces = sg.maxpieces;
     sp.s_linear = linear ? 1 : 0;
     sp.partial = c->partial.as<float2>();
     {
@@ -816,21 +813,8 @@ int ls_device(Ctx* c, const float2* ref, const float2* srv, long long n, int fil
         launch_lagstream(dim3(sg.ncta, 2), sg.threads, sg.smem, c->stream, sp);
     }
     TRY(check_launch("lagstream_kernel(ls)"));
-
-    LevinsonParams lp{};
-    lp.partial = c->partial.as<float2>();
-    lp.nchunk = sg.maxpieces;      // == pieces of the single block == ncta
-    lp.HT = sg.HT;
-    lp.M = M;
-    lp.reg = reg;
-    lp.taps = c->lstaps.as<float2>();
-    lp.status = c->status.as<int>() + c->status_slot;
-    {
-        ProfScope ps(c, K_LEVINSON);
-        if (M <= 1024) levinson_kernel<1><<<1, 1024, levinson_smem(M, 1024), c->stream>>>(lp);
-        else levinson_kernel<4><<<1, 512, levinson_smem(M, 512), c->stream>>>(lp);
-    }
-    TRY(check_launch("levinson_kernel"));
+    // one CTA; its chunks are the pieces of the single block (== ncta)
+    TRY(levinson_launch(c, sp.maxpieces, sg.HT, M, reg, 1, c->lstaps.as<float2>(), c->status.as<int>() + status_at, 1024));
 
     FirParams fp{};
     fp.ref = ref; fp.srv = srv; fp.taps = c->lstaps.as<float2>(); fp.out = out;
@@ -1026,27 +1010,22 @@ int direct_xambg_device(Ctx* c, const float2* ref, const float2* srv, long long 
     TRY(c->rs.ensure((size_t)n * sizeof(float2)));
     StreamGeo sg;
     TRY(choose_stream((int)n, 1, 1, R + 1, c->nsm, &sg));
-    TRY(c->partial.ensure((size_t)sg.maxpieces * sg.HT * sizeof(float2)));
+    TRY(c->partial.ensure((size_t)sg.sp.maxpieces * sg.HT * sizeof(float2)));
     const double cpi = (double)n / fs;
     for (int f = 0; f < F; ++f) {
         const double df = ((double)f - 0.5 * (double)F) / cpi;
         const MixParams m = make_mix(ref, IQ_C64, n, MIX_C64, df, fs, 0.0);
         TRY(mix_chunks_device(c, K_MISC, chunk_params(m, 1, 0, nullptr, 0), c->rs.as<float2>()));
-        LagStreamParams sp{};
+        LagStreamParams sp = sg.sp;
         sp.x = c->rs.as<float2>();
         sp.s[0] = srv; sp.s[1] = srv;
-        sp.dmin[0] = 0; sp.dmin[1] = 0;
         sp.n = (int)n;
-        sp.blk_first_lo = 0; sp.blk_stride = 0; sp.blk_len = (int)n; sp.nblk = 1;
-        sp.total = sg.total; sp.per_cta = sg.per_cta;
-        sp.H = sg.H; sp.G = sg.G; sp.steps = sg.steps;
-        sp.maxpieces = sg.maxpieces;
         sp.s_linear = 1;
         sp.partial = c->partial.as<float2>();
         {
             ProfScope ps(c, K_LAGCORR_CAF);
             launch_lagstream(dim3(sg.ncta, 1), sg.threads, sg.smem, c->stream, sp);
-            piece_sum_kernel<<<ceil_div(R + 1, 128), 128, 0, c->stream>>>(c->partial.as<float2>(), sg.maxpieces, sg.HT, R,
+            piece_sum_kernel<<<ceil_div(R + 1, 128), 128, 0, c->stream>>>(c->partial.as<float2>(), sp.maxpieces, sg.HT, R,
                                                                      out + (size_t)f * (R + 1));
         }
         TRY(check_launch("lagstream_kernel(direct_xambg)"));
@@ -1305,8 +1284,9 @@ int check_ls_status(Ctx* c, unsigned flags, int nf = 1) {
 // of window transforms, then the Toeplitz solve, W', and AccP - AccQ conj(W') per block
 struct OnePassPlan {
     bool on = false;
-    int Bmax = 0, ntail = 0, Bt = 0, c0 = 0;
-    long long D = 0, tail_lo = 0;
+    int Bmax = 0, ntail = 0, Bt = 0;
+    long long tail_lo = 0;
+    Decimator dm{};
 };
 
 // AccP / AccQ spectra of one chunk of frames: 2 L complex64 per Doppler block and frame (8 MiB per frame at 256 blocks
@@ -1318,7 +1298,7 @@ constexpr size_t FP_ACC_CAP = 256u << 20;
 // count x L log L is below that of the two passes (lscorr_fft_kernel + caf_fft_kernel<FUSED>).  Otherwise off, and the
 // frame runs exactly as before.
 OnePassPlan onepass_plan(const LsFftPlan& lf, const CafFftPlan& cf, long long n, int filter_len, int peek, int R, int F,
-                         long long D) {
+                         const Decimator& dm) {
     OnePassPlan op;
     if (!g_frame_onepass.load() || !lf.on || !cf.on || filter_len < 1) return op;
     const int M = filter_len + peek;
@@ -1326,8 +1306,8 @@ OnePassPlan onepass_plan(const LsFftPlan& lf, const CafFftPlan& cf, long long n,
     const long long bls = L - 2ll * M + 2;                       // lags M-1 .. 2M-2 of X_ls conj(Yr')
     const long long bmax = std::min(bls, L - M - R - peek + 1);  // CAF lags peek .. R + peek of the cleaned window
     if (bmax < L / 4 || n < L) return op;
-    const long long ntaps = D + 1;
-    const int c0 = decimator_offset(ntaps, D);
+    const long long D = dm.D, ntaps = dm.ntaps;
+    const int c0 = dm.c0;
     if (c0 - (ntaps - 1) > 0) return op;                         // samples before the first block: not a layout we run
     op.tail_lo = std::min((long long)(F - 1) * D + c0 + 1, n);
     const long long tail = n - op.tail_lo;
@@ -1345,14 +1325,14 @@ OnePassPlan onepass_plan(const LsFftPlan& lf, const CafFftPlan& cf, long long n,
     if (one_cost >= two_cost) return op;
     op.on = true;
     op.Bmax = (int)bmax;
-    op.c0 = c0;
-    op.D = D;
+    op.dm = dm;
     return op;
 }
 
 int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len,
                   int peek, double reg, int R, int F, const float* win32, float2* maps, float2* taps_out, float2* cleaned_out) {
     if (n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
+    if (op.dm.ntaps > (1ll << 30)) return fail(PRC_E_INVALID, "decimator too long");   // as fast_xambg refuses it
     constexpr int R3 = fftc::FP_R3;
     constexpr int L = 256 * R3;
     const int M = filter_len + peek;
@@ -1378,7 +1358,7 @@ int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2
         fftc::FramePassParams p{};
         p.ref = r; p.srv = s; p.frame_stride = bt.stride; p.win = win32;
         p.n = (int)n; p.M = M; p.peek = peek; p.F = F;
-        p.D = op.D; p.c0 = op.c0; p.ntaps = (int)(op.D + 1); p.Bmax = op.Bmax;
+        p.D = op.dm.D; p.c0 = op.dm.c0; p.ntaps = (int)op.dm.ntaps; p.Bmax = op.Bmax;
         p.tail_lo = (int)op.tail_lo; p.ntail = op.ntail; p.Bt = op.Bt;
         p.acc = c->fpacc.as<float2>(); p.partial = c->partial.as<float2>(); p.HT = HT; p.tw = tw;
         {
@@ -1386,7 +1366,7 @@ int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2
             fftc::launch_frame_pass(p, ncta, nf, c->stream);
         }
         TRY(check_launch("frame_pass_kernel"));
-        TRY(levinson_launch(c, ncta, HT, M, reg, nf, f0));
+        TRY(levinson_launch(c, ncta, HT, M, reg, nf, c->lstaps.as<float2>() + (size_t)f0 * M, c->status.as<int>() + f0));
         TRY(taps_spectrum(c, R3, M, nf, &c->wp_caf, f0));
         if (cleaned_out) TRY(fir_fft(c, R3, r, s, cleaned_out + (size_t)f0 * bt.stride, n, b, M, peek, false, f0));
         fftc::CafCombineParams q{};
@@ -1400,41 +1380,55 @@ int frame_onepass(Ctx* c, const OnePassPlan& op, const float2* ref, const float2
             fftc::launch_caf_combine(q, gc, nf, c->stream);
         }
         TRY(check_launch("caf_combine_kernel"));
-        TRY(xambg_device(c, r, s, n, R, F, win32, nullptr, 0, maps + (size_t)f0 * F * (R + 1), b, nullptr, 0, 0, true));
+        TRY(doppler_stage(c, BlockSums{c->fftP.as<float2>(), 1, HTc, (int)op.dm.ntaps, 0}, R, F, nf, maps + (size_t)f0 * F * (R + 1)));
     }
     if (taps_out)
         CU(cudaMemcpyAsync(taps_out, c->lstaps.p, (size_t)bt.nf * M * sizeof(float2), cudaMemcpyDeviceToDevice, c->stream));
     return PRC_OK;
 }
 
-// one frame (or, on the FFT-domain path, a batch of frames) of  LS_Filter -> fast_xambg  on device pointers
-int frame_device(Ctx* c, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len, int peek, double reg,
-                 int R, int F, const float* win32, float2* maps, float2* taps_out, float2* cleaned_out) {
+// The paths of one call of the frame: FFT-domain LS and CAF (the latter with the clutter filter fused), and the one-pass
+// frame that replaces the two.  fft(): the batched FFT-domain frame runs; otherwise the direct-form kernels, frame by
+// frame.
+struct FramePlan {
+    LsFftPlan ls;
+    CafFftPlan caf;
+    OnePassPlan one;
+    bool fft() const { return ls.on && caf.on; }
+};
+
+FramePlan frame_plan(Ctx* c, long long n, int nf, int filter_len, int peek, int R, int F) {
     const int M = filter_len + peek;
-    const long long D = n / F;
-    const LsFftPlan lf = (M >= 1 && M <= 2048) ? ls_fft_plan(c, n, M, bt.nf) : LsFftPlan{};
-    const CafFftPlan cf = (D >= 2) ? caf_fft_plan(n, R, F, D + 1, D, true, M) : CafFftPlan{};
-    const OnePassPlan op = onepass_plan(lf, cf, n, filter_len, peek, R, F, D);
-    if (op.on)
-        return frame_onepass(c, op, ref, srv, n, bt, filter_len, peek, reg, R, F, win32, maps, taps_out, cleaned_out);
-    if (lf.on && cf.on) {
+    const Decimator dm = decimator(n, F, nullptr, 0);
+    FramePlan fp;
+    fp.ls = ls_fft_plan(c, n, M, nf);
+    fp.caf = caf_fft_plan(n, R, F, dm, M);
+    fp.one = onepass_plan(fp.ls, fp.caf, n, filter_len, peek, R, F, dm);
+    return fp;
+}
+
+// one frame (or, on the FFT-domain path, a batch of frames) of  LS_Filter -> fast_xambg  on device pointers
+int frame_device(Ctx* c, const FramePlan& fp, const float2* ref, const float2* srv, long long n, Batch bt, int filter_len,
+                 int peek, double reg, int R, int F, const float* win32, float2* maps, float2* taps_out, float2* cleaned_out) {
+    const int M = filter_len + peek;
+    if (fp.one.on)
+        return frame_onepass(c, fp.one, ref, srv, n, bt, filter_len, peek, reg, R, F, win32, maps, taps_out, cleaned_out);
+    if (fp.fft()) {
         // FFT-domain frame: lag sums -> Toeplitz solve -> taps spectrum -> CAF with the clutter filter applied to the
         // surveillance spectrum inside the kernel (the cleaned channel exists only if the caller asks for it)
-        TRY(ls_device(c, ref, srv, n, filter_len, peek, reg, cleaned_out, taps_out, false, bt, cleaned_out != nullptr));
-        TRY(taps_spectrum(c, cf.r3, M, bt.nf, &c->wp_caf));
+        TRY(ls_device(c, ref, srv, n, filter_len, peek, reg, cleaned_out, taps_out, false, bt));
+        TRY(taps_spectrum(c, fp.caf.r3, M, bt.nf, &c->wp_caf));
         return xambg_device(c, ref, srv, n, R, F, win32, nullptr, 0, maps, bt, c->wp_caf.as<float2>(), M, peek);
     }
-    // FP32 direct-form kernels, frame by frame
+    // FP32 direct-form kernels, frame by frame; frame fr reports its Toeplitz-solve status in status[fr]
     TRY(c->clean.ensure((size_t)n * sizeof(float2)));
     TRY(c->status.ensure((size_t)bt.nf * sizeof(int)));
     for (int fr = 0; fr < bt.nf; ++fr) {
         const float2* r = ref + (size_t)fr * bt.stride;
         const float2* sv = srv + (size_t)fr * bt.stride;
         float2* dclean = cleaned_out ? cleaned_out + (size_t)fr * bt.stride : c->clean.as<float2>();
-        c->status_slot = fr;            // frame fr reports its Toeplitz-solve status in status[fr]
-        const int rc = ls_device(c, r, sv, n, filter_len, peek, reg, dclean, taps_out ? taps_out + (size_t)fr * M : nullptr);
-        c->status_slot = 0;
-        TRY(rc);
+        TRY(ls_device(c, r, sv, n, filter_len, peek, reg, dclean, taps_out ? taps_out + (size_t)fr * M : nullptr, false,
+                      Batch{}, fr));
         TRY(xambg_device(c, r, dclean, n, R, F, win32, nullptr, 0, maps + (size_t)fr * F * (R + 1)));
     }
     return PRC_OK;
@@ -1814,9 +1808,7 @@ int xambg_entry(Ctx* c, const prc_c64* ref, const prc_c64* srv, long long n, Bat
     if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     const float* win32;
     TRY(stage_window(c, window, n, mem_kind, flags, &win32));
-    const long long D = n / freq_bins;
-    const bool batched = D >= 2 && caf_fft_plan(n, range_bins, freq_bins, D + 1, D, true, 0).on;
-    if (batched || bt.nf == 1) {
+    if (caf_fft_plan(n, range_bins, freq_bins, decimator(n, freq_bins, taps32, ndtaps), 0).on || bt.nf == 1) {
         TRY(xambg_device(c, dref, dsrv, n, range_bins, freq_bins, win32, taps32, ndtaps, dout, bt));
     } else {
         for (int fr = 0; fr < bt.nf; ++fr)       // direct-form kernels, frame by frame
@@ -2134,9 +2126,9 @@ int prc_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframe
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
     const int M = filter_len + peek;
+    const FramePlan fp = frame_plan(c, n, nframes, filter_len, peek, range_bins, freq_bins);
     // host taps are read from c->lstaps after the call, which holds every frame's taps on the FFT-domain path only
-    if (mem_kind == PRC_MEM_HOST && taps_out && nframes > 1 &&
-        !(ls_fft_plan(c, n, M, nframes).on && caf_fft_plan(n, range_bins, freq_bins, n / freq_bins + 1, n / freq_bins, true, M).on))
+    if (mem_kind == PRC_MEM_HOST && taps_out && nframes > 1 && !fp.fft())
         return fail(PRC_E_INVALID, "taps_out with host pointers and nframes > 1 needs the FFT-domain path");
     const size_t nb = (size_t)n * sizeof(float2), sb = (size_t)bt.stride * sizeof(float2);
     const size_t ob = (size_t)freq_bins * (range_bins + 1) * sizeof(float2);
@@ -2151,7 +2143,7 @@ int prc_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframe
     if (mem_kind == PRC_MEM_HOST) bt.stride = n;      // staged frames are packed
     const float* win32;
     TRY(stage_window(c, window, n, mem_kind, flags, &win32));
-    TRY(frame_device(c, dref, dsrv, n, bt, filter_len, peek, (double)reg, range_bins, freq_bins, win32, dmap, dtaps, dclean));
+    TRY(frame_device(c, fp, dref, dsrv, n, bt, filter_len, peek, (double)reg, range_bins, freq_bins, win32, dmap, dtaps, dclean));
     TRY(unstage(c, out_maps, dmap, mem_kind, 1, ob * nframes, ob * nframes, flags));
     TRY(unstage(c, taps_out, c->lstaps.p, mem_kind, 1, tb, tb, flags));
     TRY(unstage(c, cleaned_out, dclean, mem_kind, nframes, nb, sb, flags));

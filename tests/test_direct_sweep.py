@@ -1,15 +1,15 @@
 """Sweeps of the FP32 direct-form hot path across the edges of the host planners that shape it, against float64 truths.
 
 The kernels: lagstream_kernel and lagcorr_kernel (the CAF's block sums and the LS lag sums), fir_apply_kernel, the
-single-CTA levinson_kernel<1> / <4> launch of ls_device, the Doppler stage (doppler_fft_pow2_kernel<8 | 2 | 1>, or
+single-CTA levinson_kernel<1> / <4> solve of ls_device, the Doppler stage (doppler_fft_pow2_kernel<8 | 2 | 1>, or
 chunk_sum_kernel + doppler_dft_kernel) and nlms_block_kernel<KT, NT>.  They are the library's default for every LS
 filter below fft_min_n samples, every tap-weighted (shortFilt=False) or short-block (D < 32) CAF, every CAF of more
 than 3072 lags, and all of NLMS.
 
 A Python twin of the planners (prcore.cu: choose_geo, choose_stream, stream_pieces / stream_first_cta, the branches
-of xambg_device, ls_device and nlms_device) states for every case which kernel runs with which tiling; the sweep is
-chosen from it so that every edge of the tiling is reached, CPU tests hold the twin's invariants and name a case per
-edge, and the GPU tests pin the twin to the library through the per-kernel launch counts of prc_profile_read.
+of xambg_device, doppler_stage, ls_device and nlms_device) states for every case which kernel runs with which
+tiling; the sweep is chosen from it so that every edge of the tiling is reached, CPU tests hold the twin's invariants
+and name a case per edge, and the GPU tests pin the twin to the library through the per-kernel launch counts of prc_profile_read.
 Criteria as in tests/test_path_sweep.py, TOL = 1e-5 rel-inf: maps over max|map|, taps over max|taps|, cleaned
 channels over max|srv|; NLMS outputs over max|truth| (taps 5e-5) and within 1e-5 + 1.2 x the reference arithmetic's
 own error (tests/test_kernel_variants.py:_nlms_bounds).  Figures go to $PRC_PARITY_DIR/parity.json under direct/."""
@@ -143,7 +143,7 @@ def blocks_per_cta(sg, blk_len):
 
 
 def doppler_branch(F, R, nf, nsm):
-    """The Doppler stage of xambg_device: "ct8" / "ct2" / "ct1" (doppler_fft_pow2_kernel<CT>) or "dft" (chunk sums
+    """doppler_stage: "ct8" / "ct2" / "ct1" (doppler_fft_pow2_kernel<CT>) or "dft" (chunk sums
     and the direct DFT, frame by frame)."""
     pow2 = F >= 2 and F & (F - 1) == 0
     if pow2 and F <= 8192:

@@ -564,9 +564,15 @@ COVERAGE = {
         (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1 .. 2048 at n = 2L and a one-sample last segment"),
         (PS + "test_frames_batch_sizes_hold_every_row_to_its_truth", "default", "one CTA per frame (nf > slots / 2)")],
     "levinson_launch: levinson_kernel<1>": [(PAR + "test_ls_matches_live_oracle", "fft", "M <= 1024, batched solve"),
-                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1, 2, 1023, 1024")],
+                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1, 2, 1023, 1024"),
+                                            (DIRECT_TEST, "direct", "single-CTA solve: ls_big, ls_small"),
+                                            (PAR + "test_ls_matches_live_oracle", "direct", "single-CTA solve"),
+        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "single-CTA solve, M = 1 .. 1024")],
     "levinson_launch: levinson_kernel<4>": [(PAR + "test_ls_many_taps_uses_the_wide_solver", "fft", "M = 1110"),
-                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1025 .. 2048 against the truth")],
+                                            (PS + "test_ls_filter_at_the_planner_edges", "default", "M = 1025 .. 2048 against the truth"),
+                                            (DIRECT_TEST, "direct", "single-CTA solve: ls_wide"),
+                                            (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", "single-CTA solve"),
+        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "single-CTA solve, M = 1025, 2048")],
     "taps_spectrum: fftc::taps_spectrum_kernel<R3>": [
         (FFT + "test_frame_fused_equals_separate_operators_at_awkward_sizes", "fft", "R3 = 4 and 8 (CAF transform)"),
         (PAR + "test_ls_matches_live_oracle", "fft", "R3 = 8 (FIR transform)"),
@@ -593,28 +599,22 @@ COVERAGE = {
         (DIRECT_TEST, "direct", "caf_small: blocks of < 64 taps and the tap-weighted decimator"),
         (KV + "test_tap_weighted_decimator_at_full_size", "direct", "40 961 taps"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "D = 1, ntaps 32 / 63, tap-weighted at G = 32, H = 512 and the nchunk loop")],
-    "xambg_device: twiddle_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "every fast_xambg")],
-    "xambg_device: doppler_fft_pow2_kernel<8>": [
+    "doppler_stage: twiddle_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "every fast_xambg")],
+    "doppler_stage: doppler_fft_pow2_kernel<8>": [
         (KV + "test_xambg_frames_batch_matches_oracle", "default", "5 frames x 38 column groups >= SM count"),
         (FFT + "test_long_range_and_long_filter_take_the_larger_transforms", "direct", "R = 1200, F = 64"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "default", "R = 1100, 3073, 5119")],
-    "xambg_device: doppler_fft_pow2_kernel<2>": [(PAR + "test_xambg_matches_live_oracle", "direct", "F <= 4096"),
+    "doppler_stage: doppler_fft_pow2_kernel<2>": [(PAR + "test_xambg_matches_live_oracle", "direct", "F <= 4096"),
                                                  (KV + "test_doppler_stage_at_large_F", "fft", "F = 4096"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 2 .. 4096")],
-    "xambg_device: doppler_fft_pow2_kernel<1>": [(KV + "test_doppler_stage_at_large_F", "fft", "F = 8192"),
+    "doppler_stage: doppler_fft_pow2_kernel<1>": [(KV + "test_doppler_stage_at_large_F", "fft", "F = 8192"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 8192")],
-    "xambg_device: chunk_sum_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
+    "doppler_stage: chunk_sum_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
                                        (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 1, 100, 200, 1500, 16384")],
-    "xambg_device: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
+    "doppler_stage: doppler_dft_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_nonpow2_F"),
                                          (KV + "test_doppler_stage_at_large_F", "fft", "F = 16384"),
         (DS + "test_caf_direct_form_at_the_planner_edges", "direct", "F = 1, 100, 200, 1500, 16384")],
-    "ls_device: levinson_kernel<1>": [(DIRECT_TEST, "direct", "ls_big, ls_small"),
-                                      (PAR + "test_ls_matches_live_oracle", "direct", ""),
-        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1 .. 1024")],
-    "ls_device: levinson_kernel<4>": [(DIRECT_TEST, "direct", "ls_wide"),
-                                      (PAR + "test_ls_many_taps_uses_the_wide_solver", "direct", ""),
-        (DS + "test_ls_direct_form_at_the_planner_edges", "default", "M = 1025, 2048")],
     "ls_device: fir_apply_kernel<TILE_I, TILE_D>": [(DIRECT_TEST, "direct", "ls_small, ls_wide, toep"),
                                                     (DIRECT_TEST, "direct", "ls_big, frame at config 2"),
         (DS + "test_ls_direct_form_at_the_planner_edges", "default", "Mpad = 10 .. 2050, circular and linear")],
@@ -693,7 +693,7 @@ def _is_gpu_test(test_id):
 
 def test_every_prcore_launch_site_has_a_covering_gpu_test():
     sites = launch_sites()
-    assert len(sites) == 41
+    assert len(sites) == 39
     missing = sorted(set(sites) - set(COVERAGE))
     stale = sorted(set(COVERAGE) - set(sites))
     assert not missing, "launch sites of prcore.cu without a covering test in COVERAGE: " + \
