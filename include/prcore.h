@@ -58,6 +58,7 @@ typedef struct prc_c64 { float re, im; } prc_c64;
 #define PRC_FLAG_CR_F64      16u   /* prc_cfar2d_frames: cr_out receives the float64 CR, not its float32 rounding */
 #define PRC_FLAG_PROD_F32    32u   /* prc_persistence_frames: float32 products float32(x) * float32(w) */
 #define PRC_FLAG_ORIENT      64u   /* prc_persistence_frames: frames are written as fliplr(P.T) */
+#define PRC_FLAG_TRACK_RESUME 128u /* tracker entry points: continue from the frame-0 records of `history` */
 
 /* ---- lifecycle / diagnostics ------------------------------------------------ */
 int         prc_version(void);
@@ -358,6 +359,13 @@ int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t fram
  *   0 <= n_tracks <= 64.
  * prc_simple_track_frames: history[s*nframes + i] = the tracker state after frame i of sequence s.
  * rows * cols <= 524288.
+ *
+ * PRC_FLAG_TRACK_RESUME (both trackers) continues sequences instead of starting them fresh.  On entry the
+ * frame-0 records of every sequence -- history[s*nframes*n_tracks + t] (multi-target) or history[s*nframes]
+ * (simple) -- hold the state to continue from, normally the last frame's records of an earlier call on the
+ * same sequence; they are uploaded first with PRC_MEM_HOST.  On return they hold the state after frame 0, as
+ * without the flag.  The simple tracker keeps the record's own range_extent / doppler_extent.  A sequence cut
+ * anywhere and continued this way gives the same bytes as one call.
  */
 typedef struct prc_kalman {
     double x[4], P[16], F1[16], F2[16], Q[16], H[8], R[4], S[4];

@@ -1547,6 +1547,14 @@ size_t trk_smem(const TrkMapParams& mp, int mode) {
     return mode == TRK_MODE_MEAN ? nv : nv + (size_t)mp.cap * (sizeof(unsigned long long) + sizeof(int));
 }
 
+// PRC_FLAG_TRACK_RESUME from host memory: the frame-0 records of every sequence (rec bytes, seq bytes apart) -> the
+// staged history the kernels continue from
+int trk_resume_h2d(Ctx* c, void* dev, const void* host, int nseq, size_t seq, size_t rec, unsigned flags) {
+    for (int s = 0; s < nseq; ++s)
+        TRY(h2d(c, static_cast<char*>(dev) + s * seq, static_cast<const char*>(host) + s * seq, rec, flags));
+    return PRC_OK;
+}
+
 int trk_meas_launch(Ctx* c, const TrkMapParams& mp, bool f64, int mode, int nf, int nseq) {
     const size_t smem = trk_smem(mp, mode);
     if (smem > SMEM_LIMIT) return fail(PRC_E_INVALID, "tracker measurement kernel needs %zu B of shared memory", smem);
@@ -2545,6 +2553,10 @@ int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq,
     const size_t hb = nfr * n_tracks * sizeof(prc_track);
     prc_track* dh;
     TRY(stage_out(history, mem_kind, hb, c->trk_out, &dh));
+    const bool resume = (flags & PRC_FLAG_TRACK_RESUME) != 0;
+    if (resume && mem_kind == PRC_MEM_HOST)
+        TRY(trk_resume_h2d(c, dh, history, nseq, (size_t)nframes * n_tracks * sizeof(prc_track),
+                           (size_t)n_tracks * sizeof(prc_track), flags));
     for (int f0 = 0; f0 < nframes; f0 += fc) {
         const int nf = std::min(fc, nframes - f0);
         mp.f0 = f0;
@@ -2558,6 +2570,7 @@ int prc_multitarget_track_frames(const void* maps, int rows, int cols, int nseq,
         tp.f1 = f0 + nf;
         tp.slots = mp.out;
         tp.fc = fc;
+        tp.resume = resume ? 1 : 0;
         {
             ProfScope ps(c, K_TRK_MULTI);
             track_multi_kernel<<<nseq, 32, 0, c->stream>>>(tp);
@@ -2586,12 +2599,17 @@ int prc_simple_track_frames(const void* maps, int rows, int cols, int nseq, int 
     const size_t hb = nfr * sizeof(prc_track_simple);
     prc_track_simple* dh;
     TRY(stage_out(history, mem_kind, hb, c->trk_out, &dh));
+    const bool resume = (flags & PRC_FLAG_TRACK_RESUME) != 0;
+    if (resume && mem_kind == PRC_MEM_HOST)
+        TRY(trk_resume_h2d(c, dh, history, nseq, (size_t)nframes * sizeof(prc_track_simple), sizeof(prc_track_simple),
+                           flags));
     TrkSimpleParams sp{};
     sp.m = mp;
     sp.hist = dh;
     sp.range_extent = range_extent;
     sp.doppler_extent = doppler_extent;
     py_slice(250, 260, rows, &sp.zlo, &sp.zhi);
+    sp.resume = resume ? 1 : 0;
     {
         ProfScope ps(c, K_TRK_SIMPLE);
         if (f64) track_simple_kernel<double><<<nseq, TRK_SIMPLE_THREADS, 0, c->stream>>>(sp);

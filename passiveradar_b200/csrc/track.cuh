@@ -486,6 +486,7 @@ struct TrkMultiParams {
     int f0, f1;                     // frames walked by this launch
     const double* slots;            // frame (s, f): slots + (s * fc + f - f0) * 3 * m.cap (range, Doppler, strength rows)
     int fc;
+    int resume;                     // PRC_FLAG_TRACK_RESUME: frame 0 continues from the records already at hist[s][0]
 };
 
 // initialize_track (target_detection.py:350-396): free at (0, 0) without a measurement, preliminary at it with one
@@ -594,7 +595,10 @@ __device__ TrkBest trk_scan(const TrkMultiParams& p, const double* slot, int M, 
     return TrkBest{cnt, br, bd};
 }
 
-// one frame of multitarget_tracker (target_detection.py:485-524) for the warp's sequence
+// one frame of multitarget_tracker (target_detection.py:485-524) for the warp's sequence.  prev and cur are the same
+// records at frame 0, where tracks of every status run in place (free ones fresh, any when resuming): a track reads
+// only its own record, every lane reads it before the __syncwarp that precedes lane 0's write, and trk_kalman reads
+// all of its input before writing its output.
 template <bool LIST>
 __device__ void trk_multi_frame(const TrkMultiParams& p, const prc_track* prev, prc_track* cur, const double* slot,
                                 int M, const void* map, double mean, double thr, TrkBox* boxes) {
@@ -709,9 +713,11 @@ __global__ void __launch_bounds__(32) track_multi_kernel(const __grid_constant__
     for (int f = p.f0; f < p.f1; ++f) {
         prc_track* cur = p.hist + s * per_seq + (size_t)f * p.n_tracks;
         const prc_track* prev = cur - p.n_tracks;
-        if (f == 0) {                                  // every track starts free
-            for (int t = lane; t < p.n_tracks; t += 32) trk_init_track(cur[t], false, 0.0, 0.0);
-            __syncwarp();
+        if (f == 0) {                                  // frame 0 runs in place: every track starts free, or resumes
+            if (!p.resume) {
+                for (int t = lane; t < p.n_tracks; t += 32) trk_init_track(cur[t], false, 0.0, 0.0);
+                __syncwarp();
+            }
             prev = cur;
         }
         const long long sidx = (long long)s * p.m.nframes + f;
@@ -735,6 +741,7 @@ struct TrkSimpleParams {
     prc_track_simple* hist;         // [nseq][nframes]
     double range_extent, doppler_extent;
     int zlo, zhi;                   // zeroed columns [250:260], clipped to the frame
+    int resume;                     // PRC_FLAG_TRACK_RESUME: frame 0 continues from the record already at hist[s][0]
 };
 
 // python slice [start:stop] of an axis of length len
@@ -757,7 +764,7 @@ __global__ void __launch_bounds__(TRK_SIMPLE_THREADS) track_simple_kernel(const 
         prc_track_simple* cur = p.hist + (size_t)s * p.m.nframes + f;
         const prc_track_simple* prev = cur - 1;
         if (tid == 0) {
-            if (f == 0) {
+            if (f == 0 && !p.resume) {
                 // simple_target_tracker's initial state (target_detection.py:634-653), built positionally against
                 // differently ordered fields: measurement = H x = (30, -20), measurement_idx = (35, -30),
                 // estimate = (50, 50)
@@ -784,8 +791,8 @@ __global__ void __launch_bounds__(TRK_SIMPLE_THREADS) track_simple_kernel(const 
                 for (int q = 0; q < 8; ++q) k.H[q] = (q == 0 || q == 6) ? 1.0 : 0.0;
                 k.R[0] = 5.0; k.R[1] = 0.0; k.R[2] = 0.0; k.R[3] = 5.0;
                 k.S[0] = 1.0; k.S[1] = 0.0; k.S[2] = 0.0; k.S[3] = 1.0;
-                prev = cur;
             }
+            if (f == 0) prev = cur;                  // frame 0 runs in place
             const double* lm = prev->lock_mode;
             const long long ly = prev->measurement_idx[0], lx = prev->measurement_idx[1];
             long long gated = 0, half_y = 0, half_x = 0;

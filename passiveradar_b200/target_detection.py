@@ -119,15 +119,34 @@ def _frames_layout(maps, name):
     return a, S, T, rows, cols, T * rows * cols, rows * cols, a.dtype == np.float64
 
 
-def _launch(fn, maps, S, T, rows, cols, ss, fs, f64, args, out_dtype, out_shape, device):
-    """Run a tracker entry point on host arrays or on a CUDA tensor (on the tensor's current stream)."""
+def _initial_state(initial_state, dtype, shape):
+    """initial_state of a *_frames tracker: None, or records of the tracker's dtype and shape (S, ...)."""
+    if initial_state is None:
+        return None
+    a = np.asarray(initial_state)
+    if a.dtype != dtype:
+        raise TypeError(f"initial_state must be an array of {dtype}, got {a.dtype}")
+    if a.shape != shape:
+        raise ValueError(f"initial_state must have shape {shape}, got {a.shape}")
+    return a
+
+
+def _launch(fn, maps, S, T, rows, cols, ss, fs, f64, args, out_dtype, out_shape, device, initial_state=None):
+    """Run a tracker entry point on host arrays or on a CUDA tensor (on the tensor's current stream).  With
+    initial_state every sequence continues from its records (PRC_FLAG_TRACK_RESUME) instead of starting fresh."""
     lib = _lib.load()
     flags = _lib.FLAG_MAP_F64 if f64 else 0
     hist = np.zeros(out_shape, dtype=out_dtype)
+    if initial_state is not None:
+        hist[:, 0] = initial_state
+        flags |= _lib.FLAG_TRACK_RESUME
     if _is_tensor(maps):
         import torch
         dev = maps.device.index if device is None else int(device)
-        hd = torch.empty(hist.nbytes, dtype=torch.uint8, device=maps.device)
+        if initial_state is not None:
+            hd = torch.from_numpy(hist.view(np.uint8).reshape(-1)).to(maps.device)
+        else:
+            hd = torch.empty(hist.nbytes, dtype=torch.uint8, device=maps.device)
         stream = torch.cuda.current_stream(maps.device).cuda_stream
         _lib.check(getattr(lib, fn)(maps.data_ptr(), rows, cols, S, T, ss, fs, *args, hd.data_ptr(),
                                     _lib.MEM_DEVICE, dev, stream, flags))
@@ -199,19 +218,22 @@ def multitarget_tracker(data, frame_extent, N_TRACKS, *, device=None):
     return multitarget_tracker_frames(_frames_last(a, "data"), frame_extent, n_tracks, device=device)[0]
 
 
-def multitarget_tracker_frames(maps, frame_extent, n_tracks, *, device=None):
+def multitarget_tracker_frames(maps, frame_extent, n_tracks, *, initial_state=None, device=None):
     '''multitarget_tracker on S independent sequences in one call.  maps: (S, T, rows, cols) numpy array or CUDA
     tensor (float32 / float64; a tensor's sequences may be strided).  Returns an (S, T, n_tracks) target_track_dtype
-    array.'''
+    array.  initial_state: an (S, n_tracks) target_track_dtype array -- normally history[:, -1] of an earlier call --
+    that each sequence continues from instead of starting with every track free; cutting a sequence anywhere and
+    continuing it this way gives the same records as one call.'''
     dext, rext = _extent(frame_extent)
     n_tracks = int(n_tracks)
     if n_tracks < 0:
         raise ValueError("n_tracks must be >= 0")
     m, S, T, rows, cols, ss, fs, f64 = _frames_layout(maps, "maps")
+    init = _initial_state(initial_state, target_track_dtype, (S, n_tracks))
     if n_tracks == 0 or S == 0 or T == 0:
         return np.zeros((S, T, n_tracks), dtype=target_track_dtype)
     return _launch("prc_multitarget_track_frames", m, S, T, rows, cols, ss, fs, f64, (dext, rext, n_tracks),
-                   target_track_dtype, (S, T, n_tracks), device)
+                   target_track_dtype, (S, T, n_tracks), device, init)
 
 
 def simple_target_tracker(data, rangeExtent, dopplerExtent, *, device=None):
@@ -233,15 +255,18 @@ def simple_target_tracker(data, rangeExtent, dopplerExtent, *, device=None):
     return simple_tracker_frames(_frames_last(a, "data"), rangeExtent, dopplerExtent, device=device)[0]
 
 
-def simple_tracker_frames(maps, range_extent, doppler_extent, *, device=None):
+def simple_tracker_frames(maps, range_extent, doppler_extent, *, initial_state=None, device=None):
     '''simple_target_tracker on S independent sequences in one call.  maps: (S, T, rows, cols) numpy array or CUDA
-    tensor.  Returns an (S, T) target_track_dtype_simple array.'''
+    tensor.  Returns an (S, T) target_track_dtype_simple array.  initial_state: an (S,) target_track_dtype_simple
+    array -- normally history[:, -1] of an earlier call -- that each sequence continues from instead of the
+    tracker's initial record; the record's own range_extent / doppler_extent stay in use.'''
     rext, dext = float(range_extent), float(doppler_extent)
     m, S, T, rows, cols, ss, fs, f64 = _frames_layout(maps, "maps")
+    init = _initial_state(initial_state, target_track_dtype_simple, (S,))
     if S == 0 or T == 0:
         return np.zeros((S, T), dtype=target_track_dtype_simple)
     return _launch("prc_simple_track_frames", m, S, T, rows, cols, ss, fs, f64, (rext, dext),
-                   target_track_dtype_simple, (S, T), device)
+                   target_track_dtype_simple, (S, T), device, init)
 
 
 def cfar_track(maps_d, fw, gw, frame_extent, n_tracks, *, device=None):
@@ -268,3 +293,201 @@ def cfar_track(maps_d, fw, gw, frame_extent, n_tracks, *, device=None):
                                       _lib.MEM_DEVICE, dev, stream, _lib.FLAG_ABS_C64 | _lib.FLAG_ASYNC))
     return _launch("prc_multitarget_track_frames", cf, 1, T, F, R1, T * F * R1, F * R1, False,
                    (dext, rext, n_tracks), target_track_dtype, (1, T, n_tracks), dev)[0]
+
+
+# ---------------------------------------------------------------------------------------------- tracker scripts' chain
+_MULTI_WORDS = target_track_dtype.itemsize // 8           # a record as 8-byte words: status is word 0, estimate 4-5
+_SIMPLE_WORDS = target_track_dtype_simple.itemsize // 8   # lock_mode is words 0-3, estimate 8-9
+
+
+class TrackerPipeline:
+    """The chain of the reference's tracker scripts (multitarget_kalman_tracker.py / simple_kalman_tracker.py) on the
+    device, for a stream of maps:
+
+        CF[:, :, i] = CFAR_2D(|xambg[:, :, i]|, fw, gw)                     (float64 stack, one launch per batch)
+        history = multitarget_tracker(CF, [max_doppler, max_range], n_tracks)  or
+                  simple_target_tracker(CF, max_range, max_doppler)
+        the scripts' masks of the estimates, and with render=True
+        data = fliplr(persistence(CF, kk, hold, decay).T), [percentile(data, 35), 1.5 * percentile(data, 99)]
+
+    The trackers read the float64 CF itself, as the scripts do.  ``run_device`` carries the last tracker records
+    (continued with PRC_FLAG_TRACK_RESUME) and the last hold - 1 CF frames to the next call, so a stack cut into
+    batches of any size, one map per call included, gives the same bytes as one call; ``reset()`` starts a new
+    sequence.  ``run`` takes the scripts' host layout (F, R+1, nframes).  Plotting stays with the caller."""
+
+    def __init__(self, max_range, max_doppler, *, tracker="multi", n_tracks=10, fw=18, gw=4, hold=20, decay=0.90,
+                 render=True, batch=64, device=None):
+        from .plotting_tools import _decay_plan
+        if tracker not in ("multi", "simple"):
+            raise ValueError(f"tracker must be 'multi' or 'simple', got {tracker!r}")
+        self.tracker = tracker
+        self.max_range, self.max_doppler = float(max_range), float(max_doppler)
+        self.n_tracks = int(n_tracks) if tracker == "multi" else 1
+        if not 0 <= self.n_tracks <= MAX_TRACKS:
+            raise ValueError(f"n_tracks={n_tracks} outside [0, {MAX_TRACKS}]")
+        self.fw, self.gw, self.hold, self.decay = int(fw), int(gw), int(hold), decay
+        if not (1 <= self.fw <= 64) or self.gw < 0 or self.fw * self.fw == self.gw * self.gw:
+            raise ValueError(f"fw={fw} gw={gw}: CFAR_2D needs 1 <= fw <= 64, gw >= 0 and fw != gw")
+        if self.hold < 1:
+            raise ValueError("hold must be >= 1")
+        if int(batch) < 1:
+            raise ValueError("batch must be >= 1")
+        self.render, self.batch, self.device = bool(render), int(batch), device
+        # CF is float64 in the scripts (np.zeros(xambg.shape)): the products are float64 whatever decay's type
+        self.weights, _ = _decay_plan(np.float64, decay, self.hold)
+        self.dtype = target_track_dtype if tracker == "multi" else target_track_dtype_simple
+        self.reset()
+
+    @classmethod
+    def from_config(cls, config, tracker="multi", **kw):
+        """From the dict ``passiveRadar.config.getConfiguration`` returns: its max_range_actual and
+        max_doppler_actual are the extents the scripts pass their tracker."""
+        missing = [k for k in ("max_range_actual", "max_doppler_actual") if k not in config]
+        if missing:
+            raise ValueError(f"config lacks {missing} (getConfiguration derives them)")
+        return cls(config["max_range_actual"], config["max_doppler_actual"], tracker=tracker, **kw)
+
+    def reset(self):
+        """Start a new sequence: the next map is frame 0 of the tracker and of the persistence."""
+        self._shape = None
+        self._state = None          # the last frame's tracker records (uint8 device tensor)
+        self._carry = None          # the last hold - 1 CF frames
+
+    def records(self, history, T=None):
+        """The ``history`` bytes of ``run_device`` (T maps) as the tracker's NumPy records: (T, n_tracks)
+        target_track_dtype for the multi-target tracker, (T,) target_track_dtype_simple for the simple one.  T may be
+        left out unless n_tracks is 0."""
+        raw = history.cpu().numpy() if _is_tensor(history) else np.asarray(history, dtype=np.uint8)
+        a = np.frombuffer(raw.tobytes(), dtype=self.dtype).copy()
+        return a.reshape(-1 if T is None else T, self.n_tracks) if self.tracker == "multi" else a
+
+    def run_device(self, maps_d):
+        """maps_d: (T, F, R+1) complex64 or float32 CUDA tensor (``RecordingPipeline.run_device`` output); either way
+        its magnitude is tracked, as the scripts track np.abs(xambg).  Returns a dict of device tensors, ordered on
+        the current torch stream:
+
+        * ``cf``: the (T, F, R+1) float64 CFAR_2D maps the tracker and the phosphor frames read;
+        * ``history``: the tracker records as raw bytes (``records()`` turns them into NumPy records);
+        * multi-target tracker: ``track_range``, ``track_doppler`` (T, n_tracks) float64 estimates, NaN where the
+          track is not confirmed (status != 2);
+        * simple tracker: ``estimate_locked``, ``estimate_unlocked`` (T, 2) estimates, NaN in the rows where
+          lock_mode[:, 0] is set / not set;
+        * with render=True: ``data`` (T, R+1, F) float64 and ``limits`` (T, 2) = [vmin, vmax], as
+          ``RenderPipeline.run_device`` gives them."""
+        import torch
+        from .plotting_tools import MAX_CFAR_FRAMES, PERCENTILES, VMAX_SCALE, _stream_arg
+        if not (_is_tensor(maps_d) and maps_d.is_cuda and maps_d.dim() == 3):
+            raise TypeError("maps_d must be a (T, F, R+1) CUDA tensor")
+        if maps_d.dtype not in (torch.complex64, torch.float32):
+            raise TypeError(f"maps_d must be complex64 or float32, got {maps_d.dtype}")
+        T, F, R1 = maps_d.shape
+        if self._shape is not None and self._shape != (F, R1):
+            raise ValueError(f"maps of shape {(F, R1)} continue a sequence of {self._shape} maps; call reset() first")
+        if F * R1 > 1 << 19:
+            raise ValueError(f"a {F} x {R1} map exceeds the trackers' maximum of {1 << 19} cells")
+        tdev = maps_d.device
+        dev = tdev.index if self.device is None else int(self.device)
+        N, rec = self.n_tracks, self.dtype.itemsize * self.n_tracks
+        out = {"history": torch.empty(T * rec, dtype=torch.uint8, device=tdev)}
+        if T == 0:
+            out["cf"] = torch.empty((0, F, R1), dtype=torch.float64, device=tdev)
+            if self.render:
+                out["data"] = torch.empty((0, R1, F), dtype=torch.float64, device=tdev)
+                out["limits"] = torch.empty((0, 2), dtype=torch.float64, device=tdev)
+            return self._masks(out, 0, torch)
+        lib = _lib.load()
+        # the scripts take np.abs of the stack before CFAR_2D, and the CFAR kernel keeps the sign of a real cell in its
+        # numerator: a float32 map is made |map| first (exact, and a no-op on magnitudes)
+        maps_d = (maps_d.abs() if maps_d.dtype == torch.float32 else maps_d).contiguous()
+        stream = _stream_arg(torch, tdev)
+        nc = 0 if self._carry is None else self._carry.shape[0]
+        cells = F * R1
+        cf = torch.empty((nc + T, F, R1), dtype=torch.float64, device=tdev)
+        if nc:
+            cf[:nc] = self._carry
+        flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if maps_d.dtype == torch.complex64 else 0)
+        for t0 in range(0, T, MAX_CFAR_FRAMES):
+            nb = min(MAX_CFAR_FRAMES, T - t0)
+            _lib.check(lib.prc_cfar2d_frames(maps_d[t0].data_ptr(), F, R1, nb, cells, self.fw, self.gw,
+                                             cf[nc + t0].data_ptr(), cells, _lib.MEM_DEVICE, dev, stream, flags))
+        hist = out["history"]
+        flags = _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64
+        if self._state is not None:
+            hist[:rec] = self._state
+            flags |= _lib.FLAG_TRACK_RESUME
+        if self.tracker == "multi":
+            if N:
+                _lib.check(lib.prc_multitarget_track_frames(cf[nc].data_ptr(), F, R1, 1, T, T * cells, cells,
+                                                            self.max_doppler, self.max_range, N, hist.data_ptr(),
+                                                            _lib.MEM_DEVICE, dev, stream, flags))
+        else:
+            _lib.check(lib.prc_simple_track_frames(cf[nc].data_ptr(), F, R1, 1, T, T * cells, cells, self.max_range,
+                                                   self.max_doppler, hist.data_ptr(), _lib.MEM_DEVICE, dev, stream,
+                                                   flags))
+        if self.render:
+            data = torch.empty((T, R1, F), dtype=torch.float64, device=tdev)
+            limits = torch.empty((T, 2), dtype=torch.float64, device=tdev)
+            q = np.array(PERCENTILES, dtype=np.float64)
+            scale = np.array([1.0, VMAX_SCALE], dtype=np.float64)
+            _lib.check(lib.prc_persistence_frames(cf.data_ptr(), F, R1, T, cells, nc, self.hold,
+                                                  self.weights.ctypes.data, data.data_ptr(), _lib.MEM_DEVICE, dev,
+                                                  stream, _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64 | _lib.FLAG_ORIENT))
+            _lib.check(lib.prc_percentiles_frames(data.data_ptr(), cells, T, cells, q.ctypes.data, scale.ctypes.data,
+                                                  2, limits.data_ptr(), _lib.MEM_DEVICE, dev, stream, _lib.FLAG_ASYNC))
+            out["data"], out["limits"] = data, limits
+            keep = min(nc + T, self.hold - 1)
+            self._carry = cf[nc + T - keep:].clone() if keep else None
+        self._shape = (F, R1)
+        self._state = hist[(T - 1) * rec:].clone() if rec else None
+        out["cf"] = cf[nc:]
+        return self._masks(out, T, torch)
+
+    def _masks(self, out, T, torch):
+        """The scripts' masks of the estimates, from the history bytes."""
+        hist = out["history"]
+        dev = hist.device
+        nan = torch.tensor(float("nan"), dtype=torch.float64, device=dev)
+        if self.tracker == "multi":
+            # multitarget_kalman_tracker.py:66-75: estimate[..., 0] / [..., 1], NaN where status != 2
+            w = hist.view(torch.float64).view(T, self.n_tracks, _MULTI_WORDS)
+            unconfirmed = hist.view(torch.int64).view(T, self.n_tracks, _MULTI_WORDS)[:, :, 0] != 2
+            out["track_range"] = torch.where(unconfirmed, nan, w[:, :, 4])
+            out["track_doppler"] = torch.where(unconfirmed, nan, w[:, :, 5])
+        else:
+            # simple_kalman_tracker.py:63-73: unlocked = lock_mode[:, 0].astype(bool)
+            w = hist.view(torch.float64).view(T, _SIMPLE_WORDS)
+            unlocked = (w[:, 0] != 0)[:, None]
+            out["estimate_locked"] = torch.where(unlocked, nan, w[:, 8:10])
+            out["estimate_unlocked"] = torch.where(~unlocked, nan, w[:, 8:10])
+        return out
+
+    def run(self, xambg):
+        """xambg: the scripts' (F, R+1, nframes) maps on the host, complex64 or already np.abs-ed float32 / float64
+        (CFAR_2D reads float32, as the drop-in does).  Starts a new sequence and streams it through in batches.
+        Returns host arrays: ``history`` exactly as multitarget_tracker / simple_target_tracker return it, the masked
+        estimates and, with render=True, ``data`` (nframes, R+1, F) and ``limits`` (nframes, 2)."""
+        import torch
+        xambg = np.asarray(xambg)
+        if xambg.ndim != 3:
+            raise ValueError(f"xambg must be (F, R+1, nframes), got {xambg.ndim} dimensions")
+        if xambg.dtype.kind == "c":
+            dt = np.complex64
+        elif xambg.dtype.kind in "biuf":
+            dt = np.float32
+        else:
+            raise TypeError(f"unsupported map dtype {xambg.dtype}")
+        N = xambg.shape[2]
+        dev = _lib.current_device() if self.device is None else int(self.device)
+        tdev = torch.device("cuda", dev)
+        self.reset()
+        parts = []
+        with torch.cuda.device(tdev):
+            for b0 in range(0, max(N, 1), self.batch):      # an empty stack still gives empty outputs
+                b1 = min(N, b0 + self.batch)
+                maps = torch.from_numpy(np.ascontiguousarray(np.moveaxis(xambg[:, :, b0:b1], 2, 0), dtype=dt))
+                got = self.run_device(maps.to(tdev))
+                del got["cf"]
+                parts.append({k: v.cpu().numpy() for k, v in got.items()})
+        res = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
+        res["history"] = self.records(res["history"], N)
+        return res
