@@ -453,6 +453,39 @@ int prc_psd_frames(const void* x, int dtype, int64_t n, int nframes, int64_t fra
                    int pad_to, const double* window, double scale, int onesided, double* out, int64_t out_stride,
                    int device, void* stream, unsigned flags);
 
+/* ---- FIR decimation and normalisation ---------------------------------------------------------------
+ * prc_decimate_rows replaces decimate(x, q) = scipy.signal.decimate(x, q, 20*q, ftype='fir', axis=0) (reference
+ * passiveRadar/signal_utils.py:11-13) on nrows rows of n samples, row b at x + b * row_stride elements:
+ *   y[m] = sum_{j=0}^{20q} taps[j] * x[m*q + 10q - j],  x = 0 outside [0, n),  m = 0 .. ceil(n/q) - 1,
+ * written to out + b * out_stride elements.  taps: 20q + 1 host doubles (firwin(20q+1, 1/q, window='hamming'), rounded
+ * to float32 by the caller for float32 / complex64 data, as decimate does); they are copied before the call returns.
+ * src is a PRC_DT_* code, or PRC_DEC_RAW + PRC_IQ_C64 / PRC_IQ_I8 / PRC_IQ_I16 for raw interleaved I/Q (float32, int8,
+ * int16; I and Q read as scalars) that is deinterleaved and mixed on load with mode, fc, fs and phase_offset exactly as
+ * prc_iq_mix_c64 does (channel_preprocessing, signal_utils.py:80-85: the tuned signal is never stored).  For raw I/Q,
+ * n and row_stride count complex samples.  Arithmetic and out's dtype:
+ *   PRC_DT_F32                              float32 taps and sums, float32 out
+ *   PRC_DT_C64, raw with PRC_MIX_NONE/C64   float32 taps and sums, complex64 out
+ *   PRC_DT_I8, U8, I16, F64                 float64, float64 out
+ *   PRC_DT_C128, raw with the other modes   float64 (raw: the complex64 mixed sample widened), complex128 out
+ * A row's result does not depend on nrows or on its place in the batch: row b is bit-identical to a one-row call on it.
+ * Limits (PRC_E_INVALID, naming the limit): 2 <= q <= 65536; n >= 1; nrows >= 1; row_stride >= n and out_stride >=
+ * ceil(n/q) when nrows > 1; x, taps, out not NULL.
+ *
+ * prc_normalize replaces normalize(x) = x / mean(|x|) (signal_utils.py:7-9) on n contiguous elements of dtype: the
+ * mean of |x| is summed in float64 in a fixed order (no atomics), and out receives NumPy's result dtype: float32 for
+ * PRC_DT_F32, complex64 for PRC_DT_C64 (x times float32(1 / float32(mean))), complex128 for PRC_DT_C128, float64 for
+ * the rest.  |x| of int8 and int16 wraps at -128 and -32768 as NumPy's abs does.  An all-zero x gives NaN.
+ * Limits (PRC_E_INVALID): n >= 1; x, out not NULL.
+ *
+ * x and out of both are DEVICE pointers (no mem_kind; callers stage host arrays themselves).  Scratch memory is
+ * allocated stream-ordered on the call's stream and released before the call returns it.
+ */
+#define PRC_DEC_RAW 16
+int prc_decimate_rows(const void* x, int src, int64_t n, int nrows, int64_t row_stride, int mode, double fc, double fs,
+                      double phase_offset, const double* taps, int q, void* out, int64_t out_stride, int device,
+                      void* stream, unsigned flags);
+int prc_normalize(const void* x, int dtype, int64_t n, void* out, int device, void* stream, unsigned flags);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,7 +14,8 @@ from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # n
                               LS_Filter_Toeplitz, LS_Filter_Multiple, GAL_JPE, gal_jpe_frames,
                               LS_Filter_SVD, ls_filter_svd_frames)
 from .signal_utils import (deinterleave_IQ, frequency_shift, resample, frontend,            # noqa: F401
-                           find_channel_offset, offset_compensation, shift, xcorr)
+                           find_channel_offset, offset_compensation, shift, xcorr, decimate,
+                           channel_preprocessing, normalize)
 from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
                                multitarget_tracker_frames, simple_tracker_frames, cfar_track, TrackerPipeline,
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
@@ -24,7 +25,8 @@ from .spectrum import psd, psd_frames, SignalPreview                         # n
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
            "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
-           "find_channel_offset", "offset_compensation", "shift", "xcorr", "CFAR_2D",
+           "find_channel_offset", "offset_compensation", "shift", "xcorr", "decimate", "channel_preprocessing",
+           "normalize", "CFAR_2D",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
            "simple_tracker_frames", "cfar_track", "TrackerPipeline", "RecordingPipeline", "persistence", "persistence_frames",
            "RenderPipeline", "psd", "psd_frames", "SignalPreview"]
@@ -49,7 +51,8 @@ def install(reference_package: str = "passiveRadar"):
         "range_doppler_processing": {"fast_xambg": fast_xambg, "direct_xambg": direct_xambg},
         # xcorr stays the reference's: only its LS_Filter_Toeplitz and direct_xambg call it, and both are replaced
         "signal_utils": {"deinterleave_IQ": deinterleave_IQ, "frequency_shift": frequency_shift, "resample": resample,
-                         "find_channel_offset": find_channel_offset, "offset_compensation": offset_compensation},
+                         "find_channel_offset": find_channel_offset, "offset_compensation": offset_compensation,
+                         "decimate": decimate, "channel_preprocessing": channel_preprocessing, "normalize": normalize},
         "target_detection": {"CFAR_2D": CFAR_2D, "get_measurements": get_measurements,
                              "multitarget_tracker": multitarget_tracker, "simple_target_tracker": simple_target_tracker},
         "clutter_removal": {"LS_Filter": LS_Filter, "NLMS_filter": NLMS_filter,

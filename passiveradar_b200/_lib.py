@@ -34,6 +34,7 @@ FLAG_TRACK_RESUME = 128
 IQ_C64, IQ_I8, IQ_I16 = 0, 1, 2
 MIX_NONE, MIX_C64, MIX_C128, MIX_F64, MIX_FS64 = 0, 1, 2, 3, 4
 DT_I8, DT_U8, DT_I16, DT_F32, DT_F64, DT_C64, DT_C128 = 0, 1, 2, 3, 4, 5, 6
+DEC_RAW = 16
 
 # every symbol include/prcore.h declares: name -> (restype, argtypes)
 _c64p = C.c_void_p
@@ -117,6 +118,10 @@ SIGNATURES = {
     "prc_psd_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int,
                                  C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
                                  C.c_uint]),
+    "prc_decimate_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_double, C.c_double,
+                                    C.c_double, C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                    C.c_uint]),
+    "prc_normalize": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_uint]),
 }
 
 

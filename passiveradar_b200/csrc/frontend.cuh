@@ -26,6 +26,20 @@ struct MixParams {
     double B64, rFs64;   // MIX_F64 / MIX_FS64: the same in float64 (fc or Fs was a NumPy float64 scalar)
 };
 
+// complex sample i of raw interleaved I/Q, read as scalars (the recording chain's chunks and decimate.cuh's slabs)
+__device__ __forceinline__ float2 iq_load_scalar(const void* in, int kind, long long i) {
+    if (kind == IQ_I8) {
+        const signed char* x = static_cast<const signed char*>(in);
+        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
+    }
+    if (kind == IQ_I16) {
+        const short* x = static_cast<const short*>(in);
+        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
+    }
+    const float* x = static_cast<const float*>(in);
+    return make_float2(x[2 * i], x[2 * i + 1]);
+}
+
 // x[i] * exp(1j * theta_i) with numpy's evaluation order:
 //   theta32 = fl32(fl32(B * fl32(i)) * fl32(1/Fs))                                  (complex64 arange, weak python scalars)
 //   MIX_C64 : theta = fl32(theta32 + fl32(po)), exp and product in float32     (phase_offset a python scalar)

@@ -35,6 +35,7 @@
 #include "recording.cuh"
 #include "render.cuh"
 #include "spectrum.cuh"
+#include "decimate.cuh"
 
 namespace {
 
@@ -54,13 +55,14 @@ std::atomic<uint64_t> g_launches{0};
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
                 K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_CFAR_FRAMES, K_PERSISTENCE,
-                K_PERCENTILE, K_PSD_SEGMENTS, K_PSD_FINISH, K_COUNT };
+                K_PERCENTILE, K_PSD_SEGMENTS, K_PSD_FINISH, K_DECIMATE, K_NORM_SUM, K_NORM_SCALE, K_COUNT };
 const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply", "lagcorr_caf",
                                            "doppler_fft", "nlms", "misc", "gal_jpe", "track_meas",
                                            "track_multi", "track_simple", "chanoff_load", "chanoff_iir",
                                            "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
                                            "caf_combine", "frontend_chunks", "cfar_frames",
-                                           "persistence", "percentile", "psd_segments", "psd_finish"};
+                                           "persistence", "percentile", "psd_segments", "psd_finish",
+                                           "decimate", "norm_sum", "norm_scale"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -248,6 +250,7 @@ int set_kernel_attrs(int device) {
 #undef PRC_FFT_ATTRS
     CU(fftc::framepass_set_attrs(lim));
     CU(spec::set_attrs(lim));
+    CU(dec::set_attrs(lim));
     g_attrs_set[device].store(true);
     return PRC_OK;
 }
@@ -1901,6 +1904,56 @@ int psd_device(Ctx* c, const void* x, int dt, long long n, int nframes, long lon
     return PRC_OK;
 }
 
+// ---- FIR decimator and normalize (decimate.cuh) ------------------------------------------------------------------
+// nrows rows of n samples -> ceil(n / q) outputs each: the taps to the device in the accumulator's precision, then one
+// launch per 65535 rows (grid.y); a row's result does not depend on which launch it is in.
+int decimate_device(Ctx* c, dec::DecParams p, int acc, int nrows, const double* taps) {
+    using namespace dec;
+    const size_t nt = (size_t)20 * p.q + 1;
+    AsyncScratch ws(c->stream);
+    if (acc == 0 || acc == 1) {
+        std::vector<float> t32(nt);
+        for (size_t j = 0; j < nt; ++j) t32[j] = (float)taps[j];
+        float* d;
+        TRY(ws.get(&d, nt * sizeof(float)));
+        CU(cudaMemcpyAsync(d, t32.data(), nt * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        p.taps = d;
+    } else {
+        double* d;
+        TRY(ws.get(&d, nt * sizeof(double)));
+        CU(cudaMemcpyAsync(d, taps, nt * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+        p.taps = d;
+    }
+    for (int r0 = 0; r0 < nrows; r0 += 65535) {
+        {
+            ProfScope ps(c, K_DECIMATE);
+            launch_decimate(p, acc, r0, std::min(65535, nrows - r0), c->stream);
+        }
+        TRY(check_launch("dec_kernel"));
+    }
+    return PRC_OK;
+}
+
+int normalize_device(Ctx* c, const void* x, int dt, long long n, void* y) {
+    using namespace dec;
+    NormParams p{};
+    p.x = x; p.dt = dt; p.n = n; p.y = y;
+    p.nctas = norm_ctas(n);
+    p.per_cta = (n + p.nctas - 1) / p.nctas;
+    AsyncScratch ws(c->stream);
+    TRY(ws.get(&p.part, (size_t)p.nctas * sizeof(double)));
+    {
+        ProfScope ps(c, K_NORM_SUM);
+        launch_norm_sum(p, c->stream);
+    }
+    TRY(check_launch("norm_sum_kernel"));
+    {
+        ProfScope ps(c, K_NORM_SCALE);
+        launch_norm_scale(p, c->nsm, c->stream);
+    }
+    return check_launch("norm_scale_kernel");
+}
+
 }  // namespace
 
 // =========================================================================== C ABI
@@ -2733,6 +2786,49 @@ int prc_psd_frames(const void* x, int dtype, int64_t n, int nframes, int64_t fra
     std::lock_guard<std::mutex> lk(c->mu);
     TRY(psd_device(c, x, dtype, n, nframes, frame_stride, nfft, noverlap, ilog2(pad_to), window, scale, onesided, out,
                    out_stride));
+    return finish(c, flags);
+}
+
+int prc_decimate_rows(const void* x, int src, int64_t n, int nrows, int64_t row_stride, int mode, double fc, double fs,
+                      double phase_offset, const double* taps, int q, void* out, int64_t out_stride, int device,
+                      void* stream, unsigned flags) {
+    if (!x || !taps || !out) return fail(PRC_E_INVALID, "x/taps/out must not be NULL");
+    const bool raw = src >= PRC_DEC_RAW;
+    if (raw ? (src - PRC_DEC_RAW < PRC_IQ_C64 || src - PRC_DEC_RAW > PRC_IQ_I16) : (src < PRC_DT_I8 || src > PRC_DT_C128))
+        return fail(PRC_E_INVALID, "src=%d invalid: a PRC_DT_* code, or PRC_DEC_RAW + PRC_IQ_C64 / PRC_IQ_I8 / PRC_IQ_I16",
+                    src);
+    if (raw && (mode < PRC_MIX_NONE || mode > PRC_MIX_FS64)) return fail(PRC_E_INVALID, "mode=%d invalid", mode);
+    if (q < dec::MIN_Q || q > dec::MAX_Q)
+        return fail(PRC_E_INVALID, "q=%d outside [%d, %d]: the decimation factor's limits", q, dec::MIN_Q, dec::MAX_Q);
+    if (n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    if (nrows < 1) return fail(PRC_E_INVALID, "nrows=%d invalid", nrows);
+    if (nrows > 1 && row_stride < n)
+        return fail(PRC_E_INVALID, "row_stride=%lld smaller than n=%lld", (long long)row_stride, (long long)n);
+    const long long nout = (n + q - 1) / q;
+    if (nrows > 1 && out_stride < nout)
+        return fail(PRC_E_INVALID, "out_stride=%lld smaller than the %lld outputs per row", (long long)out_stride, nout);
+    dec::DecParams p{};
+    p.x = x; p.src = src; p.n = n; p.row_stride = row_stride; p.q = q; p.nout = nout;
+    p.y = out; p.out_stride = out_stride;
+    if (raw) p.mix = make_mix(x, src - PRC_DEC_RAW, n, mode, fc, fs, phase_offset);
+    p.G = dec::group_lanes(q);
+    dec::slab_geometry(q, p.G, &p.ks, &p.ksp, &p.nslab);
+    const int acc = dec::acc_kind(src, raw ? mode : PRC_MIX_NONE);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    TRY(decimate_device(c, p, acc, nrows, taps));
+    return finish(c, flags);
+}
+
+int prc_normalize(const void* x, int dtype, int64_t n, void* out, int device, void* stream, unsigned flags) {
+    if (!x || !out) return fail(PRC_E_INVALID, "x/out must not be NULL");
+    if (dtype < PRC_DT_I8 || dtype > PRC_DT_C128) return fail(PRC_E_INVALID, "dtype=%d invalid: a PRC_DT_* code", dtype);
+    if (n < 1) return fail(PRC_E_INVALID, "n=%lld invalid", (long long)n);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    TRY(normalize_device(c, x, dtype, n, out));
     return finish(c, flags);
 }
 

@@ -24,19 +24,6 @@ struct ChunkParams {
 
 constexpr int MIX_THREADS = 256;
 
-__device__ __forceinline__ float2 iq_load_scalar(const void* in, int kind, long long i) {
-    if (kind == IQ_I8) {
-        const signed char* x = static_cast<const signed char*>(in);
-        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
-    }
-    if (kind == IQ_I16) {
-        const short* x = static_cast<const short*>(in);
-        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
-    }
-    const float* x = static_cast<const float*>(in);
-    return make_float2(x[2 * i], x[2 * i + 1]);
-}
-
 // what chunk b's samples are mixed with: chunk 0's description moved to chunk b's raw samples and phase offset
 __device__ __forceinline__ MixParams chunk_mix(const ChunkParams& p, int b) {
     MixParams m = p.rs.mix;

@@ -5,8 +5,8 @@ Drop-ins for ``passiveRadar.signal_utils.deinterleave_IQ`` (reference
 (``:15-17``), the chain ``main.py:105-166`` runs on every input chunk, plus ``frontend`` which runs
 the three in one pass on the device (raw IQ in, resampled complex64 out), and the channel-offset estimator
 ``find_channel_offset`` (``:73-78``) with ``offset_compensation`` (``:49-71``), ``shift`` (``:34-47``) and ``xcorr``
-(``:29-32``).  All arithmetic runs in
-``libprcore.so``; no CPU fallback.
+(``:29-32``), and ``decimate`` (``:11-13``), ``channel_preprocessing`` (``:80-85``) and ``normalize`` (``:7-9``).  All
+arithmetic runs in ``libprcore.so``; no CPU fallback.
 """
 from __future__ import annotations
 
@@ -290,3 +290,216 @@ def xcorr(s1, s2, nlead, nlag, *, device=None):
     if rt.kind in "iu":
         return np.around(out).astype(np.int64).astype(rt)
     return out.astype(rt, copy=False)
+
+
+# ---- decimate, channel_preprocessing, normalize (reference signal_utils.py:7-13, :80-85) ---------------------------
+_NATIVE = {np.dtype(np.int8): _lib.DT_I8, np.dtype(np.uint8): _lib.DT_U8, np.dtype(np.int16): _lib.DT_I16,
+           np.dtype(np.float32): _lib.DT_F32, np.dtype(np.float64): _lib.DT_F64,
+           np.dtype(np.complex64): _lib.DT_C64, np.dtype(np.complex128): _lib.DT_C128}
+_RAW_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.dtype(np.float32): _lib.IQ_C64}
+
+
+def _torch():
+    import torch
+    return torch
+
+
+def _np_dtype_of(torch, t):
+    """NumPy dtype of a tensor's elements (None for the ones NumPy has no name for here, e.g. bfloat16)."""
+    return {torch.bool: np.bool_, torch.int8: np.int8, torch.uint8: np.uint8, torch.int16: np.int16,
+            torch.int32: np.int32, torch.int64: np.int64, torch.float16: np.float16, torch.float32: np.float32,
+            torch.float64: np.float64, torch.complex64: np.complex64, torch.complex128: np.complex128}.get(t.dtype)
+
+
+def _torch_dtype(torch, dt):
+    return {np.dtype(np.int8): torch.int8, np.dtype(np.uint8): torch.uint8, np.dtype(np.int16): torch.int16,
+            np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
+            np.dtype(np.complex64): torch.complex64, np.dtype(np.complex128): torch.complex128}[np.dtype(dt)]
+
+
+def _device_of(torch, device):
+    if not torch.cuda.is_available():
+        raise _lib.PrcoreError(_lib.PRC_E_CUDA, "no CUDA device available; libprcore has no CPU fallback")
+    return torch.device("cuda", _lib.current_device() if device is None else int(device))
+
+
+def _forked(torch, tdev, call):
+    """Run one library call on a side stream forked from, and joined back into, the current torch stream.  The library
+    gives a NULL stream (torch's default stream) a stream of its own, so the call is never enqueued on it directly."""
+    cur = torch.cuda.current_stream(tdev)
+    side = torch.cuda.Stream(device=tdev)
+    side.wait_stream(cur)
+    _lib.check(call(side.cuda_stream))
+    cur.wait_stream(side)
+
+
+@functools.lru_cache(maxsize=32)
+def _decimate_taps(q, single):
+    """decimate's FIR design, firwin(20q + 1, 1/q, window='hamming'), float32-rounded when the result is float32 or
+    complex64 (``b = np.asarray(b, dtype=result_type)`` in scipy.signal.decimate)."""
+    from scipy.signal import firwin
+    b = firwin(20 * q + 1, 1.0 / q, window='hamming')
+    if single:
+        b = b.astype(np.float32).astype(np.float64)
+    return np.ascontiguousarray(b, dtype=np.float64)
+
+
+def _decimation_factor(q):
+    """scipy.signal.decimate's argument errors for q, raised before the library is loaded."""
+    q = operator.index(q)
+    if q == 0:
+        raise ZeroDivisionError("float division by zero")
+    if q < 2:
+        raise ValueError("Invalid cutoff frequency: frequencies must be greater than 0 and less than fs/2.")
+    return q
+
+
+def _decimate_dtype(dt):
+    """scipy.signal.decimate's result dtype: x's own when inexact, float64 for integers, bools and float16."""
+    dt = np.dtype(dt)
+    if dt in (np.dtype(np.longdouble), np.dtype(np.clongdouble)) and dt not in _NATIVE:
+        raise TypeError("No matching signature found")
+    if dt.kind == "c":
+        return dt
+    if dt.kind not in "biuf":
+        raise TypeError(f"decimate takes numeric arrays, got {dt}")
+    return dt if dt == np.float32 else np.dtype(np.float64)
+
+
+def _run_decimate(torch, rows, src, n, mode, fc, Fs, po, q, single, out_dtype, tdev):
+    """One prc_decimate_rows call on the current torch stream: rows (k, n) contiguous on tdev -> (k, ceil(n/q))."""
+    k = rows.shape[0]
+    out = torch.empty(k, -(-n // q), dtype=_torch_dtype(torch, out_dtype), device=tdev)
+    taps = _decimate_taps(q, single)
+    lib = _lib.load()
+    _forked(torch, tdev, lambda st: lib.prc_decimate_rows(rows.data_ptr(), src, n, k, n, mode, float(fc), float(Fs), po,
+                                                          taps.ctypes.data, q, out.data_ptr(), out.shape[1], tdev.index,
+                                                          st, _lib.FLAG_ASYNC))
+    return out
+
+
+def decimate(x, q, *, device=None):
+    '''decimate x by a factor of q
+
+    ``scipy.signal.decimate(x, q, 20*q, ftype='fir', axis=0)`` on the device: the zero-phase FIR decimator with 20q+1
+    Hamming taps along axis 0 of an array of any shape, in SciPy's dtype (x's own when inexact, float64 otherwise;
+    float32 taps and sums for float32 and complex64, float64 for the rest).  A NumPy (or array-like) x gives NumPy; a
+    CUDA tensor gives a tensor on its device, ordered on the current torch stream.'''
+    q = _decimation_factor(q)
+    torch = None
+    if type(x).__module__.startswith("torch"):
+        torch = _torch()
+    if torch is not None and isinstance(x, torch.Tensor):
+        if not x.is_cuda:
+            raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
+        ndt = _np_dtype_of(torch, x)
+        if ndt is None:
+            raise TypeError(f"decimate takes numeric tensors, got {x.dtype}")
+        shape, rd = tuple(x.shape), _decimate_dtype(ndt)
+    else:
+        x = np.asarray(x)
+        shape, rd = x.shape, _decimate_dtype(x.dtype)
+    if len(shape) == 0:
+        raise IndexError("tuple index out of range")
+    n = shape[0]
+    k = int(np.prod(shape[1:], dtype=np.int64))
+    nout = -(-n // q)
+    if n == 0 or k == 0:
+        if torch is not None and isinstance(x, torch.Tensor):
+            return torch.empty((nout,) + shape[1:], dtype=_torch_dtype(torch, rd), device=x.device)
+        return np.empty((nout,) + shape[1:], dtype=rd)
+    single = rd in (np.float32, np.complex64)
+    if torch is not None and isinstance(x, torch.Tensor):
+        t = x
+        if np.dtype(ndt) not in _NATIVE:
+            t = t.to(torch.float64)
+        rows = t.reshape(n, k).T.contiguous()
+        out = _run_decimate(torch, rows, _NATIVE[np.dtype(_np_dtype_of(torch, rows))], n, _lib.MIX_NONE, 0.0, 1.0, 0.0,
+                            q, single, rd, x.device)
+        return out.T.reshape((nout,) + shape[1:])
+    a = x if x.dtype in _NATIVE else x.astype(rd)
+    torch = _torch()
+    tdev = _device_of(torch, device)
+    rows = torch.from_numpy(np.ascontiguousarray(a.reshape(n, k).T)).to(tdev)
+    out = _run_decimate(torch, rows, _NATIVE[a.dtype], n, _lib.MIX_NONE, 0.0, 1.0, 0.0, q, single, rd, tdev)
+    return np.ascontiguousarray(out.cpu().numpy().T).reshape((nout,) + shape[1:])
+
+
+def channel_preprocessing(sig, dec, fc, Fs, *, device=None):
+    '''deinterleave IQ samples, tune to channel frequency and decimate
+
+    ``decimate(frequency_shift(deinterleave_IQ(sig), fc, Fs), dec)`` in one pass on the device: the raw int8, int16 or
+    float32 I/Q is deinterleaved (I = sig[0:-1:2], Q = sig[1::2]) and mixed as it is staged, so the tuned signal is never
+    stored.  complex64 when the reference's is (Python-scalar fc and Fs), complex128 otherwise.  A CUDA tensor of raw
+    samples gives a tensor on its device, ordered on the current torch stream.'''
+    q = _decimation_factor(dec)
+    mode, po = _mix_mode(fc, Fs, 0)
+    rd = np.dtype(np.complex64) if mode == _lib.MIX_C64 else np.dtype(np.complex128)
+    torch = _torch() if type(sig).__module__.startswith("torch") else None
+    if torch is not None and isinstance(sig, torch.Tensor):
+        if not sig.is_cuda:
+            raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
+        if sig.dim() != 1:
+            raise ValueError("interleaved IQ must be one-dimensional")
+        n = sig.shape[0] // 2
+        t = sig[:2 * n]
+        ndt = _np_dtype_of(torch, t)
+        if ndt is None or np.dtype(ndt) not in _RAW_KINDS:
+            t = t.to(torch.float32)
+            ndt = np.float32
+        if n == 0:
+            return torch.empty(0, dtype=_torch_dtype(torch, rd), device=sig.device)
+        raw, kind, tdev = t.contiguous(), _RAW_KINDS[np.dtype(ndt)], sig.device
+    else:
+        buf, kind, n = _raw_iq(sig)
+        if n == 0:
+            return np.empty(0, dtype=rd)
+        torch = _torch()
+        tdev = _device_of(torch, device)
+        raw = torch.from_numpy(buf).to(tdev)
+    out = _run_decimate(torch, raw.view(1, -1), _lib.DEC_RAW + kind, n, mode, fc, Fs, po, q, mode == _lib.MIX_C64, rd,
+                        tdev)[0]
+    return out if isinstance(sig, torch.Tensor) else out.cpu().numpy()
+
+
+_NORM_OUT = {np.dtype(np.float32): np.dtype(np.float32), np.dtype(np.complex64): np.dtype(np.complex64),
+             np.dtype(np.complex128): np.dtype(np.complex128)}
+
+
+def normalize(x, *, device=None):
+    '''normalize ndarray to unit mean
+
+    ``x / np.mean(np.abs(x).flatten())`` on the device for int8, uint8, int16, float32, float64, complex64 and
+    complex128 x of any shape, in NumPy's result dtype (float64 for the integers).  The mean is summed in float64 in a
+    fixed order.  An all-zero x gives NaN, an empty x an empty result.  A CUDA tensor gives a tensor on its device,
+    ordered on the current torch stream.'''
+    torch = _torch() if type(x).__module__.startswith("torch") else None
+    is_t = torch is not None and isinstance(x, torch.Tensor)
+    if is_t:
+        if not x.is_cuda:
+            raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
+        dt = _np_dtype_of(torch, x)
+        dt = None if dt is None else np.dtype(dt)
+    else:
+        x = np.asarray(x)
+        dt = x.dtype
+    if dt not in _NATIVE:
+        raise TypeError(f"normalize takes int8, uint8, int16, float32, float64, complex64 or complex128, got {dt}")
+    rd = _NORM_OUT.get(dt, np.dtype(np.float64))
+    shape = tuple(x.shape)
+    n = int(np.prod(shape, dtype=np.int64))
+    if n == 0:
+        if is_t:
+            return torch.empty(shape, dtype=_torch_dtype(torch, rd), device=x.device)
+        return np.empty(shape, dtype=rd)
+    if is_t:
+        src, tdev = x.contiguous(), x.device
+    else:
+        torch = _torch()
+        tdev = _device_of(torch, device)
+        src = torch.from_numpy(np.ascontiguousarray(x).reshape(-1)).to(tdev)
+    out = torch.empty(shape, dtype=_torch_dtype(torch, rd), device=tdev)
+    lib = _lib.load()
+    _forked(torch, tdev, lambda st: lib.prc_normalize(src.data_ptr(), _NATIVE[dt], n, out.data_ptr(), tdev.index, st,
+                                                      _lib.FLAG_ASYNC))
+    return out if is_t else out.cpu().numpy()
