@@ -118,12 +118,9 @@ def onepass_limits(L, M, R, peek):
     return bls, min(bls, L - M - R - peek + 1)
 
 
-def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
-    """framepass.cuh in numpy: per Doppler-block segment Ys' (srv from i0 - peek), Yr' (ref from i0 - (M-1)), X_ls and
-    X_caf; LS sums from X_ls, AccP / AccQ per block from X_caf, then AccP - AccQ conj(W') and lags peek .. R + peek.
-    The sample two blocks share goes to the first block's X_ls only; samples after the last block are LS-only
-    segments.  Returns (c, x, P)."""
-    n, M = len(ref), len(w)
+def onepass_partition(n, F, M, R, peek, L, limits=None):
+    """The segments of the one-pass frame: per Doppler block (lo, hi, ls_end, nseg, Bs) -- samples [lo, hi) in nseg
+    segments of Bs, X_ls takes [lo, ls_end) -- and the LS-only tail (tail_lo, ntail, Bt)."""
     D = n // F
     ntaps = D + 1
     half = (ntaps - 1) // 2
@@ -132,6 +129,25 @@ def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
     assert c0 - (ntaps - 1) <= 0, "no samples before the first block"
     bls, bmax = limits or onepass_limits(L, M, R, peek)
     assert bmax >= 1
+    blocks = []
+    for j in range(F):
+        lo = max(j * D + c0 - (ntaps - 1), 0)
+        hi = min(j * D + c0 + 1, n)
+        ls_end = min(hi, max((j + 1) * D + c0 - (ntaps - 1), 0)) if j + 1 < F else hi
+        nseg = -(-(hi - lo) // bmax)
+        blocks.append((lo, hi, ls_end, nseg, -(-(hi - lo) // nseg) if nseg else 0))
+    tail_lo = min((F - 1) * D + c0 + 1, n)
+    ntail = -(-(n - tail_lo) // bls)
+    return blocks, (tail_lo, ntail, -(-(n - tail_lo) // ntail) if ntail else 0)
+
+
+def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
+    """framepass.cuh in numpy: per Doppler-block segment Ys' (srv from i0 - peek), Yr' (ref from i0 - (M-1)), X_ls and
+    X_caf; LS sums from X_ls, AccP / AccQ per block from X_caf, then AccP - AccQ conj(W') and lags peek .. R + peek.
+    The sample two blocks share goes to the first block's X_ls only; samples after the last block are LS-only
+    segments.  Returns (c, x, P)."""
+    n, M = len(ref), len(w)
+    blocks, (tail_lo, ntail, Bt) = onepass_partition(n, F, M, R, peek, L, limits)
     Wp = taps_spectrum(w, L)
     xw = ref * (win if win is not None else 1.0)
 
@@ -147,12 +163,7 @@ def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
     accX = np.zeros(L, complex)
     P = np.zeros((F, R + 1), complex)
     covered = np.zeros(n, int)
-    for j in range(F):
-        lo = max(j * D + c0 - (ntaps - 1), 0)
-        hi = min(j * D + c0 + 1, n)
-        ls_end = min(hi, max((j + 1) * D + c0 - (ntaps - 1), 0)) if j + 1 < F else hi
-        nseg = -(-(hi - lo) // bmax)
-        Bs = -(-(hi - lo) // nseg)
+    for j, (lo, hi, ls_end, nseg, Bs) in enumerate(blocks):
         accP = np.zeros(L, complex)
         accQ = np.zeros(L, complex)
         for q in range(nseg):
@@ -169,17 +180,13 @@ def model_onepass(ref, srv, win, w, R, F, peek, L, limits=None):
             accQ += Xcaf * np.conj(Yr)
             accP += Xcaf * np.conj(Ys)
         P[j] = np.fft.fft(accP - accQ * np.conj(Wp))[peek:peek + R + 1] / L
-    tail_lo = min((F - 1) * D + c0 + 1, n)
-    if n > tail_lo:
-        ntail = -(-(n - tail_lo) // bls)
-        Bt = -(-(n - tail_lo) // ntail)
-        for k in range(ntail):
-            i0 = tail_lo + k * Bt
-            ln = min(Bt, n - i0)
-            covered[i0:i0 + ln] += 1
-            Xls = seg(ref, i0, ln)
-            accC += Xls * np.conj(spec(ref, i0 - (M - 1)))
-            accX += Xls * np.conj(spec(srv, i0 - peek))
+    for k in range(ntail):
+        i0 = tail_lo + k * Bt
+        ln = min(Bt, n - i0)
+        covered[i0:i0 + ln] += 1
+        Xls = seg(ref, i0, ln)
+        accC += Xls * np.conj(spec(ref, i0 - (M - 1)))
+        accX += Xls * np.conj(spec(srv, i0 - peek))
     assert (covered == 1).all(), "every sample in exactly one X_ls"
     c = np.fft.fft(accC)[M - 1:2 * M - 1] / L
     x = np.fft.fft(accX)[:M] / L
@@ -212,49 +219,6 @@ def check(name, a, b, den=None, tol=1e-9):
     assert e < tol, name
 
 
-for n, M, peek, L in [(8192, 110, 10, 2048), (20000, 310, 10, 2048), (5000, 64, 0, 1024), (12345, 300, 7, 2048)]:
-    ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    for linear in (False, True):
-        C, X = model_lscorr(ref, srv, M, peek, L, linear)
-        check(f"lscorr n={n} M={M} L={L} linear={linear} autocorr", C, direct_lags(ref, ref, range(M), n, linear))
-        check(f"lscorr n={n} M={M} L={L} linear={linear} xcorr", X, direct_lags(ref, srv, range(-peek, M - peek), n, linear))
-    w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M
-    for linear in (False, True):
-        got = model_fir(ref, srv, w, peek, L, linear)
-        want = srv.copy()
-        for k in range(M):
-            sh = np.roll(ref, k - peek)
-            if linear:
-                d = k - peek
-                sh = np.zeros(n, complex)
-                if d >= 0:
-                    sh[d:] = ref[:n - d]
-                else:
-                    sh[:n + d] = ref[-d:]
-            want = want - w[k] * sh
-        check(f"fir n={n} M={M} linear={linear}", got, want)
-
-for n, F, R, M, peek, L in [(16384, 8, 40, 50, 10, 2048), (20000, 16, 100, 110, 10, 2048), (8192, 32, 20, 30, 10, 1024), (10000, 7, 33, 0, 0, 1024)]:
-    ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    win = np.kaiser(n, 5.0)
-    D = n // F
-    ntaps = D + 1
-    half = (ntaps - 1) // 2
-    pre_pad = D - half % D
-    c0 = ((half + pre_pad) // D) * D - pre_pad
-    w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M if M else None
-    s_eff = srv if w is None else srv - sum(w[k] * np.roll(ref, k - peek) for k in range(M))
-    want = np.zeros((F, R + 1), complex)
-    xw = ref * win
-    for j in range(F):
-        for m in range(ntaps):
-            i = j * D + c0 - m
-            if 0 <= i < n:
-                want[j] += xw[i] * np.conj(s_eff[(i + np.arange(R + 1)) % n])
-    got = model_caf(ref, srv, win, R, F, L, w, peek)
-    check(f"caf n={n} F={F} R={R} M={M} L={L}", got, want)
 # the one-pass frame: the headline shape (c2) and the planner's edges -- M = 1, 2, 1023, 1024 with peek 0 and M - 1, D = 32,
 # F = 1, n not a multiple of F, R + M near L (the CAF limit below the LS one), no window and a float window
 ONEPASS = [
@@ -270,17 +234,67 @@ ONEPASS = [
     (20011, 7, 60, 40, 39, 1024, True),
     (12000, 10, 600, 200, 5, 1024, False),
 ]
-for n, F, R, M, peek, L, use_win in ONEPASS:
-    ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
-    win = np.kaiser(n, 5.0) if use_win else None
-    w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M
-    tc, tx, tP = onepass_truth(ref, srv, win, w, R, F, peek)
-    c, x, P = model_onepass(ref, srv, win, w, R, F, peek, L)
-    tag = f"onepass n={n} F={F} R={R} M={M} peek={peek} L={L}"
-    check(tag + " c", c, tc, tol=1e-12)
-    check(tag + " x", x, tx, tol=1e-12)
-    check(tag + " P", P, tP, tol=1e-12)
-# the headline shape: Bmax = 1429, three segments per block, a 2047-sample LS-only tail
-assert onepass_limits(2048, 310, 300, 10) == (1430, 1429)
-print("model OK")
+
+
+def main():
+    for n, M, peek, L in [(8192, 110, 10, 2048), (20000, 310, 10, 2048), (5000, 64, 0, 1024), (12345, 300, 7, 2048)]:
+        ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        for linear in (False, True):
+            C, X = model_lscorr(ref, srv, M, peek, L, linear)
+            check(f"lscorr n={n} M={M} L={L} linear={linear} autocorr", C, direct_lags(ref, ref, range(M), n, linear))
+            check(f"lscorr n={n} M={M} L={L} linear={linear} xcorr", X, direct_lags(ref, srv, range(-peek, M - peek), n, linear))
+        w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M
+        for linear in (False, True):
+            got = model_fir(ref, srv, w, peek, L, linear)
+            want = srv.copy()
+            for k in range(M):
+                sh = np.roll(ref, k - peek)
+                if linear:
+                    d = k - peek
+                    sh = np.zeros(n, complex)
+                    if d >= 0:
+                        sh[d:] = ref[:n - d]
+                    else:
+                        sh[:n + d] = ref[-d:]
+                want = want - w[k] * sh
+            check(f"fir n={n} M={M} linear={linear}", got, want)
+
+    for n, F, R, M, peek, L in [(16384, 8, 40, 50, 10, 2048), (20000, 16, 100, 110, 10, 2048), (8192, 32, 20, 30, 10, 1024), (10000, 7, 33, 0, 0, 1024)]:
+        ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        win = np.kaiser(n, 5.0)
+        D = n // F
+        ntaps = D + 1
+        half = (ntaps - 1) // 2
+        pre_pad = D - half % D
+        c0 = ((half + pre_pad) // D) * D - pre_pad
+        w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M if M else None
+        s_eff = srv if w is None else srv - sum(w[k] * np.roll(ref, k - peek) for k in range(M))
+        want = np.zeros((F, R + 1), complex)
+        xw = ref * win
+        for j in range(F):
+            for m in range(ntaps):
+                i = j * D + c0 - m
+                if 0 <= i < n:
+                    want[j] += xw[i] * np.conj(s_eff[(i + np.arange(R + 1)) % n])
+        got = model_caf(ref, srv, win, R, F, L, w, peek)
+        check(f"caf n={n} F={F} R={R} M={M} L={L}", got, want)
+    for n, F, R, M, peek, L, use_win in ONEPASS:
+        ref = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        srv = rng.standard_normal(n) + 1j * rng.standard_normal(n)
+        win = np.kaiser(n, 5.0) if use_win else None
+        w = (rng.standard_normal(M) + 1j * rng.standard_normal(M)) / M
+        tc, tx, tP = onepass_truth(ref, srv, win, w, R, F, peek)
+        c, x, P = model_onepass(ref, srv, win, w, R, F, peek, L)
+        tag = f"onepass n={n} F={F} R={R} M={M} peek={peek} L={L}"
+        check(tag + " c", c, tc, tol=1e-12)
+        check(tag + " x", x, tx, tol=1e-12)
+        check(tag + " P", P, tP, tol=1e-12)
+    # the headline shape: Bmax = 1429, three segments per block, a 2047-sample LS-only tail
+    assert onepass_limits(2048, 310, 300, 10) == (1430, 1429)
+    print("model OK")
+
+
+if __name__ == "__main__":
+    main()

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import scipy.signal as signal
 
+from conftest import record_parity
 from passiveradar_b200 import _lib, synth
 from oracle import clutter_oracle as co
 from oracle import xambg_oracle as xo
@@ -163,6 +164,22 @@ EDGE_CASES = [
     ("n_not_multiple_of_F", 2 ** 17 + 3, 7, 60, 30, 9, "P0"),
     ("Bmax=1429", 2 ** 17, 16, 300, 300, 10, "P0"),
     ("P1", 2 ** 17, 16, 100, 50, 10, "P1"),
+    # segments at their limits (test_onepass_sweep.py's planner twin states each partition): blocks of 2 x Bmax under
+    # the CAF limit, of 3 x (Bmax + 1) (what a CAF limit one too large would make), the same for the LS limit bls, a
+    # tail of exactly bls and of bls + 1, segments and a tail of the whole transform, and the smallest Bmax the plan
+    # takes (545 from a sample of shapes, and L / 4 = 512, the plan's floor)
+    ("caf_exact", 45712, 16, 300, 300, 10, "P0"),
+    ("caf_one_past", 68624, 16, 300, 300, 10, "P0"),
+    ("ls_exact", 45744, 16, 100, 300, 10, "P0"),
+    ("ls_one_past", 68672, 16, 100, 300, 10, "P0"),
+    ("tail_exact", 45745, 16, 100, 300, 10, "P0"),
+    ("tail_plus_one", 45746, 16, 100, 300, 10, "P0"),
+    ("full_L", 65520, 16, 0, 1, 0, "P0"),
+    ("full_L_tail", 65552, 16, 0, 1, 0, "P0"),
+    ("smallest_Bmax", 1048708, 1024, 912, 564, 14, "P0"),
+    ("Bmax=L/4", 523264, 1024, 768, 769, 0, "P0"),
+    ("caf_exact_P1", 45712, 16, 300, 300, 10, "P1"),
+    ("ls_exact_P1", 45744, 16, 100, 300, 10, "P1"),
 ]
 
 
@@ -179,6 +196,7 @@ def test_onepass_at_the_plan_edges(edge, n, F, R, fl, peek, prof):
     refs = torch.from_numpy(ref[None]).to(dev)
     srvs = torch.from_numpy(srv[None]).to(dev)
     ref_err = None
+    fig = {}
     for win in ("none", "f64", "f32"):
         w = None if win == "none" else (w64 if win == "f64" else w64.astype(np.float32))
         d_w = None if w is None else torch.from_numpy(w).to(dev)
@@ -186,8 +204,10 @@ def test_onepass_at_the_plan_edges(edge, n, F, R, fl, peek, prof):
         maps1, taps1, _, ran = _frames(refs, srvs, fl, peek, R, F, d_w, 1, profile=True)
         assert ran, edge
         den = np.abs(amb).max()
-        assert rel(taps1[0], t_taps, np.abs(t_taps).max()) <= TOL, (edge, win)
+        e_taps = rel(taps1[0], t_taps, np.abs(t_taps).max())
+        assert e_taps <= TOL, (edge, win)
         e1 = rel(maps1[0], amb, den)
+        fig[f"E_taps_{win}"], fig[f"E_map_{win}"] = e_taps, e1
         if prof == "P0":
             assert e1 <= TOL, (edge, win, e1)
             continue
@@ -196,4 +216,6 @@ def test_onepass_at_the_plan_edges(edge, n, F, R, fl, peek, prof):
         if ref_err is None or win != "none":
             chain = xo.fast_xambg_oracle(ref, co.ls_filter_oracle(ref, srv, fl, 1.0, peek), R, F, n, w)[:, :, 0]
             ref_err = rel(chain, amb, den)
+        fig[f"E_map_two_pass_{win}"], fig[f"reference_map_vs_truth_{win}"] = e0, ref_err
         assert e1 <= 1e-5 + 1.2 * ref_err and e1 <= 2 * e0, (edge, win, e1, e0, ref_err)
+    record_parity(f"onepass/edge_{edge}", **fig)
