@@ -25,6 +25,8 @@
 // need none between them.  Twiddle tables (built in float64 by fft_twiddle_kernel, staged to shared memory):
 //   tw1[k1 * T + t]   = W_L^{t k1}            (L entries)
 //   tw2[k2 * R3 + n3] = W_{16 R3}^{n3 k2}     (16 R3 entries)
+// Pass 1 / pass 3 take their twiddles from a source (Tw1Table: tw1 in shared memory; Tw1Seeds: five registers per
+// thread, for frame_pass_kernel, whose shared-memory pipe is its bottleneck and which then stages tw2 alone).
 //
 // Every per-thread phase is a __host__ __device__ function of (registers, t, buffers): the same code is run
 // thread-by-thread on the CPU by scripts/fft/emul.cu and tests/test_fft_emulation.py to pin the index algebra
@@ -123,13 +125,50 @@ template <> struct Dft<16> {
     }
 };
 
+// ---- twiddle sources of n2p pass 1 and p2n pass 3: tw(t, k1) = W_L^{t k1}, k1 = 1..15 --------------------------
+// Tw1Table reads the tw1 table in shared memory.  Tw1Seeds holds five table values of its thread in registers (read
+// once from the global table) and forms each other twiddle as ONE product of two of them, so every twiddle is at most
+// one rounding beyond the float64-built table: k1 = 1, 3, 5, 7, 8 are table values ({1, 3, 5, 7, 8} is the smallest
+// set whose sums of two cover 1..15), the rest are 2 = 1+1, 4 = 1+3, 6 = 3+3, 9 = 1+8, 10 = 3+7, 11 = 3+8, 12 = 5+7,
+// 13 = 5+8, 14 = 7+7, 15 = 7+8.  No recurrence: errors do not chain.
+template <int R3> struct Tw1Table {
+    const float2* __restrict__ tw1;
+    PRC_HD float2 operator()(int t, int k1) const { return tw1[k1 * Geo<R3>::T + t]; }
+};
+
+template <int R3> struct Tw1Seeds {
+    float2 w1, w3, w5, w7, w8;
+    PRC_HD Tw1Seeds(const float2* __restrict__ tw1, int t)
+        : w1(tw1[Geo<R3>::T + t]), w3(tw1[3 * Geo<R3>::T + t]), w5(tw1[5 * Geo<R3>::T + t]),
+          w7(tw1[7 * Geo<R3>::T + t]), w8(tw1[8 * Geo<R3>::T + t]) {}
+    PRC_HD float2 operator()(int, int k1) const {
+        switch (k1) {
+        case 1: return w1;
+        case 2: return cmul(w1, w1);
+        case 3: return w3;
+        case 4: return cmul(w1, w3);
+        case 5: return w5;
+        case 6: return cmul(w3, w3);
+        case 7: return w7;
+        case 8: return w8;
+        case 9: return cmul(w1, w8);
+        case 10: return cmul(w3, w7);
+        case 11: return cmul(w3, w8);
+        case 12: return cmul(w5, w7);
+        case 13: return cmul(w5, w8);
+        case 14: return cmul(w7, w7);
+        default: return cmul(w7, w8);
+        }
+    }
+};
+
 // ---- natural -> permuted -------------------------------------------------------------------------------------
-template <int R3>
-PRC_HD void n2p_pass1(float2 (&v)[16], int t, float2* __restrict__ ea, const float2* __restrict__ tw1) {
+template <int R3, class Tw1 = Tw1Table<R3>>
+PRC_HD void n2p_pass1(float2 (&v)[16], int t, float2* __restrict__ ea, const Tw1& tw1) {
     using G = Geo<R3>;
     float2 w[16];                      // twiddle loads in flight while the butterflies run
 #pragma unroll
-    for (int k1 = 1; k1 < 16; ++k1) w[k1] = tw1[k1 * G::T + t];
+    for (int k1 = 1; k1 < 16; ++k1) w[k1] = tw1(t, k1);
     Dft<16>::run(v);
     const int n2 = t / R3, n3 = t - n2 * R3;
     float2* dst = ea + n2 * R3 + n3;
@@ -210,14 +249,14 @@ PRC_HD void p2n_pass2(float2 (&v)[16], int t, const float2* __restrict__ eb, flo
     for (int n2 = 0; n2 < 16; ++n2) dst[n2 * R3] = v[n2];
 }
 
-template <int R3>
-PRC_HD void p2n_pass3(float2 (&v)[16], int t, const float2* __restrict__ ea, const float2* __restrict__ tw1) {
+template <int R3, class Tw1 = Tw1Table<R3>>
+PRC_HD void p2n_pass3(float2 (&v)[16], int t, const float2* __restrict__ ea, const Tw1& tw1) {
     using G = Geo<R3>;
     const int n2 = t / R3, n3 = t - n2 * R3;
     const float2* src = ea + n2 * R3 + n3;
     float2 w[16];
 #pragma unroll
-    for (int k1 = 1; k1 < 16; ++k1) w[k1] = tw1[k1 * G::T + t];
+    for (int k1 = 1; k1 < 16; ++k1) w[k1] = tw1(t, k1);
 #pragma unroll
     for (int k1 = 0; k1 < 16; ++k1) v[k1] = src[k1 * G::S];
 #pragma unroll
@@ -228,13 +267,22 @@ PRC_HD void p2n_pass3(float2 (&v)[16], int t, const float2* __restrict__ ea, con
 #ifdef __CUDACC__
 // Block-wide transforms: every thread of the group (blockDim.x == T) calls them; `sm` = [ea | eb | tw1 | tw2].
 template <int R3> struct Smem {
-    float2* ea; float2* eb; const float2* tw1; const float2* tw2;
+    float2* ea; float2* eb; Tw1Table<R3> tw1; const float2* tw2;
     __device__ __forceinline__ explicit Smem(float2* base)
-        : ea(base), eb(base + Geo<R3>::EX), tw1(base + 2 * Geo<R3>::EX), tw2(base + 2 * Geo<R3>::EX + Geo<R3>::TW1) {}
+        : ea(base), eb(base + Geo<R3>::EX), tw1{base + 2 * Geo<R3>::EX}, tw2(base + 2 * Geo<R3>::EX + Geo<R3>::TW1) {}
 };
 
-template <int R3>
-__device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Smem<R3>& s) {
+// the same transforms with pass-1 / pass-3 twiddles from per-thread seeds: `sm` = [ea | eb | tw2], the seeds are read
+// from the global table [tw1 | tw2] (fft_twiddle_kernel's); the caller stages tw2 (stage_tw2) and synchronises
+template <int R3> struct SmemSeeded {
+    static constexpr int SMEM_FLOAT2 = 2 * Geo<R3>::EX + Geo<R3>::TW2;
+    float2* ea; float2* eb; Tw1Seeds<R3> tw1; const float2* tw2;
+    __device__ __forceinline__ SmemSeeded(float2* base, const float2* __restrict__ tw_global, int t)
+        : ea(base), eb(base + Geo<R3>::EX), tw1(tw_global, t), tw2(base + 2 * Geo<R3>::EX) {}
+};
+
+template <int R3, class Sm>
+__device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Sm& s) {
     n2p_pass1<R3>(v, t, s.ea, s.tw1);
     __syncthreads();
     n2p_pass2<R3>(v, t, s.ea, s.eb, s.tw2);
@@ -244,8 +292,8 @@ __device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Smem<R3>& 
 
 // same, with `after_pass1()` run once the group's first barrier has passed (every register of v has been consumed by
 // then): the place to start asynchronous copies that overwrite the shared-memory slots v was fetched from
-template <int R3, class Hook>
-__device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Smem<R3>& s, Hook after_pass1) {
+template <int R3, class Sm, class Hook>
+__device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Sm& s, Hook after_pass1) {
     n2p_pass1<R3>(v, t, s.ea, s.tw1);
     __syncthreads();
     after_pass1();
@@ -254,8 +302,8 @@ __device__ __forceinline__ void fft_n2p(float2 (&v)[16], int t, const Smem<R3>& 
     n2p_pass3<R3>(v, t, s.eb);
 }
 
-template <int R3>
-__device__ __forceinline__ void fft_p2n(float2 (&v)[16], int t, const Smem<R3>& s) {
+template <int R3, class Sm>
+__device__ __forceinline__ void fft_p2n(float2 (&v)[16], int t, const Sm& s) {
     p2n_pass1<R3>(v, t, s.eb);
     __syncthreads();
     p2n_pass2<R3>(v, t, s.eb, s.ea, s.tw2);
@@ -269,6 +317,13 @@ __device__ __forceinline__ void stage_twiddles(float2* base, const float2* __res
     using G = Geo<R3>;
     float2* dst = base + 2 * G::EX;
     for (int i = t; i < G::TW1 + G::TW2; i += G::T) dst[i] = tw_global[i];
+}
+
+// stage tw2 alone into SmemSeeded's layout; caller synchronises
+template <int R3>
+__device__ __forceinline__ void stage_tw2(float2* base, const float2* __restrict__ tw_global, int t) {
+    using G = Geo<R3>;
+    for (int i = t; i < G::TW2; i += G::T) base[2 * G::EX + i] = tw_global[G::TW1 + i];
 }
 
 // tw[0 .. L) = tw1, tw[L .. L + 16 R3) = tw2, evaluated in float64

@@ -24,7 +24,10 @@
 // samples before Ys', exactly as R_seg starts before S in caf_fft_kernel.
 //
 // Registers: AccP, AccQ and the two held spectra Ys', Yr' stay in registers; accC and accX live in thread-private
-// shared memory (4 x 8 KB at R3 = 8), so a CTA has 109 568 B of shared memory and two fit in an SM.
+// shared memory (4 x 8 KB at R3 = 8).  The pass-1 / pass-3 twiddles come from five per-thread registers (fft::Tw1Seeds)
+// instead of the tw1 table: that takes 15 of each thread's 64-bit shared loads per transform off the shared-memory
+// pipe, which bounds this kernel, and 16 KB out of the layout, so a CTA has 93 184 B of shared memory and two fit in
+// an SM.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -51,9 +54,9 @@ struct FramePassParams {
     const float2* tw;
 };
 
-// shared memory: [fft::Smem | staging L float2 | accC, accX 2 L float2 | window staging L float]
+// shared memory: [fft::SmemSeeded | staging L float2 | accC, accX 2 L float2 | window staging L float]
 template <int R3> constexpr int framepass_smem_float2() {
-    return fft::Geo<R3>::SMEM_FLOAT2 + 3 * fft::Geo<R3>::L + fft::Geo<R3>::L / 2;
+    return fft::SmemSeeded<R3>::SMEM_FLOAT2 + 3 * fft::Geo<R3>::L + fft::Geo<R3>::L / 2;
 }
 
 // a unit of a CTA's run: Doppler block u < F, else LS-only tail segment u - F
@@ -96,8 +99,8 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
     using G = fft::Geo<R3>;
     extern __shared__ __align__(16) float2 sm[];
     const int t = threadIdx.x;
-    const fft::Smem<R3> S(sm);
-    float2* stg = sm + G::SMEM_FLOAT2;
+    const fft::SmemSeeded<R3> S(sm, p.tw, t);
+    float2* stg = sm + fft::SmemSeeded<R3>::SMEM_FLOAT2;
     float2* accs = stg + G::L;                                   // accC [r T + t], accX [L + r T + t]
     float* wst = reinterpret_cast<float*>(accs + 2 * G::L);
     const float2* ref = p.ref + (size_t)blockIdx.y * p.frame_stride;
@@ -124,7 +127,7 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
         cp_async_commit();
     };
     if (cu < u1) issue(cu, cg, 0, 0);
-    fft::stage_twiddles<R3>(sm, p.tw, t);
+    fft::stage_tw2<R3>(sm, p.tw, t);
 #pragma unroll
     for (int r = 0; r < 16; ++r) accs[r * G::T + t] = accs[G::L + r * G::T + t] = make_float2(0.f, 0.f);
     __syncthreads();
