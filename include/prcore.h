@@ -59,6 +59,9 @@ typedef struct prc_c64 { float re, im; } prc_c64;
 #define PRC_FLAG_PROD_F32    32u   /* prc_persistence_frames: float32 products float32(x) * float32(w) */
 #define PRC_FLAG_ORIENT      64u   /* prc_persistence_frames: frames are written as fliplr(P.T) */
 #define PRC_FLAG_TRACK_RESUME 128u /* tracker entry points: continue from the frame-0 records of `history` */
+#define PRC_FLAG_CHANNEL_PAIR 256u /* prc_iq_mix_c64, prc_frontend_c64, prc_frontend_chunks_c64: `in` is one channel of a
+                                    * two-channel stream whose complex samples alternate between the channels */
+/* Every entry point ignores the flags that are not its own. */
 
 /* ---- lifecycle / diagnostics ------------------------------------------------ */
 int         prc_version(void);
@@ -264,6 +267,14 @@ int prc_direct_xambg_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int 
  *           the exponential is then evaluated in float64).  Results are complex64 either way.
  * in      : I and Q are read as scalars, so `in` may sit at any raw element, odd ones included (a raw array
  *           sliced by a channel offset, main.py:87-92).
+ * PRC_FLAG_CHANNEL_PAIR: `in` is one channel of a stream that holds two channels' I/Q as
+ *           [ref_I[0], ref_Q[0], srv_I[0], srv_Q[0], ref_I[1], ...] (PRconfig.yaml's interleaved_input_channels):
+ *           complex sample i is read from raw elements 4i and 4i+1 of `in`.  Pass the stream's element 0 for the
+ *           reference channel and element 2 for the surveillance channel, plus 4 * start for a channel trimmed to
+ *           start at sample `start`.  n and chunk_stride count the channel's complex samples; every other argument
+ *           and check is unchanged.  From host memory exactly the raw span the channel's samples occupy is copied,
+ *           its first I to its last Q (2 * (2 * N - 1) elements for N samples), so the surveillance channel's buffer
+ *           may end at its last Q.
  * prc_frontend_c64 additionally applies resample() = scipy.signal.resample_poly(x, up, down,
  * padtype='line') (signal_utils.py:15-17) in the same pass: h = the nh = 2*half_len+1 low-pass taps
  * ALREADY multiplied by up (what resample_poly hands to upfirdn; host doubles, designed by the caller

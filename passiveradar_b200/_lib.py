@@ -31,6 +31,7 @@ FLAG_CR_F64 = 16
 FLAG_PROD_F32 = 32
 FLAG_ORIENT = 64
 FLAG_TRACK_RESUME = 128
+FLAG_CHANNEL_PAIR = 256
 IQ_C64, IQ_I8, IQ_I16 = 0, 1, 2
 MIX_NONE, MIX_C64, MIX_C128, MIX_F64, MIX_FS64 = 0, 1, 2, 3, 4
 DT_I8, DT_U8, DT_I16, DT_F32, DT_F64, DT_C64, DT_C128 = 0, 1, 2, 3, 4, 5, 6

@@ -107,7 +107,7 @@ __device__ __forceinline__ void add_down(double2& a, int off, int G) {
 __device__ __forceinline__ float2 raw_sample(const DecParams& p, int b, long long i) {
     const int kind = p.mix.kind;
     const void* in = static_cast<const char*>(p.x) + (size_t)b * p.row_stride * (kind == IQ_I8 ? 2 : kind == IQ_I16 ? 4 : 8);
-    return mix_sample(p.mix, iq_load_scalar(in, kind, i), i);
+    return mix_sample(p.mix, iq_load_scalar(in, kind, i, 2), i);
 }
 template <class V> __device__ V load(const DecParams& p, int b, long long i);
 template <> __device__ __forceinline__ float load<float>(const DecParams& p, int b, long long i) {

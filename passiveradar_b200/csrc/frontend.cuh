@@ -17,6 +17,8 @@ enum MixMode { MIX_NONE = 0, MIX_C64 = 1, MIX_C128 = 2, MIX_F64 = 3, MIX_FS64 = 
 struct MixParams {
     const void* in;
     int kind;            // IqKind
+    int pitch;           // raw elements from one complex sample to the next: 2, or 4 for one channel of a stream whose
+                         // complex samples alternate between two channels (PRC_FLAG_CHANNEL_PAIR)
     long long n;         // complex samples
     int mode;            // MixMode
     float B;             // float32(2 pi fc): imaginary part of complex64(1j*2*pi*fc)
@@ -26,18 +28,20 @@ struct MixParams {
     double B64, rFs64;   // MIX_F64 / MIX_FS64: the same in float64 (fc or Fs was a NumPy float64 scalar)
 };
 
-// complex sample i of raw interleaved I/Q, read as scalars (the recording chain's chunks and decimate.cuh's slabs)
-__device__ __forceinline__ float2 iq_load_scalar(const void* in, int kind, long long i) {
+// complex sample i of raw interleaved I/Q whose samples are `pitch` raw elements apart, read as scalars (the recording
+// chain's chunks and decimate.cuh's slabs)
+__device__ __forceinline__ float2 iq_load_scalar(const void* in, int kind, long long i, int pitch) {
+    const long long j = pitch * i;
     if (kind == IQ_I8) {
         const signed char* x = static_cast<const signed char*>(in);
-        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
+        return make_float2((float)x[j], (float)x[j + 1]);
     }
     if (kind == IQ_I16) {
         const short* x = static_cast<const short*>(in);
-        return make_float2((float)x[2 * i], (float)x[2 * i + 1]);
+        return make_float2((float)x[j], (float)x[j + 1]);
     }
     const float* x = static_cast<const float*>(in);
-    return make_float2(x[2 * i], x[2 * i + 1]);
+    return make_float2(x[j], x[j + 1]);
 }
 
 // x[i] * exp(1j * theta_i) with numpy's evaluation order:

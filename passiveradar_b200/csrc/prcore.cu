@@ -865,9 +865,23 @@ size_t iq_bytes(int kind, long long n) {
     return (size_t)n * (kind == IQ_I8 ? 2 : kind == IQ_I16 ? 4 : 8);
 }
 
-MixParams make_mix(const void* in, int kind, long long n, int mode, double fc, double fs, double po) {
+// raw bytes from the first I to the last Q of n >= 1 complex samples `pitch` raw elements apart: with pitch 4 (one
+// channel of a PRC_FLAG_CHANNEL_PAIR stream) the other channel's last sample, which may lie past the caller's buffer,
+// is not part of it
+size_t iq_span_bytes(int kind, long long n, int pitch) {
+    return iq_bytes(kind, 1) / 2 * ((size_t)pitch * (size_t)(n - 1) + 2);
+}
+
+// raw elements from one complex sample to the next: 4 for one channel of a PRC_FLAG_CHANNEL_PAIR stream, 2 otherwise
+int iq_pitch(unsigned flags) {
+    return (flags & PRC_FLAG_CHANNEL_PAIR) ? 4 : 2;
+}
+
+// flags: the front-end entry points' own (PRC_FLAG_CHANNEL_PAIR); every other caller reads plain I/Q
+MixParams make_mix(const void* in, int kind, long long n, int mode, double fc, double fs, double po, unsigned flags = 0) {
     MixParams m{};
     m.in = in; m.kind = kind; m.n = n; m.mode = mode;
+    m.pitch = iq_pitch(flags);
     m.B = (float)(2.0 * 3.14159265358979323846 * fc);
     m.rFs = 1.0f / (float)fs;
     m.po = po;
@@ -929,12 +943,13 @@ int resample_table(Ctx* c, const ResampleGeo& g, const double* h, int nh, Resamp
     return PRC_OK;
 }
 
-// nchunks chunks of mix.n samples each, chunk b at raw sample b * chunk_stride of mix.in, mixed with phase offset po[b]
-// (device doubles; NULL: mix.po, for a single chunk), its output at out + b * out_stride (recording.cuh)
+// nchunks chunks of mix.n samples each, chunk b at complex sample b * chunk_stride of mix.in (samples mix.pitch raw
+// elements apart), mixed with phase offset po[b] (device doubles; NULL: mix.po, for a single chunk), its output at
+// out + b * out_stride (recording.cuh)
 rec::ChunkParams chunk_params(const MixParams& mix, int nchunks, long long chunk_stride, const double* po, long long out_stride) {
     rec::ChunkParams p{};
     p.rs.mix = mix;
-    p.chunk_bytes = (long long)iq_bytes(mix.kind, chunk_stride);
+    p.chunk_bytes = (long long)(iq_bytes(mix.kind, 1) / 2 * mix.pitch) * chunk_stride;     // raw element size x pitch
     p.out_stride = out_stride;
     p.po = po;
     p.nchunks = nchunks;
@@ -2310,12 +2325,13 @@ int prc_iq_mix_c64(const void* in, int in_kind, int64_t n, int mode, double fc, 
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t ib = iq_bytes(in_kind, n), ob = (size_t)n * sizeof(float2);
+    const size_t ib = iq_span_bytes(in_kind, n, iq_pitch(flags)), ob = (size_t)n * sizeof(float2);
     const void* din;
     float2* dout;
     TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
     TRY(stage_out(out, mem_kind, ob, c->fe_out, &dout));
-    TRY(mix_chunks_device(c, K_MISC, chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset), 1, 0, nullptr, 0),
+    TRY(mix_chunks_device(c, K_MISC, chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset, flags), 1, 0,
+                                                  nullptr, 0),
                           dout));
     TRY(unstage(c, out, dout, mem_kind, 1, ob, ob, flags));
     return finish(c, flags);
@@ -2340,12 +2356,13 @@ int prc_frontend_c64(const void* in, int in_kind, int64_t n, int mode, double fc
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t ib = iq_bytes(in_kind, n);
+    const size_t ib = iq_span_bytes(in_kind, n, iq_pitch(flags));
     const void* din;
     float2* dout;
     TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
     TRY(stage_out(out, mem_kind, (size_t)g.n_out * sizeof(float2), c->fe_out, &dout));
-    TRY(frontend_device(c, K_MISC, chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset), 1, 0, nullptr, 0), g,
+    TRY(frontend_device(c, K_MISC,
+                        chunk_params(make_mix(din, in_kind, n, mode, fc, fs, phase_offset, flags), 1, 0, nullptr, 0), g,
                         h, nh, dout));
     TRY(unstage(c, out, dout, mem_kind, 1, (size_t)g.n_out * sizeof(float2), (size_t)g.n_out * sizeof(float2), flags));
     return finish(c, flags);
@@ -2370,7 +2387,8 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
     Ctx* c;
     TRY(get_ctx(device, stream, &c));
     std::lock_guard<std::mutex> lk(c->mu);
-    const size_t ib = iq_bytes(in_kind, (long long)(nchunks - 1) * cstride + n), cb = (size_t)g.n_out * sizeof(float2);
+    const size_t ib = iq_span_bytes(in_kind, (long long)(nchunks - 1) * cstride + n, iq_pitch(flags));
+    const size_t cb = (size_t)g.n_out * sizeof(float2);
     const void* din;
     float2* dout;
     TRY(stage_in(c, in, mem_kind, 1, ib, ib, c->fe_in, flags, &din));
@@ -2378,7 +2396,8 @@ int prc_frontend_chunks_c64(const void* in, int in_kind, int64_t n, int nchunks,
     const long long dstride = mem_kind == PRC_MEM_HOST ? g.n_out : ostride;      // staged chunks are packed
     TRY(copy_params(c, phase_offsets, nchunks, c->fe_po));
     TRY(frontend_device(c, K_FRONTEND_CHUNKS,
-                        chunk_params(make_mix(din, in_kind, n, mode, fc, fs, 0.0), nchunks, cstride, c->fe_po.as<double>(),
+                        chunk_params(make_mix(din, in_kind, n, mode, fc, fs, 0.0, flags), nchunks, cstride,
+                                     c->fe_po.as<double>(),
                                      dstride),
                         g, h, nh, dout));
     TRY(unstage(c, out, dout, mem_kind, nchunks, cb, (size_t)ostride * sizeof(float2), flags));

@@ -3,7 +3,9 @@
 // resample_poly's line extension taken from its own end points (main.py:151-166).  gridDim.y is the chunk.  These are
 // the front end's only kernels: prc_iq_mix_c64 and prc_frontend_c64 run them on one chunk, so every chunk of
 // prc_frontend_chunks_c64 is bit-identical to a single call on it.  I and Q are loaded as scalars: main.py slices the
-// raw arrays by the channel offset (main.py:87-92), so a chunk may start at any raw element, odd ones included.
+// raw arrays by the channel offset (main.py:87-92), so a chunk may start at any raw element, odd ones included.  With
+// PRC_FLAG_CHANNEL_PAIR the raw input is one channel of a two-channel stream (rs.mix.pitch = 4): complex sample i is
+// raw elements 4i and 4i+1, and the other channel's samples in between are never read.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,7 +39,7 @@ __global__ void rec_ends_kernel(const __grid_constant__ ChunkParams p) {
     if (t >= 2 * p.nchunks) return;
     const MixParams m = chunk_mix(p, t >> 1);
     const long long i = (t & 1) ? m.n - 1 : 0;
-    p.ends[t] = mix_sample(m, iq_load_scalar(m.in, m.kind, i), i);
+    p.ends[t] = mix_sample(m, iq_load_scalar(m.in, m.kind, i, m.pitch), i);
 }
 
 __global__ void __launch_bounds__(RS_THREADS) rec_resample_kernel(const __grid_constant__ ChunkParams p,
@@ -67,7 +69,7 @@ __global__ void __launch_bounds__(RS_THREADS) rec_resample_kernel(const __grid_c
             // the chunk's MixParams are rebuilt per sample from the grid constants: a copy held across the staging
             // loop would be kept live over its 64-bit divisions and spill
             const MixParams m = chunk_mix(p, b);
-            v = mix_sample(m, iq_load_scalar(m.in, m.kind, i), i);
+            v = mix_sample(m, iq_load_scalar(m.in, m.kind, i, m.pitch), i);
         }
         xs[q] = v;
     }
@@ -83,7 +85,7 @@ __global__ void rec_mix_kernel(const __grid_constant__ ChunkParams p, float2* __
     const long long i = (long long)blockIdx.x * MIX_THREADS + threadIdx.x;
     const MixParams m = chunk_mix(p, b);
     if (i >= m.n) return;
-    out[(size_t)b * p.out_stride + i] = mix_sample(m, iq_load_scalar(m.in, m.kind, i), i);
+    out[(size_t)b * p.out_stride + i] = mix_sample(m, iq_load_scalar(m.in, m.kind, i, m.pitch), i);
 }
 
 // ---- launches (host side; prcore.cu brackets them with its profiling scope and checks the launch) ----------------

@@ -30,9 +30,18 @@ Decisions where main.py cannot be followed literally:
   instead (main.py:70-72): ``ref[:offset]``, ``srv[-offset:]``.
 * ``overlap_cpi: False`` is refused: the reference's own ``getConfiguration`` raises ``KeyError`` there
   (config.py:77 reads ``config['cpi']``), so no reference run has that geometry.
-* ``interleaved_input_channels: True`` is refused with ``NotImplementedError``: that branch rechunks to
-  ``input_chunk_length`` complex samples while its phase offsets assume ``input_chunk_length // 2``, and which of the
-  two it means is an open question.
+* ``interleaved_input_channels: True`` (one raw source, ``[ref_I[0], ref_Q[0], srv_I[0], srv_Q[0], ref_I[1], ...]``)
+  runs only with ``interleaved_chunking="separate"``, and is refused with ``NotImplementedError`` without it.  That
+  branch of main.py (main.py:46-75) rechunks each channel to ``input_chunk_length`` complex samples, while its phase
+  offsets, its declared resampled chunks and its overlap depth assume ``input_chunk_length // 2``: taken literally, every
+  frame is longer than ``cpi_samples`` and ``fast_xambg``'s padding raises, so it makes no map.  ``"separate"`` cuts
+  each channel into chunks of ``input_chunk_length // 2`` complex samples, as the separate-channel branch does; only
+  where the samples come from changes.  The offset is then in complex samples: it is estimated as main.py:50-54 does,
+  on ``[0::2]`` and ``[1::2]`` of ``deinterleave_IQ(stream[0:20 cpi])``, and trims as main.py:67-72 does.  With
+  ``nb = ceil(len(stream) / (2 icl))`` raw blocks dask declares ``nb * (icl // 2)`` samples per channel, so
+  ``N_chunks = min((nb * (icl // 2) - |offset|) // (icl // 2), num_frames) - 1``.  An interleaved recording and the
+  same channels stored separately, at offset ``c`` against ``2 c`` raw elements, give bit-identical maps when both count
+  the same chunks.
 * A resampling ratio whose CTA needs more than the front end's 200 KB of shared memory is refused at construction with
   the library's message (``PrcoreError``).
 * ``N_chunks = min(N_ref, N_srv, num_frames) - 1`` where ``N_x`` counts the ``input_chunk_length`` blocks dask cuts the
@@ -47,7 +56,7 @@ import numpy as np
 import scipy.signal as signal
 
 from . import _lib
-from .signal_utils import _decimate_sos, _mix_mode, _OFFSET_DTYPES, _resample_taps, find_channel_offset
+from .signal_utils import _decimate_sos, _mix_mode, _OFFSET_DTYPES, _PADLEN, _resample_taps, find_channel_offset
 
 _IQ_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.dtype(np.float32): _lib.IQ_C64}
 DOPPLER_BINS = (0, 1, -1, 2, -2)         # main.py:174: clutter at 0 Hz, +/-1 Hz, +/-2 Hz
@@ -94,11 +103,20 @@ def trim(n_ref, n_srv, offset):
 class RecordingPipeline:
     """main.py's recording chain on one device; see the module docstring.  ``batch`` chunks are processed per step."""
 
-    def __init__(self, config, *, batch=8, device=None):
-        if config.get("interleaved_input_channels"):
+    def __init__(self, config, *, batch=8, device=None, interleaved_chunking=None):
+        self.interleaved = bool(config.get("interleaved_input_channels"))
+        if interleaved_chunking is not None and not self.interleaved:
+            raise ValueError("interleaved_chunking applies to interleaved_input_channels: True only")
+        if self.interleaved and interleaved_chunking is None:
             raise NotImplementedError(
-                "interleaved_input_channels: True is not supported: that branch of main.py rechunks to input_chunk_length "
-                "complex samples while its phase offsets assume input_chunk_length // 2")
+                "interleaved_input_channels: True needs interleaved_chunking='separate': main.py's interleaved branch "
+                "rechunks to input_chunk_length complex samples while its phase offsets, resampled chunks and overlap "
+                "assume input_chunk_length // 2, so taken literally its frames exceed cpi_samples and it makes no map; "
+                "'separate' cuts each channel into input_chunk_length // 2 samples as the separate-channel branch does")
+        if self.interleaved and interleaved_chunking != "separate":
+            raise ValueError(f"interleaved_chunking={interleaved_chunking!r}: the one chunking offered is 'separate'")
+        if self.interleaved and int(config["input_chunk_length"]) % 2:
+            raise ValueError("interleaved_input_channels: True needs an even input_chunk_length (config.py makes it so)")
         if not config.get("overlap_cpi"):
             raise ValueError("overlap_cpi: False is not supported: the reference's getConfiguration raises KeyError "
                              "for it (config.py:77), so main.py never runs that geometry")
@@ -138,7 +156,8 @@ class RecordingPipeline:
 
     @classmethod
     def from_config(cls, config, **kw):
-        """From the dict ``passiveRadar.config.getConfiguration`` returns (main.py:231)."""
+        """From the dict ``passiveRadar.config.getConfiguration`` returns (main.py:231).  An interleaved config needs
+        ``interleaved_chunking="separate"`` (see the module docstring)."""
         return cls(config, **kw)
 
     # ------------------------------------------------------------------ geometry (no device)
@@ -149,7 +168,16 @@ class RecordingPipeline:
         return 2 * np.pi * np.arange(nchunks) * per_block * (self.fo / self.fs)
 
     def plan(self, n_ref, n_srv, offset):
-        """Raw slices and chunk count main.py:86-120 gives raw channels of n_ref / n_srv elements."""
+        """Raw slices and chunk count main.py:86-120 gives raw channels of n_ref / n_srv elements.  Interleaved: n_ref
+        is the stream's raw length, n_srv is None and the offset is in complex samples; the channel starts are in
+        complex samples, and sample j of channel q (0 = ref, 1 = srv) is raw elements 4j + 2q and 4j + 2q + 1."""
+        if self.interleaved:
+            h, offset = self.n_in, int(offset)
+            nb = -(-int(n_ref) // (2 * self.icl))                 # da.from_array(chunks=(2 icl,)) blocks
+            nchunks = max(0, min((nb * h - abs(offset)) // h, self.num_frames) - 1)
+            r0, s0 = max(offset, 0), max(-offset, 0)
+            return {"ref_start": r0, "srv_start": s0, "ref_raw_start": 4 * r0, "srv_raw_start": 4 * s0 + 2,
+                    "nchunks": nchunks, "phase_offsets": self.phase_offsets(nchunks)}
         r0, r1, s0, s1 = trim(n_ref, n_srv, offset)
         blocks = lambda n: -(-n // self.icl)
         nchunks = max(0, min(blocks(r1 - r0), blocks(s1 - s0), self.num_frames) - 1)
@@ -220,7 +248,8 @@ class RecordingPipeline:
         _lib.check(self.lib.prc_frontend_chunks_c64(
             raw_ptr, kind, self.n_in, nb, self.n_in, self.mix_mode, float(self.fo), float(self.fs), po.ctypes.data,
             self.up, self.dn, self.taps.ctypes.data, self.taps.shape[0], out_ptr, self.Lc, nb * self.Lc,
-            _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream, _lib.FLAG_ASYNC))
+            _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream,
+            _lib.FLAG_ASYNC | (_lib.FLAG_CHANNEL_PAIR if self.interleaved else 0)))
 
     def _clean(self, ref_rows, srv_rs, out_rows, nb):
         _lib.check(self.lib.prc_ls_multiple_frames_c64(
@@ -248,16 +277,59 @@ class RecordingPipeline:
                                                _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream, 0))
         return int(off.item())
 
-    # ------------------------------------------------------------------ public entry points
-    def run_device(self, ref_raw, srv_raw, maps=None, offset=None):
-        """ref_raw, srv_raw: 1-D contiguous raw interleaved IQ CUDA tensors (int8, int16 or float32) on the pipeline's
-        device.  Writes the maps as (nframes, F, R+1) complex64 into ``maps`` (allocated when None) on the device and
-        returns it.  Work is forked from, and joined back into, the current torch stream: the raw tensors may still be
-        being written by work queued there, and the maps are ready for work queued there after the call."""
+    def _offset_interleaved(self, head, kind):
+        """find_channel_offset(refc1, srvc1, 1, 5_000_000) (main.py:50-54) for device-resident raw data head =
+        stream[0:20 cpi]: refc1 and srvc1 are [0::2] and [1::2] of deinterleave_IQ(head), complex64, so the offset is
+        in complex samples.  Both channels are read out of the stream in place."""
         torch = _torch()
+        m = head.shape[0] // 2                                    # deinterleave_IQ's complex samples
+        lens = ((m + 1) // 2, m // 2)
+        if min(lens) <= _PADLEN:
+            raise ValueError(f"The length of the input vector x must be greater than padlen, which is {_PADLEN}.")
+        chans = [torch.empty(n, dtype=torch.complex64, device=self.tdev) for n in lens]
+        for q in range(2):
+            _lib.check(self.lib.prc_iq_mix_c64(head.data_ptr() + 2 * q * head.element_size(), kind, lens[q],
+                                               _lib.MIX_NONE, 0.0, 1.0, 0.0, chans[q].data_ptr(), _lib.MEM_DEVICE,
+                                               self.dev, self.stream.cuda_stream,
+                                               _lib.FLAG_ASYNC | _lib.FLAG_CHANNEL_PAIR))
+        sos, zi = _decimate_sos(1, True)
+        sos, zi = np.ascontiguousarray(np.stack([sos, sos])), np.ascontiguousarray(np.stack([zi, zi]))
+        off = torch.zeros(1, dtype=torch.int64, device=self.tdev)
+        _lib.check(self.lib.prc_channel_offset(chans[0].data_ptr(), _lib.DT_C64, lens[0], chans[1].data_ptr(),
+                                               _lib.DT_C64, lens[1], 1, 5_000_000, sos.ctypes.data, zi.ctypes.data,
+                                               off.data_ptr(), None, _lib.MEM_DEVICE, self.dev,
+                                               self.stream.cuda_stream, 0))
+        return int(off.item())
+
+    def _sources(self, ref_raw, srv_raw):
+        """The raw sources of a run: the one stream of an interleaved pipeline, or ref_raw and srv_raw."""
+        if self.interleaved:
+            if srv_raw is not None:
+                raise ValueError("interleaved_input_channels is True: pass the one interleaved source only")
+            return (ref_raw,)
+        if srv_raw is None:
+            raise ValueError("interleaved_input_channels is False: pass ref_raw and srv_raw")
+        return ref_raw, srv_raw
+
+    def _reads(self, p):
+        """Where the front end reads a plan's chunks: for each channel the raw element of its source where its chunk 0
+        starts and the source it is in (0 or 1), and the raw elements from one chunk to the next."""
+        if self.interleaved:
+            return (p["ref_raw_start"], p["srv_raw_start"]), (0, 0), 4 * self.n_in
+        return (p["ref_start"], p["srv_start"]), (0, 1), self.icl
+
+    # ------------------------------------------------------------------ public entry points
+    def run_device(self, ref_raw, srv_raw=None, maps=None, offset=None):
+        """ref_raw, srv_raw: 1-D contiguous raw interleaved IQ CUDA tensors (int8, int16 or float32) on the pipeline's
+        device; for an interleaved pipeline ref_raw is the one two-channel stream and srv_raw is None, and ``offset``
+        is in complex samples.  Writes the maps as (nframes, F, R+1) complex64 into ``maps`` (allocated when None) on
+        the device and returns it.  Work is forked from, and joined back into, the current torch stream: the raw tensors
+        may still be being written by work queued there, and the maps are ready for work queued there after the call."""
+        torch = _torch()
+        srcs = self._sources(ref_raw, srv_raw)
         self._setup()
         kinds = []
-        for name, t in (("ref_raw", ref_raw), ("srv_raw", srv_raw)):
+        for name, t in zip(("ref_raw", "srv_raw"), srcs):
             if not isinstance(t, torch.Tensor) or t.device != self.tdev:
                 raise ValueError(f"{name} must be a tensor on {self.tdev}")
             if t.dim() != 1 or not t.is_contiguous():
@@ -270,8 +342,9 @@ class RecordingPipeline:
         self.stream.wait_stream(cur)
         if offset is None:
             with torch.cuda.stream(self.stream):
-                offset = self._offset_device(ref_raw, srv_raw)
-        p = self.plan(ref_raw.shape[0], srv_raw.shape[0], offset)
+                offset = (self._offset_interleaved(ref_raw[:20 * self.cpi], kinds[0]) if self.interleaved else
+                          self._offset_device(ref_raw, srv_raw))
+        p = self.plan(ref_raw.shape[0], None if self.interleaved else srv_raw.shape[0], offset)
         N = p["nchunks"]
         if maps is None:                  # allocated on the caller's stream, which it is returned to
             maps = torch.empty(N, self.F, self.R + 1, dtype=torch.complex64, device=self.tdev)
@@ -280,15 +353,15 @@ class RecordingPipeline:
             raise ValueError(f"maps must be a contiguous complex64 tensor of shape (>= {N}, {self.F}, {self.R + 1}) "
                              f"on {self.tdev}")
         with torch.cuda.stream(self.stream):
-            starts = (p["ref_start"], p["srv_start"])
-            size = [t.element_size() for t in (ref_raw, srv_raw)]
-            base = [t.data_ptr() for t in (ref_raw, srv_raw)]
+            starts, src, step = self._reads(p)
+            size = [t.element_size() for t in srcs]
+            base = [t.data_ptr() for t in srcs]
 
             def compute(c0, nb, ref_rows, srv_rows):
                 po = p["phase_offsets"][c0:c0 + nb]
-                raw = [base[q] + (starts[q] + c0 * self.icl) * size[q] for q in range(2)]
-                self._frontend(raw[0], kinds[0], nb, po, ref_rows.data_ptr())
-                self._frontend(raw[1], kinds[1], nb, po, self.srv_rs.data_ptr())
+                raw = [base[src[q]] + (starts[q] + c0 * step) * size[src[q]] for q in range(2)]
+                self._frontend(raw[0], kinds[src[0]], nb, po, ref_rows.data_ptr())
+                self._frontend(raw[1], kinds[src[1]], nb, po, self.srv_rs.data_ptr())
                 self._clean(ref_rows, self.srv_rs[:nb], srv_rows, nb)
 
             self._stream(N, self.tdev, compute, lambda j0, rf, sf: self._maps(rf, sf, maps[j0:j0 + rf.shape[0]]))
@@ -296,30 +369,41 @@ class RecordingPipeline:
         self.nframes, self.offset = N, int(offset)
         return maps
 
-    def run(self, ref_raw, srv_raw, offset=None):
+    def run(self, ref_raw, srv_raw=None, offset=None):
         """ref_raw, srv_raw: 1-D raw interleaved IQ sources (ndarray, np.memmap, h5py dataset: anything sliceable),
-        int8, int16 or float32.  Returns main.py's ``xambg``: (F, R+1, nframes) complex64 on the host."""
+        int8, int16 or float32; for an interleaved pipeline ref_raw is the one two-channel stream and srv_raw is None,
+        and ``offset`` is in complex samples.  Returns main.py's ``xambg``: (F, R+1, nframes) complex64 on the host."""
         torch = _torch()
         from .frames import pinned_empty
+        srcs = self._sources(ref_raw, srv_raw)
         self._setup()
-        if offset is None:
-            offset = find_channel_offset(ref_raw[0:10 * self.cpi], srv_raw[0:10 * self.cpi], 1, 5_000_000, device=self.dev)
-        p = self.plan(ref_raw.shape[0], srv_raw.shape[0], offset)
-        N, B, icl = p["nchunks"], self.batch, self.icl
-        dtypes = [np.dtype(src.dtype) for src in (ref_raw, srv_raw)]
+        dtypes = [np.dtype(x.dtype) for x in srcs]
         kinds = [_IQ_KINDS[dt] for dt in dtypes]
-        starts = (p["ref_start"], p["srv_start"])
+        if offset is None and self.interleaved:
+            with torch.cuda.stream(self.stream):             # the head's copy is ordered before its reads
+                head = torch.from_numpy(np.ascontiguousarray(ref_raw[0:20 * self.cpi])).to(self.tdev)
+                offset = self._offset_interleaved(head, kinds[0])
+        elif offset is None:
+            offset = find_channel_offset(ref_raw[0:10 * self.cpi], srv_raw[0:10 * self.cpi], 1, 5_000_000, device=self.dev)
+        p = self.plan(ref_raw.shape[0], None if self.interleaved else srv_raw.shape[0], offset)
+        N, B = p["nchunks"], self.batch
+        starts, src, step = self._reads(p)
+        # a batch of nb chunks from chunk c0 stages raw elements [win[j] + c0 step, + nb step + extra) of source j: the
+        # stream's window holds both channels' chunks, the trimmed channel's |offset| samples later than the other's
+        win, extra = ((0,), 4 * abs(int(offset))) if self.interleaved else (starts, 0)
+        at = [starts[q] - win[src[q]] for q in range(2)]        # channel q's first chunk in its staged window
         out = np.empty((self.F, self.R + 1, N), dtype=np.complex64)
         # two slots of raw batches (pinned host, device), of maps (device, pinned host); kept for the next run, since
         # page-locking them costs more than a short recording takes
         tdt = {np.dtype(np.int8): torch.int8, np.dtype(np.int16): torch.int16, np.dtype(np.float32): torch.float32}
-        if getattr(self, "_ring_key", None) != (tuple(dtypes), self.dev):
-            self._ring = ([[torch.empty(B * icl, dtype=tdt[dt], pin_memory=True) for dt in dtypes] for _ in range(2)],
-                          [[torch.empty(B * icl, dtype=tdt[dt], device=self.tdev) for dt in dtypes] for _ in range(2)],
+        slot = B * step + extra
+        if getattr(self, "_ring_key", None) != (tuple(dtypes), slot, self.dev):
+            self._ring = ([[torch.empty(slot, dtype=tdt[dt], pin_memory=True) for dt in dtypes] for _ in range(2)],
+                          [[torch.empty(slot, dtype=tdt[dt], device=self.tdev) for dt in dtypes] for _ in range(2)],
                           [torch.empty(B + 1, self.F, self.R + 1, dtype=torch.complex64, device=self.tdev)
                            for _ in range(2)],
                           [pinned_empty((B + 1, self.F, self.R + 1)) for _ in range(2)])
-            self._ring_key = (tuple(dtypes), self.dev)
+            self._ring_key = (tuple(dtypes), slot, self.dev)
         host_raw, dev_raw, dev_maps, host_maps = self._ring
         copied = [torch.cuda.Event() for _ in range(2)]         # raw slot's host-to-device copy done
         read = [torch.cuda.Event() for _ in range(2)]           # raw slot's front end done
@@ -339,18 +423,20 @@ class RecordingPipeline:
             state["batch"] += 1
             if state["batch"] > 2:
                 copied[s].synchronize()                         # the slot's previous copy has left host memory
-            for q in range(2):
-                a = starts[q] + c0 * icl
-                host_raw[s][q][:nb * icl].numpy()[:] = np.asarray(src[q][a:a + nb * icl])
+            L = nb * step + extra
+            for j, x in enumerate(srcs):
+                a = win[j] + c0 * step
+                host_raw[s][j][:L].numpy()[:] = np.asarray(x[a:a + L])
             with torch.cuda.stream(self.copy_stream):
                 self.copy_stream.wait_event(read[s])            # the batch two back has finished reading the slot
-                for q in range(2):
-                    dev_raw[s][q][:nb * icl].copy_(host_raw[s][q][:nb * icl], non_blocking=True)
+                for j in range(len(srcs)):
+                    dev_raw[s][j][:L].copy_(host_raw[s][j][:L], non_blocking=True)
                 copied[s].record(self.copy_stream)
             self.stream.wait_event(copied[s])
             po = p["phase_offsets"][c0:c0 + nb]
-            self._frontend(dev_raw[s][0].data_ptr(), kinds[0], nb, po, ref_rows.data_ptr())
-            self._frontend(dev_raw[s][1].data_ptr(), kinds[1], nb, po, self.srv_rs.data_ptr())
+            raw = [dev_raw[s][src[q]].data_ptr() + at[q] * dev_raw[s][src[q]].element_size() for q in range(2)]
+            self._frontend(raw[0], kinds[src[0]], nb, po, ref_rows.data_ptr())
+            self._frontend(raw[1], kinds[src[1]], nb, po, self.srv_rs.data_ptr())
             read[s].record(self.stream)
             self._clean(ref_rows, self.srv_rs[:nb], srv_rows, nb)
 
@@ -364,7 +450,6 @@ class RecordingPipeline:
             landed[s].record(self.stream)
             pending[s] = (j0, m)
 
-        src = (ref_raw, srv_raw)
         with torch.cuda.stream(self.stream):
             self._stream(N, self.tdev, compute, emit)
         for s in range(2):

@@ -270,6 +270,12 @@ class SignalPreview:
         _lib.check(self.lib.prc_iq_mix_c64(raw.data_ptr(), kind, n, _lib.MIX_NONE, 0.0, 1.0, 0.0, out.data_ptr(),
                                            _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream, _lib.FLAG_ASYNC))
 
+    def _channel(self, data, kind, q, n, out):
+        """deinterleave_IQ(data)[q::2]: the first n samples of channel q of a two-channel stream, read in place"""
+        _lib.check(self.lib.prc_iq_mix_c64(data.data_ptr() + 2 * q * data.element_size(), kind, n, _lib.MIX_NONE, 0.0,
+                                           1.0, 0.0, out.data_ptr(), _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream,
+                                           _lib.FLAG_ASYNC | _lib.FLAG_CHANNEL_PAIR))
+
     def _psd(self, rows, n, nfft, Fs, out):
         """plt.psd's spectrum of rows (a (k, >= n) complex64 tensor) at NFFT nfft, scaled with Fs, into out."""
         w = self._window(nfft)
@@ -299,12 +305,12 @@ class SignalPreview:
                 raise ValueError("interleaved_input_channels is True: pass the one interleaved source only")
             k = self._check_raw("data", ref_raw)
             data = ref_raw[:self.icl]
-            iq = torch.empty(data.shape[0] // 2, dtype=torch.complex64, device=self.tdev)
-            self._deinterleave(data, k, iq)
-            n_ref, n_srv = (iq.shape[0] + 1) // 2, iq.shape[0] // 2
+            m = data.shape[0] // 2                                 # deinterleave_IQ's complex samples
+            n_ref, n_srv = (m + 1) // 2, m // 2
             chans = torch.zeros(2, n_ref, dtype=torch.complex64, device=self.tdev)
-            chans[0].copy_(iq[0::2])
-            chans[1, :n_srv].copy_(iq[1::2])
+            for q, n in enumerate((n_ref, n_srv)):
+                if n:
+                    self._channel(data, k, q, n, chans[q])
         else:
             if srv_raw is None:
                 raise ValueError("interleaved_input_channels is False: pass ref_raw and srv_raw")
