@@ -88,7 +88,7 @@ def decimate_chunked(x, nd, chunk, warm):
 
 
 def warmup_samples(sos):
-    """W of the device decimator (csrc/prcore.cu chanoff_warmup): from the largest pole radius of the sections."""
+    """W of the device decimator (csrc/prcore_signal.cu chanoff_warmup): from the largest pole radius of the sections."""
     r = 0.0
     for s in np.asarray(sos, dtype=np.float64):
         r = max(r, float(np.abs(np.roots([1.0, s[4], s[5]])).max()))

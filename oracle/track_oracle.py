@@ -3,7 +3,7 @@
 Written from the arithmetic DESIGN.md section 11 lists, with the documented tie rule for equal candidate strengths:
 strength descending, then descending position in the transformed frame (np.flip(np.argsort(s, kind="stable"))).
 Kalman products go through NumPy's matmul and np.linalg.inv, as in the reference.  ``pairwise_mean_twin`` is the host
-twin of the measurement kernel's mean (csrc/track.cuh: the summation tree of prcore.cu's trk_plan).
+twin of the measurement kernel's mean (csrc/track.cuh: the summation tree of prcore_detect.cu's trk_plan).
 """
 from __future__ import annotations
 

@@ -15,8 +15,9 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libprcore.so")
-SOURCES = [os.path.join(CSRC, "prcore.cu")]
-# every header prcore.cu includes: a stale library after editing one of them is the worst kind of bug
+# the runtime (prcore.cu) and one translation unit per operator family (prcore_*.cu), linked into one library
+SOURCES = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
+# every header the sources include: a stale library after editing one of them is the worst kind of bug
 HEADERS = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + \
           [os.path.join(ROOT, "include", "prcore.h")]
 
@@ -25,6 +26,7 @@ NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-Xcompiler", "-fPIC", "-shared",
+    "-Xcompiler", "-fvisibility=hidden",      # the modules' shared host functions stay internal; prc_* are exported
     "-Xptxas", "-v",
 ]
 

@@ -323,7 +323,7 @@ __global__ void __launch_bounds__(ARG_THREADS) chanoff_argmax_final_kernel(const
     if (threadIdx.x == 0) { res[0] = bk; res[1] = (bk - nl) * nd; }
 }
 
-// ---- launches (host side; prcore.cu brackets them with its profiling scopes and checks the launch) ----------------
+// ---- launches (host side; prcore_signal.cu brackets them with its profiling scopes and checks the launch) ----------------
 template <bool CPLX, bool BACKWARD>
 inline void launch_iir_t(const IirParams& p, cudaStream_t st) {
     const long long nchunk = (p.next + p.chunk - 1) / p.chunk;

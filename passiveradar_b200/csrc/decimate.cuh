@@ -284,7 +284,7 @@ __global__ void __launch_bounds__(NORM_THREADS) norm_scale_kernel(const NormPara
     }
 }
 
-// ---- launches (host side; prcore.cu brackets them with its profiling scopes and checks the launch) --------------------
+// ---- launches (host side; prcore_signal.cu brackets them with its profiling scopes and checks the launch) --------------------
 template <class V> inline cudaError_t set_attr_t(int lim) {
     return cudaFuncSetAttribute(dec_kernel<V>, cudaFuncAttributeMaxDynamicSharedMemorySize, lim);
 }

@@ -131,20 +131,7 @@ __global__ void __launch_bounds__(CFAR_TX * CFAR_TY) cfar_frames_kernel(const __
     if (p.det) p.det[o] = cr > (double)p.thresh ? 1 : 0;
 }
 
-// one row of direct_xambg: out[f][k] = sum over pieces of partial[piece][R - k]
-__global__ void piece_sum_kernel(const float2* __restrict__ partial, int npieces, int HT, int R, float2* __restrict__ out_row) {
-    const int k = blockIdx.x * blockDim.x + threadIdx.x;
-    if (k > R) return;
-    float2 s = make_float2(0.f, 0.f);
-    for (int q = 0; q < npieces; ++q) {
-        const float2 v = partial[(size_t)q * HT + (R - k)];
-        s.x += v.x;
-        s.y += v.y;
-    }
-    out_row[k] = s;
-}
-
-// ---- launches (host side; prcore.cu brackets them with its profiling scope and checks the launch) ----------------
+// ---- launches (host side; prcore_detect.cu brackets them with its profiling scope and checks the launch) ----------------
 inline cudaError_t allow_cfar_smem(int bytes) {
     return cudaFuncSetAttribute(cfar_frames_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }

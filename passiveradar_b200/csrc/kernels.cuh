@@ -590,7 +590,7 @@ struct DopplerParams {
     int blk_len;             // stream layout (lagstream_kernel): rows actually written for block j =
     long long per_cta;       //   stream_pieces(j, blk_len, per_cta); per_cta == 0: all nchunk rows
     // optional boundary sample of every Doppler block, i = j*bstride + boff, added to its lag sums
-    // (bx == nullptr: none; every launch in prcore.cu leaves it null)
+    // (bx == nullptr: none; every launch in prcore_corr.cu leaves it null)
     const float2* bx;
     const float2* bs;
     const float* bwin;       // optional: bx is the unweighted reference, multiply by bwin[i]

@@ -199,4 +199,17 @@ __global__ void weight_kernel(const float2* __restrict__ x, const float* __restr
     }
 }
 
+// one row of direct_xambg: out[f][k] = sum over pieces of partial[piece][R - k]
+__global__ void piece_sum_kernel(const float2* __restrict__ partial, int npieces, int HT, int R, float2* __restrict__ out_row) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k > R) return;
+    float2 s = make_float2(0.f, 0.f);
+    for (int q = 0; q < npieces; ++q) {
+        const float2 v = partial[(size_t)q * HT + (R - k)];
+        s.x += v.x;
+        s.y += v.y;
+    }
+    out_row[k] = s;
+}
+
 }  // namespace prc

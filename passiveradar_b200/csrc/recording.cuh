@@ -88,7 +88,7 @@ __global__ void rec_mix_kernel(const __grid_constant__ ChunkParams p, float2* __
     out[(size_t)b * p.out_stride + i] = mix_sample(m, iq_load_scalar(m.in, m.kind, i, m.pitch), i);
 }
 
-// ---- launches (host side; prcore.cu brackets them with its profiling scope and checks the launch) ----------------
+// ---- launches (host side; prcore_signal.cu brackets them with its profiling scope and checks the launch) ----------------
 inline cudaError_t allow_smem(int bytes) {
     return cudaFuncSetAttribute(rec_resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }

@@ -201,7 +201,7 @@ __global__ void __launch_bounds__(PCT_THREADS) pct_kernel(const __grid_constant_
     }
 }
 
-// ---- launches (host side; prcore.cu brackets them with its profiling scope and checks the launch) ----------------
+// ---- launches (host side; prcore_detect.cu brackets them with its profiling scope and checks the launch) ----------------
 inline void launch_persistence(const PersistParams& p, cudaStream_t st) {
     const dim3 grid((unsigned)((p.cols + PST_TX - 1) / PST_TX), (unsigned)((p.rows + PST_TY - 1) / PST_TY));
     pst_kernel<<<grid, dim3(PST_TX, PST_TY), 0, st>>>(p);

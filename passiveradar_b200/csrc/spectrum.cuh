@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(FIN_THREADS) spec_finish_kernel(const FinParam
     p.out[(p.f0 + blockIdx.y) * p.out_stride + j] = v;
 }
 
-// ---- launches (host side; prcore.cu brackets them with its profiling scopes and checks the launch) ----------------
+// ---- launches (host side; prcore_signal.cu brackets them with its profiling scopes and checks the launch) ----------------
 inline size_t segments_smem(int m) { return ((size_t)1 << m) * sizeof(double2); }
 
 template <int ACC>

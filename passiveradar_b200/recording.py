@@ -62,7 +62,7 @@ _IQ_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.
 DOPPLER_BINS = (0, 1, -1, 2, -2)         # main.py:174: clutter at 0 Hz, +/-1 Hz, +/-2 Hz
 LS_PEEK = 10                             # LS_Filter_Multiple's default (clutter_removal.py:162)
 RS_THREADS = 256                         # outputs per resample CTA (frontend.cuh)
-SMEM_LIMIT = 200 * 1024                  # shared memory a front-end CTA may use (prcore.cu)
+SMEM_LIMIT = 200 * 1024                  # shared memory a front-end CTA may use (prcore_host.h)
 
 
 def _torch():
@@ -71,7 +71,7 @@ def _torch():
 
 
 def resample_smem_refusal(up, dn):
-    """The library's refusal of resample_poly(up, dn)'s CTA (prcore.cu: resample_table), or None if it fits."""
+    """The library's refusal of resample_poly(up, dn)'s CTA (prcore_signal.cu: resample_table), or None if it fits."""
     g = math.gcd(up, dn)
     up, dn = up // g, dn // g
     half_len = 10 * max(up, dn)

@@ -3,8 +3,9 @@
     python scripts/fft/ab_bench.py build --base REV        # compile REV's sources and the working tree's (no GPU needed)
     python scripts/fft/ab_bench.py run --out DIR           # A, B, A, B, A, B on the GPU; DIR/ab.json
 
-``build`` compiles ``passiveradar_b200/csrc`` + ``include`` of the commit REV (A: ``git archive``) and of the working
-tree (B) with the flags of passiveradar_b200/build.py into the git-ignored ``build/ab/{A,B}/libprcore.so``.  ``run``
+``build`` compiles every ``*.cu`` of ``passiveradar_b200/csrc`` (+ ``include``) of the commit REV (A: ``git archive``) and of
+the working tree (B), each with the flags of its own passiveradar_b200/build.py, into the git-ignored
+``build/ab/{A,B}/libprcore.so``.  ``run``
 alternates ``bench.py --no-cpu-baseline`` between the two (each child loads its build through PRC_LIBRARY; the Python
 side is the working tree's for both), so a drift of clocks or temperature over the session hits both builds alike.  The
 first run of each build also writes its ``--dump-outputs`` maps, and the two are compared bit for bit.  Per run it keeps
@@ -16,6 +17,7 @@ more power, and the cap then lowers the clock of everything running beside it.
 from __future__ import annotations
 
 import argparse
+import importlib.util
 import io
 import json
 import os
@@ -29,14 +31,24 @@ AB = os.path.join(ROOT, "build", "ab")
 KERNELS = ("lagcorr_ls", "lagcorr_caf", "caf_combine", "levinson", "doppler_fft")
 
 
+def tree_flags(src_root: str) -> list:
+    """NVCC_FLAGS of the tree's own build.py: a revision is compiled as it builds itself (the flags that export its C
+    entry points changed when prcore.cu was split into modules)."""
+    spec = importlib.util.spec_from_file_location("ab_tree_build", os.path.join(src_root, "passiveradar_b200", "build.py"))
+    m = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(m)
+    return m.NVCC_FLAGS
+
+
 def compile_lib(src_root: str, out_dir: str) -> str:
     sys.path.insert(0, ROOT)
     from passiveradar_b200 import build as b
     os.makedirs(out_dir, exist_ok=True)
     lib = os.path.join(out_dir, "libprcore.so")
-    cmd = [b.find_nvcc()] + b.NVCC_FLAGS + ["-I", os.path.join(src_root, "include"),
-                                            "-I", os.path.join(src_root, "passiveradar_b200", "csrc"),
-                                            "-o", lib, os.path.join(src_root, "passiveradar_b200", "csrc", "prcore.cu")]
+    csrc = os.path.join(src_root, "passiveradar_b200", "csrc")
+    sources = sorted(os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith(".cu"))
+    cmd = [b.find_nvcc()] + tree_flags(src_root) + ["-I", os.path.join(src_root, "include"), "-I", csrc,
+                                                    "-o", lib] + sources
     res = subprocess.run(cmd, capture_output=True, text=True)
     with open(os.path.join(out_dir, "ptxas.log"), "w") as f:
         f.write(res.stdout + res.stderr)
@@ -50,7 +62,8 @@ def cmd_build(args):
     rev = subprocess.run(["git", "-C", ROOT, "rev-parse", args.base], capture_output=True, text=True, check=True).stdout.strip()
     src_a = os.path.join(AB, "A", "src")
     os.makedirs(src_a, exist_ok=True)
-    tar = subprocess.run(["git", "-C", ROOT, "archive", rev, "passiveradar_b200/csrc", "include"], capture_output=True, check=True).stdout
+    tar = subprocess.run(["git", "-C", ROOT, "archive", rev, "passiveradar_b200/csrc", "passiveradar_b200/build.py",
+                          "include"], capture_output=True, check=True).stdout
     with tarfile.open(fileobj=io.BytesIO(tar)) as tf:
         tf.extractall(src_a, filter="data")
     compile_lib(src_a, os.path.join(AB, "A"))

@@ -36,7 +36,7 @@ SHAPES = [("main_int8", "int8", 5242880), ("main_interleaved_c64", "complex64", 
 
 
 def plan(n, nl):
-    """Transform length and pass count of the device path (csrc/prcore.cu chanoff_device, nd = 1)."""
+    """Transform length and pass count of the device path (csrc/prcore_signal.cu chanoff_device, nd = 1)."""
     nvalid = 2 * nl + 1
     p0 = -nl
     need = max(n, n, p0 + nvalid - 1 + n, n - p0, 2)

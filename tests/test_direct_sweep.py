@@ -6,7 +6,7 @@ chunk_sum_kernel + doppler_dft_kernel) and nlms_block_kernel<KT, NT>.  They are 
 filter below fft_min_n samples, every tap-weighted (shortFilt=False) or short-block (D < 32) CAF, every CAF of more
 than 3072 lags, and all of NLMS.
 
-A Python twin of the planners (prcore.cu: choose_geo, choose_stream, stream_pieces / stream_first_cta, the branches
+A Python twin of the planners (prcore_corr.cu: choose_geo, choose_stream, stream_pieces / stream_first_cta, the branches
 of xambg_device, doppler_stage, ls_device and nlms_device) states for every case which kernel runs with which
 tiling; the sweep is chosen from it so that every edge of the tiling is reached, CPU tests hold the twin's invariants
 and name a case per edge, and the GPU tests pin the twin to the library through the per-kernel launch counts of prc_profile_read.
@@ -28,7 +28,7 @@ from oracle import clutter_oracle as co
 from oracle import xambg_oracle as xo
 
 TOL = 1e-5
-TILE_I = TILE_D = 10                  # prcore.cu: register tile of the FP32 sliding-window kernels
+TILE_I = TILE_D = 10                  # prcore_corr.cu: register tile of the FP32 sliding-window kernels
 SMEM_LIMIT = 200 * 1024
 SMEM_SOFT = 100 * 1024                # the tile loops shrink a tile until it fits this, as long as they can
 FIR_THREADS = 128
@@ -44,7 +44,7 @@ class PlanError(ValueError):
     """The library refuses the shape (PRC_E_INVALID) with this message."""
 
 
-# ------------------------------------------------------------------ planner twin (prcore.cu)
+# ------------------------------------------------------------------ planner twin (prcore_corr.cu)
 @dataclass(frozen=True)
 class Geo:
     """choose_geo: lagcorr_kernel, one CTA per (block, chunk).  doublings: how often the nchunk loop halved the chunk
@@ -508,7 +508,7 @@ def test_sweep_reaches_every_edge(nsm):
 
 
 def test_twin_edges_sit_where_the_library_puts_them():
-    """Spot values of the branches, read off prcore.cu, so that an edit of the twin shows up here."""
+    """Spot values of the branches, read off prcore_corr.cu, so that an edit of the twin shows up here."""
     assert caf_direct(62 * 200 + 9, 20, 200, False, True, 132).kernel == "lagcorr"
     assert caf_direct(63 * 128, 20, 128, False, True, 132).kernel == "lagstream"
     assert caf_direct(63 * 128, 20, 128, False, False, 132).kernel == "lagcorr"      # taps: always lagcorr

@@ -1,4 +1,4 @@
-"""Host operands are staged through one path (prcore.cu stage_in / unstage): a host call on frames laid out wider than
+"""Host operands are staged through one path (prcore_host.h: stage_in / unstage): a host call on frames laid out wider than
 a frame gives the bits of the same call on device copies, and writes nothing into the caller's padding."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""Every kernel instantiation prcore.cu can launch, run against the suite's oracles and float64 truths.
+"""Every kernel instantiation prcore's host code can launch, run against the suite's oracles and float64 truths.
 
 Three parts:
 
@@ -8,7 +8,7 @@ Three parts:
   tests/test_gpu_parity.py.  Each oracle is computed once per module.
 * GPU cases for dispatches of the default configuration no other test reaches: NLMS with more than 1024 taps, the
   Doppler stage at F = 4096 .. 16384, the tap-weighted decimator at full size, and 5-frame CAF batches.
-* A CPU guard: every kernel launch site of prcore.cu must appear in COVERAGE with the GPU tests that reach it.
+* A CPU guard: every kernel launch site of the library's sources must appear in COVERAGE with the GPU tests that reach it.
 
 Per-case figures go to $PRC_PARITY_DIR/parity.json (tests/conftest.py:record_parity).
 """
@@ -21,11 +21,10 @@ import scipy.signal as signal
 
 import _golden as G
 from conftest import record_parity
-from passiveradar_b200 import _lib, synth
+from passiveradar_b200 import _lib, build, synth
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-PRCORE = os.path.join(ROOT, "passiveradar_b200", "csrc", "prcore.cu")
 TOL = 1e-5
 
 DIRECT = ["ls_big", "ls_small", "ls_wide", "toep", "caf_big", "caf_small", "frame"]
@@ -538,7 +537,7 @@ def test_xambg_frames_batch_matches_oracle(n, F, R):
 
 
 # ------------------------------------------------------------------ CPU guard: every launch site is covered
-# (host function, kernel<template arguments>) of every launch in prcore.cu -> [(test id, variant, what it reaches)].
+# (host function, kernel<template arguments>) of every launch in build.SOURCES -> [(test id, variant, what it reaches)].
 # The launches in the headers' own launchers are covered where those headers are tested: the front end's in
 # tests/test_recording.py, CFAR_2D's and the frame chain's in tests/test_render.py.
 # Variant: "default" (shipped configuration), or "fft" / "direct" (the both_paths fixture; "direct" also marks the
@@ -662,22 +661,23 @@ _FUNC_DEF = re.compile(r"^(?!(?:return|typedef|using|namespace|struct|enum|exter
 _LAUNCH = re.compile(r"([A-Za-z_][\w:]*)\s*(<[^<>;()]*>)?\s*<<<")
 
 
-def launch_sites(path=PRCORE):
-    """{'host function: kernel<template arguments>': [line numbers]} of every kernel launch in the file, including
-    the ones inside macros (PRC_R3_SWITCH, PRC_TRK_MEAS)."""
+def launch_sites(paths=build.SOURCES):
+    """{'host function: kernel<template arguments>': [(file, line number)]} of every kernel launch in the files,
+    including the ones inside macros (PRC_R3_SWITCH, PRC_TRK_MEAS)."""
     sites = {}
-    func = None
-    with open(path) as f:
-        for no, line in enumerate(f, 1):
-            m = _FUNC_DEF.match(line)
-            if m:
-                func = m.group(1)
-            code = line.split("//", 1)[0]
-            for k in _LAUNCH.finditer(code):
-                targs = ""
-                if k.group(2):
-                    targs = "<" + ", ".join(a.strip() for a in k.group(2)[1:-1].split(",")) + ">"
-                sites.setdefault(f"{func}: {k.group(1)}{targs}", []).append(no)
+    for path in paths:
+        func = None
+        with open(path) as f:
+            for no, line in enumerate(f, 1):
+                m = _FUNC_DEF.match(line)
+                if m:
+                    func = m.group(1)
+                code = line.split("//", 1)[0]
+                for k in _LAUNCH.finditer(code):
+                    targs = ""
+                    if k.group(2):
+                        targs = "<" + ", ".join(a.strip() for a in k.group(2)[1:-1].split(",")) + ">"
+                    sites.setdefault(f"{func}: {k.group(1)}{targs}", []).append((os.path.basename(path), no))
     return sites
 
 
@@ -691,14 +691,14 @@ def _is_gpu_test(test_id):
     return re.search(r"^pytestmark = pytest\.mark\.gpu$", src, re.M) is not None or "@pytest.mark.gpu" in decorators
 
 
-def test_every_prcore_launch_site_has_a_covering_gpu_test():
+def test_every_launch_site_of_the_library_sources_has_a_covering_gpu_test():
     sites = launch_sites()
     assert len(sites) == 39
     missing = sorted(set(sites) - set(COVERAGE))
     stale = sorted(set(COVERAGE) - set(sites))
-    assert not missing, "launch sites of prcore.cu without a covering test in COVERAGE: " + \
-        "; ".join(f"{s} (line {sites[s][0]})" for s in missing)
-    assert not stale, f"COVERAGE rows that are no launch site of prcore.cu: {stale}"
+    assert not missing, "launch sites without a covering test in COVERAGE: " + \
+        "; ".join(f"{s} ({sites[s][0][0]}, line {sites[s][0][1]})" for s in missing)
+    assert not stale, f"COVERAGE rows that are no launch site of the library's sources: {stale}"
     for site, reached in COVERAGE.items():
         assert reached, f"{site}: no test"
         for test_id, variant, _ in reached:
@@ -708,8 +708,12 @@ def test_every_prcore_launch_site_has_a_covering_gpu_test():
 
 def test_coverage_guard_sees_a_new_launch(tmp_path):
     """The guard fails for a launch it has not been told about."""
-    src = open(PRCORE).read()
-    scratch = tmp_path / "prcore.cu"
-    scratch.write_text(src + "\nint new_entry(Ctx* c) {\n    new_kernel<3><<<1, 32, 0, c->stream>>>();\n    return 0;\n}\n")
-    extra = set(launch_sites(str(scratch))) - set(COVERAGE)
+    paths = []
+    for path in build.SOURCES:
+        scratch = tmp_path / os.path.basename(path)
+        scratch.write_text(open(path).read())
+        paths.append(str(scratch))
+    with open(paths[-1], "a") as f:
+        f.write("\nint new_entry(Ctx* c) {\n    new_kernel<3><<<1, 32, 0, c->stream>>>();\n    return 0;\n}\n")
+    extra = set(launch_sites(paths)) - set(COVERAGE)
     assert extra == {"new_entry: new_kernel<3>"}

@@ -1,6 +1,6 @@
 """The channel-offset estimator and xcorr (csrc/chanoff.cuh) across their planner's edges.
 
-A plain-Python twin of prcore.cu's chanoff_device and of prc_channel_offset / prc_xcorr's argument handling gives, for
+A plain-Python twin of prcore_signal.cu's chanoff_device and of prc_channel_offset / prc_xcorr's argument handling gives, for
 any call, the lag mapping, the transform size and its passes, the decimator's chunking, the argmax grid and the launches
 the call makes.  On the CPU the twin is held to SciPy's 'valid' correlation and to oracle/offset_oracle.py, and a test
 names, for every edge of the plan, a sweep case that reaches it.  On the GPU every sweep case runs against a float64 /
@@ -16,8 +16,8 @@ import scipy.signal as signal
 from oracle import offset_oracle as oo
 
 PADLEN = 27                 # sosfiltfilt's default padlen
-MAX_ND = 64                 # prcore.cu CHANOFF_MAX_ND
-MAX_LOG2 = 26               # prcore.cu CHANOFF_MAX_LOG2
+MAX_ND = 64                 # prcore_signal.cu CHANOFF_MAX_ND
+MAX_LOG2 = 26               # prcore_signal.cu CHANOFF_MAX_LOG2
 TILE_BITS = 11              # chanoff.cuh FFT_TILE_BITS
 TW_LO_BITS = 11
 IIR_THREADS = 128
@@ -456,7 +456,7 @@ def test_twin_agrees_with_the_offset_oracle():
 
 
 def test_twin_edges_sit_where_the_library_puts_them():
-    """Spot values read off prcore.cu and chanoff.cuh, so that an edit of the twin shows up here."""
+    """Spot values read off prcore_signal.cu and chanoff.cuh, so that an edit of the twin shows up here."""
     assert [iir_plan(n, _sos(1, np.int8)).chunk for n in (4194250, 4194251)] == [256, 257]
     assert iir_plan(4194250, _sos(1, np.int8)).grid == 128 and iir_plan(100, _sos(1, np.int8)).grid == 1
     assert [argmax_blocks(v) for v in (1, 2048, 2049, 4096, 4097, 2097152, 2097153)] == [1, 1, 2, 2, 3, 1024, 1024]

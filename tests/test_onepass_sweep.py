@@ -1,4 +1,4 @@
-"""The one-pass FFT-domain frame (csrc/framepass.cuh, planned by prcore.cu's onepass_plan) across its planner, its
+"""The one-pass FFT-domain frame (csrc/framepass.cuh, planned by prcore_corr.cu's onepass_plan) across its planner, its
 segment limits, its batch chunks, its CTA walks, the Doppler stages it hands its rows to, and strided frame layouts.
 
 A Python twin of onepass_plan (built on test_path_sweep's ls_plan / caf_plan and the decimator's alignment) states for
@@ -41,7 +41,7 @@ def _model():
     return mod
 
 
-# ------------------------------------------------------------------ planner twin (prcore.cu: onepass_plan, frame_onepass)
+# ------------------------------------------------------------------ planner twin (prcore_corr.cu: onepass_plan, frame_onepass)
 @dataclass(frozen=True)
 class OnePlan:
     """on/off and why; bls (LS-only segment limit), Bmax (block segment limit); per Doppler block (lo, hi, ls_end,
@@ -96,7 +96,7 @@ def onepass_plan(n, F, filter_len, peek, R, fft_min_n=ps.FFT_MIN_N, floor=L // 4
 
 
 def doppler_kernel(F, R, nf, nsm):
-    """The Doppler stage's kernel for a chunk of nf frames (prcore.cu: doppler_stage)."""
+    """The Doppler stage's kernel for a chunk of nf frames (prcore_corr.cu: doppler_stage)."""
     if F >= 2 and F & (F - 1) == 0 and F <= 8192:
         if F <= 1024 and -(-(R + 1) // 8) * nf >= nsm:
             return "pow2<8>"

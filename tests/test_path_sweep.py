@@ -1,5 +1,5 @@
 """Sweeps of the FFT-domain hot path (csrc/fftcorr.cuh: lscorr_fft_kernel, levinson_kernel, taps_spectrum_kernel,
-fir_fft_kernel, caf_fft_kernel<R3, FUSED>) across the edges of the three host planners that choose it (prcore.cu:
+fir_fft_kernel, caf_fft_kernel<R3, FUSED>) across the edges of the three host planners that choose it (prcore_corr.cu:
 ls_fft_plan, caf_fft_plan with and without the fused clutter filter, fir_fft's segment count), against float64 truths.
 
 A Python twin of the planners states, for every case, which transform length and which segments the library uses; the
@@ -30,7 +30,7 @@ def rel(a, b, den):
     return float(np.abs(np.asarray(a) - np.asarray(b)).max() / den)
 
 
-# ------------------------------------------------------------------ planner twin (prcore.cu)
+# ------------------------------------------------------------------ planner twin (prcore_corr.cu)
 @dataclass(frozen=True)
 class LsPlan:
     """ls_fft_plan: on/off, R3, L = 256 R3, the segment bound L - M + 1, segment length Bs, segment count, length of

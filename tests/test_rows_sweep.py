@@ -79,7 +79,7 @@ def cfar_cells(gpu, want):
 def _acc_dtype():
     """The accumulator cfar_frames_kernel declares for its window sums."""
     src = open(DETECT).read()
-    kern = src[src.index("cfar_frames_kernel("):src.index("piece_sum_kernel")]
+    kern = src[src.index("cfar_frames_kernel("):src.index("// ---- launches")]
     acc = re.search(r"\b(float|double) acc = ", kern).group(1)
     racc = re.search(r"\b(float|double) racc = ", kern).group(1)
     assert acc == racc
@@ -111,7 +111,7 @@ def cfar_model(X, fw, gw, acc):
     return ((X.astype(acc) * inv_mean) / (total * scale + acc(1e-10))).astype(np.float32)
 
 
-def test_cfar_frames_summation_model_matches_float64_oracle():
+def test_cfar_frames_kernel_summation_model_matches_float64_oracle():
     acc = _acc_dtype()
     cases = [("rayleigh_256x301", rayleigh(256, 301, 1), 18, 4), ("rayleigh_256x301", rayleigh(256, 301, 1), 64, 10),
              ("ridge_256x301", clutter_ridge(256, 301, 2), 18, 4), ("ridge_256x301", clutter_ridge(256, 301, 2), 64, 3),
@@ -334,11 +334,11 @@ def test_resample_short_inputs(up, dn):
     record_parity(f"rows/resample_short_{up}_{dn}", E_vs_truth=worst)
 
 
-RS_SMEM_LIMIT = 200 * 1024          # SMEM_LIMIT of csrc/prcore.cu
+RS_SMEM_LIMIT = 200 * 1024          # SMEM_LIMIT of csrc/prcore_host.h
 
 
 def _resample_smem(up, dn):
-    """Shared memory the resampler asks for (csrc/prcore.cu: resample_geo, resample_table), reduced ratio."""
+    """Shared memory the resampler asks for (csrc/prcore_signal.cu: resample_geo, resample_table), reduced ratio."""
     g = math.gcd(up, dn)
     up, dn = up // g, dn // g
     half_len = 10 * max(up, dn)
