@@ -98,8 +98,8 @@ static c128 zconj(c128 a) { c128 r = {a.re, -a.im}; return r; }
 static c128 zsub(c128 a, c128 b) { c128 r = {a.re - b.re, a.im - b.im}; return r; }
 static c128 zadd(c128 a, c128 b) { c128 r = {a.re + b.re, a.im + b.im}; return r; }
 
-int gal_truth_c128(const c64* ref, const c64* srv, long n, int L, int D, double mu1, double mu2, int peek,
-                   c128* out, c128* k_out, c128* h_out)
+static int gal_truth_run(const c64* ref, const c64* srv, long n, int L, int D, double mu1, double mu2, int peek,
+                         c128* out, c128* k_out, c128* h_out, double* stats)
 {
     if (L < 1 || D < L || peek < 0) return -2;
     c128* st = (c128*)calloc((size_t)D * 5, sizeof(c128));
@@ -110,6 +110,8 @@ int gal_truth_c128(const c64* ref, const c64* srv, long n, int L, int D, double 
     int mu_py = 1;
     double mu_d = mu1;
     c128 mu_c = {0.0, 0.0};
+    long clamps = 0;
+    double margin = INFINITY, xr_max = 0.0;
     memset(out, 0, (size_t)n * sizeof(c128));
     for (long t = 0; t < n - peek - 1; ++t) {
         memcpy(bo, b, (size_t)D * sizeof(c128));
@@ -152,11 +154,38 @@ int gal_truth_c128(const c64* ref, const c64* srv, long n, int L, int D, double 
         double xr, xi;
         if (mu_py) { xr = 0.999 * mu_d + 1e-8 * e2.re; xi = 1e-8 * e2.im; }
         else { xr = 0.999 * mu_c.re + 1e-8 * e2.re; xi = 0.999 * mu_c.im + 1e-8 * e2.im; }
-        if (xr > 5e-3 || (xr == 5e-3 && xi > 0.0)) { mu_py = 1; mu_d = 5e-3; }
+        const double mg = fabs(xr - 5e-3) / 5e-3;
+        if (mg < margin) margin = mg;
+        if (fabs(xr) > xr_max) xr_max = fabs(xr);
+        if (xr > 5e-3 || (xr == 5e-3 && xi > 0.0)) { mu_py = 1; mu_d = 5e-3; ++clamps; }
         else { mu_py = 0; mu_c.re = xr; mu_c.im = xi; }
+    }
+    if (stats) {
+        stats[0] = (double)clamps;
+        stats[1] = margin;
+        stats[2] = xr_max;
+        stats[3] = mu_py ? mu_d : mu_c.re;
+        stats[4] = mu_py ? 0.0 : mu_c.im;
     }
     if (k_out) memcpy(k_out, k, (size_t)D * sizeof(c128));
     if (h_out) memcpy(h_out, h, (size_t)D * sizeof(c128));
     free(st); free(P);
     return 0;
+}
+
+int gal_truth_c128(const c64* ref, const c64* srv, long n, int L, int D, double mu1, double mu2, int peek,
+                   c128* out, c128* k_out, c128* h_out)
+{
+    return gal_truth_run(ref, srv, n, L, D, mu1, mu2, peek, out, k_out, h_out, NULL);
+}
+
+/* gal_truth_c128 (the same code path, so the same bits) that also reports on mu1's clamp, in stats[5]: the number of
+ * samples at which the clamp at 5e-3 won, the smallest |xr - 5e-3| / 5e-3 over all clamp decisions (INFINITY when
+ * there were none), the largest |xr|, and mu1 after the last sample (real and imaginary part; a real value when the
+ * clamp won last).  xr is the real part min() compares with 5e-3.  A complex64 evaluation of a decision whose margin
+ * is below its own rounding error can go the other way. */
+int gal_truth_stats_c128(const c64* ref, const c64* srv, long n, int L, int D, double mu1, double mu2, int peek,
+                         c128* out, c128* k_out, c128* h_out, double* stats)
+{
+    return gal_truth_run(ref, srv, n, L, D, mu1, mu2, peek, out, k_out, h_out, stats);
 }

@@ -546,6 +546,9 @@ def test_xambg_frames_batch_matches_oracle(n, F, R):
 PAR, FFT, KV = "tests/test_gpu_parity.py::", "tests/test_gpu_fft.py::", "tests/test_kernel_variants.py::"
 FE, GAL, TRK = "tests/test_gpu_frontend.py::", "tests/test_gal_jpe.py::", "tests/test_tracking.py::"
 RS = "tests/test_rows_sweep.py::"
+GS = "tests/test_gal_sweep.py::"
+GAL_SWEEP = GS + "test_gal_matches_truth_and_oracle"
+GAL_BATCH = GS + "test_gal_batch_is_bit_identical_to_single_frames_in_every_variant"
 PS = "tests/test_path_sweep.py::"
 DS = "tests/test_direct_sweep.py::"
 DIRECT_TEST = KV + "test_direct_form_matches_truth_and_reference"
@@ -639,11 +642,21 @@ COVERAGE = {
                                           (KV + "test_nlms_accepts_4096_taps_and_names_the_limit_above", "default", "M = 4096"),
         (DS + "test_nlms_at_the_tiling_edges", "default", "M = 2049, 4096 with initial taps"),
         (DS + "test_nlms_frames_past_the_sm_count_at_the_kt_edges", "default", "M = 2049: more frames than SMs, 1024-thread CTAs")],
-    "gal_device: gal_jpe_kernel<1, false>": [(GAL + "test_gal_edge_cases", "default", "D = 1")],
-    "gal_device: gal_jpe_kernel<2, false>": [(GAL + "test_gal_edge_cases", "default", "D = 40")],
-    "gal_device: gal_jpe_kernel<4, false>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 77")],
-    "gal_device: gal_jpe_kernel<8, false>": [(GAL + "test_gal_long_run_matches_c_oracle_and_truth", "default", "D = 185")],
-    "gal_device: gal_jpe_kernel<GAL_CTA_T, true>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 300, 4096")],
+    "gal_device: gal_jpe_kernel<1, false>": [(GAL + "test_gal_edge_cases", "default", "D = 1"),
+        (GAL_SWEEP, "default", "D = 1, 31, 32; 1, 31, 32, 33 sample steps; 2^19 samples at D = 32"),
+        (GAL_BATCH, "default", "D = 20: 1, 3, 4, 5 and more frames than the GPU holds")],
+    "gal_device: gal_jpe_kernel<2, false>": [(GAL + "test_gal_edge_cases", "default", "D = 40"),
+        (GAL_SWEEP, "default", "D = 33, 63, 64; 2^15 samples at D = 64"),
+        (GAL_BATCH, "default", "D = 50: 1, 3, 4, 5 and more frames than the GPU holds")],
+    "gal_device: gal_jpe_kernel<4, false>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 77"),
+        (GAL_SWEEP, "default", "D = 65, 127, 128; x3e4 at D = 100; 2^19 samples x1e-3 at D = 128"),
+        (GAL_BATCH, "default", "D = 100: 1, 3, 4, 5 and more frames than the GPU holds")],
+    "gal_device: gal_jpe_kernel<8, false>": [(GAL + "test_gal_long_run_matches_c_oracle_and_truth", "default", "D = 185"),
+        (GAL_SWEEP, "default", "D = 129, 255, 256; clamp held at D = 200, 255; 2^19 samples at D = 256"),
+        (GAL_BATCH, "default", "D = 200: 1, 3, 4, 5 and more frames than the GPU holds")],
+    "gal_device: gal_jpe_kernel<GAL_CTA_T, true>": [(GAL + "test_gal_shapes_match_c_oracle", "default", "D = 300, 4096"),
+        (GAL_SWEEP, "default", "D = 257 .. 4096, 2 .. 16 warps; 2^19 samples at 2 and 16 warps"),
+        (GAL_BATCH, "default", "D = 700 (3 warps): 1, 3, 4, 5 and more frames than the GPU holds")],
     "stage_window: f64_to_f32_kernel": [(PAR + "test_xambg_matches_live_oracle", "fft", "float64 window")],
     "prc_xambg_c64: f64_to_f32_kernel": [(PAR + "test_xambg_matches_reference_golden", "direct", "xambg_longfilt taps")],
     "trk_meas_launch: track_meas_kernel<T, TRK_MODE_MEAN>": [
