@@ -26,7 +26,9 @@
 //   tw1[k1 * T + t]   = W_L^{t k1}            (L entries)
 //   tw2[k2 * R3 + n3] = W_{16 R3}^{n3 k2}     (16 R3 entries)
 // Pass 1 / pass 3 take their twiddles from a source (Tw1Table: tw1 in shared memory; Tw1Seeds: five registers per
-// thread, for frame_pass_kernel, whose shared-memory pipe is its bottleneck and which then stages tw2 alone).
+// thread, for frame_pass_kernel, whose shared-memory pipe is its bottleneck and which then stages tw2 alone), and so
+// does pass 2 (Tw2Table: tw2 as above; Tw2Rows: tw2 staged as padded rows [n3][k2], read two twiddles per load, for
+// frame_pass_kernel).
 //
 // Every per-thread phase is a __host__ __device__ function of (registers, t, buffers): the same code is run
 // thread-by-thread on the CPU by scripts/fft/emul.cu and tests/test_fft_emulation.py to pin the index algebra
@@ -162,6 +164,40 @@ template <int R3> struct Tw1Seeds {
     }
 };
 
+// ---- twiddle sources of pass 2 (both directions): w[k2] = W_{16 R3}^{n3 k2}, k2 = 1..15 -------------------------
+// Tw2Table reads tw2[k2 R3 + n3]: 15 64-bit loads, each a broadcast of R3 distinct addresses.  Tw2Rows reads the same
+// values staged as rows [n3][k2] of STRIDE = 18 float2 (k2 = 0 holds W^0 = 1, k2 = 16, 17 are zero padding): one
+// 128-bit load per aligned pair (k2, k2 + 1), 8 instead of 15.  At R3 = 8 the 144-byte stride starts row n3 at bank
+// 4 n3, so the 8 rows of a warp's pair load cover the 32 banks once: one wavefront, as each 64-bit load of the table.
+template <int R3> struct Tw2Table {
+    static constexpr int FLOAT2 = Geo<R3>::TW2;
+    const float2* __restrict__ tw2;
+    PRC_HD void load(float2 (&w)[16], int n3) const {
+#pragma unroll
+        for (int k2 = 1; k2 < 16; ++k2) w[k2] = tw2[k2 * R3 + n3];
+    }
+    // entry i of the staged table from the global table tw2 [k2 R3 + n3]
+    static PRC_HD float2 staged(const float2* __restrict__ tw2, int i) { return tw2[i]; }
+};
+
+template <int R3> struct Tw2Rows {
+    static constexpr int STRIDE = 18, FLOAT2 = R3 * STRIDE;
+    const float2* __restrict__ rows;           // 16-byte aligned
+    PRC_HD void load(float2 (&w)[16], int n3) const {
+        const float4* row = reinterpret_cast<const float4*>(rows + n3 * STRIDE);
+#pragma unroll
+        for (int h = 0; h < 8; ++h) {
+            const float4 q = row[h];
+            if (h) w[2 * h] = make_float2(q.x, q.y);
+            w[2 * h + 1] = make_float2(q.z, q.w);
+        }
+    }
+    static PRC_HD float2 staged(const float2* __restrict__ tw2, int i) {
+        const int n3 = i / STRIDE, k2 = i - n3 * STRIDE;
+        return k2 < 16 ? tw2[k2 * R3 + n3] : make_float2(0.f, 0.f);
+    }
+};
+
 // ---- natural -> permuted -------------------------------------------------------------------------------------
 template <int R3, class Tw1 = Tw1Table<R3>>
 PRC_HD void n2p_pass1(float2 (&v)[16], int t, float2* __restrict__ ea, const Tw1& tw1) {
@@ -177,17 +213,15 @@ PRC_HD void n2p_pass1(float2 (&v)[16], int t, float2* __restrict__ ea, const Tw1
     for (int k1 = 1; k1 < 16; ++k1) dst[k1 * G::S] = cmul(v[k1], w[k1]);
 }
 
-template <int R3>
-PRC_HD void n2p_pass2(float2 (&v)[16], int t, const float2* __restrict__ ea, float2* __restrict__ eb,
-                      const float2* __restrict__ tw2) {
+template <int R3, class Tw2 = Tw2Table<R3>>
+PRC_HD void n2p_pass2(float2 (&v)[16], int t, const float2* __restrict__ ea, float2* __restrict__ eb, const Tw2& tw2) {
     using G = Geo<R3>;
     const int k1 = t / R3, n3 = t - k1 * R3;
     const float2* src = ea + k1 * G::S + n3;
 #pragma unroll
     for (int n2 = 0; n2 < 16; ++n2) v[n2] = src[n2 * R3];
     float2 w[16];
-#pragma unroll
-    for (int k2 = 1; k2 < 16; ++k2) w[k2] = tw2[k2 * R3 + n3];
+    tw2.load(w, n3);
     Dft<16>::run(v);
     float2* dst = eb + k1 * G::S + n3 * 17;
     dst[0] = v[0];
@@ -230,15 +264,13 @@ PRC_HD void p2n_pass1(float2 (&v)[16], int t, float2* __restrict__ eb) {
     }
 }
 
-template <int R3>
-PRC_HD void p2n_pass2(float2 (&v)[16], int t, const float2* __restrict__ eb, float2* __restrict__ ea,
-                      const float2* __restrict__ tw2) {
+template <int R3, class Tw2 = Tw2Table<R3>>
+PRC_HD void p2n_pass2(float2 (&v)[16], int t, const float2* __restrict__ eb, float2* __restrict__ ea, const Tw2& tw2) {
     using G = Geo<R3>;
     const int k1 = t / R3, n3 = t - k1 * R3;
     const float2* src = eb + k1 * G::S + n3 * 17;
     float2 w[16];
-#pragma unroll
-    for (int k2 = 1; k2 < 16; ++k2) w[k2] = tw2[k2 * R3 + n3];
+    tw2.load(w, n3);
 #pragma unroll
     for (int k2 = 0; k2 < 16; ++k2) v[k2] = src[k2];
 #pragma unroll
@@ -267,18 +299,19 @@ PRC_HD void p2n_pass3(float2 (&v)[16], int t, const float2* __restrict__ ea, con
 #ifdef __CUDACC__
 // Block-wide transforms: every thread of the group (blockDim.x == T) calls them; `sm` = [ea | eb | tw1 | tw2].
 template <int R3> struct Smem {
-    float2* ea; float2* eb; Tw1Table<R3> tw1; const float2* tw2;
+    float2* ea; float2* eb; Tw1Table<R3> tw1; Tw2Table<R3> tw2;
     __device__ __forceinline__ explicit Smem(float2* base)
-        : ea(base), eb(base + Geo<R3>::EX), tw1{base + 2 * Geo<R3>::EX}, tw2(base + 2 * Geo<R3>::EX + Geo<R3>::TW1) {}
+        : ea(base), eb(base + Geo<R3>::EX), tw1{base + 2 * Geo<R3>::EX}, tw2{base + 2 * Geo<R3>::EX + Geo<R3>::TW1} {}
 };
 
-// the same transforms with pass-1 / pass-3 twiddles from per-thread seeds: `sm` = [ea | eb | tw2], the seeds are read
-// from the global table [tw1 | tw2] (fft_twiddle_kernel's); the caller stages tw2 (stage_tw2) and synchronises
-template <int R3> struct SmemSeeded {
-    static constexpr int SMEM_FLOAT2 = 2 * Geo<R3>::EX + Geo<R3>::TW2;
-    float2* ea; float2* eb; Tw1Seeds<R3> tw1; const float2* tw2;
+// the same transforms with pass-1 / pass-3 twiddles from per-thread seeds: `sm` = [ea | eb | tw2 as Tw2 stages it],
+// the seeds are read from the global table [tw1 | tw2] (fft_twiddle_kernel's); the caller stages tw2 (stage_tw2) and
+// synchronises
+template <int R3, class Tw2 = Tw2Table<R3>> struct SmemSeeded {
+    static constexpr int SMEM_FLOAT2 = 2 * Geo<R3>::EX + Tw2::FLOAT2;
+    float2* ea; float2* eb; Tw1Seeds<R3> tw1; Tw2 tw2;
     __device__ __forceinline__ SmemSeeded(float2* base, const float2* __restrict__ tw_global, int t)
-        : ea(base), eb(base + Geo<R3>::EX), tw1(tw_global, t), tw2(base + 2 * Geo<R3>::EX) {}
+        : ea(base), eb(base + Geo<R3>::EX), tw1(tw_global, t), tw2{base + 2 * Geo<R3>::EX} {}
 };
 
 template <int R3, class Sm>
@@ -319,11 +352,11 @@ __device__ __forceinline__ void stage_twiddles(float2* base, const float2* __res
     for (int i = t; i < G::TW1 + G::TW2; i += G::T) dst[i] = tw_global[i];
 }
 
-// stage tw2 alone into SmemSeeded's layout; caller synchronises
-template <int R3>
+// stage tw2 alone into SmemSeeded<R3, Tw2>'s layout; caller synchronises
+template <int R3, class Tw2>
 __device__ __forceinline__ void stage_tw2(float2* base, const float2* __restrict__ tw_global, int t) {
     using G = Geo<R3>;
-    for (int i = t; i < G::TW2; i += G::T) base[2 * G::EX + i] = tw_global[G::TW1 + i];
+    for (int i = t; i < Tw2::FLOAT2; i += G::T) base[2 * G::EX + i] = Tw2::staged(tw_global + G::TW1, i);
 }
 
 // tw[0 .. L) = tw1, tw[L .. L + 16 R3) = tw2, evaluated in float64

@@ -23,10 +23,14 @@
 // ln - 1 + R + peek, so ln <= L - M - R - peek + 1.  W' keeps taps_spectrum_kernel's placement: Yr' starts M - 1 - peek
 // samples before Ys', exactly as R_seg starts before S in caf_fft_kernel.
 //
-// Registers: AccP, AccQ and the two held spectra Ys', Yr' stay in registers; accC and accX live in thread-private
-// shared memory (4 x 8 KB at R3 = 8).  The pass-1 / pass-3 twiddles come from five per-thread registers (fft::Tw1Seeds)
-// instead of the tw1 table: that takes 15 of each thread's 64-bit shared loads per transform off the shared-memory
-// pipe, which bounds this kernel, and 16 KB out of the layout, so a CTA has 93 184 B of shared memory and two fit in
+// Registers: accC, accX (summed over the CTA's whole run) and the two held spectra Ys', Yr' stay in registers; AccP and
+// AccQ (summed over one Doppler block) live in thread-private shared memory (2 x 16 KB at R3 = 8): a block's first
+// segment stores its products there, the middle ones add to them, and the last one adds its products to what it reads
+// and writes the sums to `acc` without storing them back, so a block of one segment never touches those slots.  (The
+// other way round every X_ls item paid a read-modify-write of accC and accX; this way a block of nseg segments pays
+// nseg - 1 reads and nseg - 1 writes.)  The shared-memory pipe bounds this kernel, so what it spares is what counts:
+// the pass-1 / pass-3 twiddles come from five per-thread registers (fft::Tw1Seeds) instead of the tw1 table, and pass 2
+// reads its twiddles two per load from padded rows (fft::Tw2Rows).  A CTA has 93 312 B of shared memory, and two fit in
 // an SM.
 #pragma once
 #include <cuda_runtime.h>
@@ -54,9 +58,10 @@ struct FramePassParams {
     const float2* tw;
 };
 
-// shared memory: [fft::SmemSeeded | staging L float2 | accC, accX 2 L float2 | window staging L float]
+// shared memory: [fft::SmemSeeded with tw2 rows | staging L float2 | AccP, AccQ 2 L float2 | window staging L float]
+template <int R3> using FpSmem = fft::SmemSeeded<R3, fft::Tw2Rows<R3>>;
 template <int R3> constexpr int framepass_smem_float2() {
-    return fft::SmemSeeded<R3>::SMEM_FLOAT2 + 3 * fft::Geo<R3>::L + fft::Geo<R3>::L / 2;
+    return FpSmem<R3>::SMEM_FLOAT2 + 3 * fft::Geo<R3>::L + fft::Geo<R3>::L / 2;
 }
 
 // a unit of a CTA's run: Doppler block u < F, else LS-only tail segment u - F
@@ -99,9 +104,9 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
     using G = fft::Geo<R3>;
     extern __shared__ __align__(16) float2 sm[];
     const int t = threadIdx.x;
-    const fft::SmemSeeded<R3> S(sm, p.tw, t);
-    float2* stg = sm + fft::SmemSeeded<R3>::SMEM_FLOAT2;
-    float2* accs = stg + G::L;                                   // accC [r T + t], accX [L + r T + t]
+    const FpSmem<R3> S(sm, p.tw, t);
+    float2* stg = sm + FpSmem<R3>::SMEM_FLOAT2;
+    float2* accs = stg + G::L;                                   // AccP [r T + t], AccQ [L + r T + t]
     float* wst = reinterpret_cast<float*>(accs + 2 * G::L);
     const float2* ref = p.ref + (size_t)blockIdx.y * p.frame_stride;
     const float2* srv = p.srv + (size_t)blockIdx.y * p.frame_stride;
@@ -127,14 +132,12 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
         cp_async_commit();
     };
     if (cu < u1) issue(cu, cg, 0, 0);
-    fft::stage_tw2<R3>(sm, p.tw, t);
-#pragma unroll
-    for (int r = 0; r < 16; ++r) accs[r * G::T + t] = accs[G::L + r * G::T + t] = make_float2(0.f, 0.f);
+    fft::stage_tw2<R3, fft::Tw2Rows<R3>>(sm, p.tw, t);
     __syncthreads();
 
-    float2 accP[16], accQ[16], ys[16], yr[16], v[16];
+    float2 accC[16], accX[16], ys[16], yr[16], v[16];
 #pragma unroll
-    for (int r = 0; r < 16; ++r) accP[r] = accQ[r] = ys[r] = yr[r] = make_float2(0.f, 0.f);
+    for (int r = 0; r < 16; ++r) accC[r] = accX[r] = ys[r] = yr[r] = make_float2(0.f, 0.f);
 #pragma unroll 1
     while (cu < u1) {
         const int i0 = cg.lo + cq * cg.Bs;
@@ -171,9 +174,9 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
             fetch_staged<G::T, true>(v, stg, t, G::L);
         }
         fft::fft_n2p<R3>(v, t, S, [&] { if (nu < u1 && !(nk == 2)) issue(nu, ng, nq, nk); });
-        // Ys', Yr', AccP and AccQ are updated by selects in place, not by assignments on separate branches: with
-        // branches ptxas kept each array in two register sets and copied it back and forth on every item
-        // (~100 MOV per item; without them the frame pass at C2 takes 8 % less time)
+        // Ys', Yr', accC and accX are updated in place, not by assignments on separate branches: with branches ptxas
+        // kept each array in two register sets and copied it back and forth on every item (~100 MOV per item; without
+        // them the frame pass at C2 takes 8 % less time)
         if (ck < 2) {
 #pragma unroll
             for (int r = 0; r < 16; ++r) {
@@ -183,31 +186,30 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
         } else if (ck == 2) {
 #pragma unroll
             for (int r = 0; r < 16; ++r) {
-                float2 c = accs[r * G::T + t], x = accs[G::L + r * G::T + t];
-                cmacc(c, v[r], yr[r]);                                   // accC += X_ls conj(Yr')
-                cmacc(x, v[r], ys[r]);                                   // accX += X_ls conj(Ys')
-                accs[r * G::T + t] = c;
-                accs[G::L + r * G::T + t] = x;
+                cmacc(accC[r], v[r], yr[r]);                             // accC += X_ls conj(Yr')
+                cmacc(accX[r], v[r], ys[r]);                             // accX += X_ls conj(Ys')
             }
         } else {
+            // AccP += X_caf conj(Ys'), AccQ += X_caf conj(Yr'), from zero on the block's first segment; its last
+            // segment writes the sums out
+            const bool first = cq == 0, last = cq + 1 == cg.nseg;
+            float2* dst = p.acc + ((size_t)blockIdx.y * p.F + cu) * 2 * G::L;
 #pragma unroll
             for (int r = 0; r < 16; ++r) {
-                cmacc(accQ[r], v[r], yr[r]);                             // AccQ += X_caf conj(Yr')
-                cmacc(accP[r], v[r], ys[r]);                             // AccP += X_caf conj(Ys')
-            }
-            const bool last = cq + 1 == cg.nseg;                          // the block's last segment: write its sums
-            if (last) {
-                float2* dst = p.acc + ((size_t)blockIdx.y * p.F + cu) * 2 * G::L;
-#pragma unroll
-                for (int r = 0; r < 16; ++r) {
-                    dst[r * G::T + t] = accP[r];
-                    dst[G::L + r * G::T + t] = accQ[r];
+                float2 a = make_float2(0.f, 0.f), b = make_float2(0.f, 0.f);
+                if (!first) {
+                    a = accs[r * G::T + t];
+                    b = accs[G::L + r * G::T + t];
                 }
-            }
-#pragma unroll
-            for (int r = 0; r < 16; ++r) {
-                accP[r] = last ? make_float2(0.f, 0.f) : accP[r];
-                accQ[r] = last ? make_float2(0.f, 0.f) : accQ[r];
+                cmacc(b, v[r], yr[r]);
+                cmacc(a, v[r], ys[r]);
+                if (last) {
+                    dst[r * G::T + t] = a;
+                    dst[G::L + r * G::T + t] = b;
+                } else {
+                    accs[r * G::T + t] = a;
+                    accs[G::L + r * G::T + t] = b;
+                }
             }
         }
         if (nu != cu) cg = ng;
@@ -218,7 +220,7 @@ __global__ void __launch_bounds__(16 * R3, framepass_min_ctas<R3>()) frame_pass_
 #pragma unroll 1
     for (int w = 0; w < 2; ++w) {
 #pragma unroll
-        for (int r = 0; r < 16; ++r) v[r] = accs[w * G::L + r * G::T + t];
+        for (int r = 0; r < 16; ++r) v[r] = w ? accX[r] : accC[r];
         fft::fft_p2n<R3>(v, t, S);
         float2* row = p.partial + ((size_t)(blockIdx.y * 2 + w) * gridDim.x + blockIdx.x) * p.HT;
         const int sh = w ? 0 : off;
