@@ -53,9 +53,11 @@ typedef struct prc_c64 { float re, im; } prc_c64;
 /* flags */
 #define PRC_FLAG_ASYNC        1u   /* do not synchronise `stream` before returning */
 #define PRC_FLAG_WINDOW_F32   2u   /* `window` points at float, not double */
-#define PRC_FLAG_ABS_C64      4u   /* prc_cfar2d_f32: `x` is a complex64 map, |x| is used */
+#define PRC_FLAG_ABS_C64      4u   /* prc_cfar2d_f32, prc_cfar2d_frames, prc_os_cfar2d_frames: `x` is a complex64 map,
+                                    * |x| is used */
 #define PRC_FLAG_MAP_F64      8u   /* tracker entry points, prc_persistence_frames: maps are float64, not float32 */
-#define PRC_FLAG_CR_F64      16u   /* prc_cfar2d_frames: cr_out receives the float64 CR, not its float32 rounding */
+#define PRC_FLAG_CR_F64      16u   /* prc_cfar2d_frames, prc_os_cfar2d_frames: cr_out receives the float64 CR, not its
+                                    * float32 rounding */
 #define PRC_FLAG_PROD_F32    32u   /* prc_persistence_frames: float32 products float32(x) * float32(w) */
 #define PRC_FLAG_ORIENT      64u   /* prc_persistence_frames: frames are written as fliplr(P.T) */
 #define PRC_FLAG_TRACK_RESUME 128u /* tracker entry points: continue from the frame-0 records of `history` */
@@ -350,6 +352,25 @@ int prc_persistence_frames(const void* x, int rows, int cols, int nframes, int64
 int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t frame_stride, const double* q,
                            const double* scale, int nq, double* out, int mem_kind, int device, void* stream,
                            unsigned flags);
+
+/* ---- ordered-statistic CFAR (Rohling) ----------------------------------------------------------------------------
+ * prc_os_cfar2d_frames: CFAR_2D's detector with the window's k-th smallest cell as the noise estimate, for nframes maps
+ *   in one launch (not in the reference).  The window is exactly the cells CFAR_2D sums (its Tfilt, guard hole and
+ *   'same' / wrap placement, quirks included); N = their count (299 at fw = 18, gw = 4).  For cell (i, j):
+ *     T  = the k-th smallest of the N window values, 1 <= k <= N (signed values of a real map; hypotf(re, im) of a
+ *          complex64 map with PRC_FLAG_ABS_C64)
+ *     CR = (x[i, j] * inv_mean) / (T + 1e-10) in float64, with x[i, j] (its sign kept; |x| of a complex map) and
+ *          inv_mean = rows*cols / sum|x| formed exactly as prc_cfar2d_frames forms them: the two differ only in the
+ *          denominator.
+ *   Map b at x + b*frame_stride elements (float32, or complex64 with PRC_FLAG_ABS_C64), its CR at cr_out + b*cr_stride
+ *   elements: the float32 rounding of the float64 CR, or with PRC_FLAG_CR_F64 the float64 CR.  A frame's CR does not
+ *   depend on nframes.  Maps must be finite.
+ *   x and cr_out are DEVICE pointers (no mem_kind; callers stage host arrays themselves).
+ *   Limits (PRC_E_INVALID, naming the limit, before any CUDA call): prc_cfar2d_frames's (1 <= fw <= 64, fw^2 != gw^2,
+ *   rows <= 524 280, nframes <= 65535, strides >= rows*cols when nframes > 1), N >= 1 and 1 <= k <= N.
+ */
+int prc_os_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int fw, int gw, int k,
+                         void* cr_out, int64_t cr_stride, int device, void* stream, unsigned flags);
 
 /* ---- Kalman target trackers ------------------------------------------------------------------------
  * Replace get_measurements(), multitarget_tracker() and simple_target_tracker(), reference

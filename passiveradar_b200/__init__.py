@@ -16,7 +16,7 @@ from .clutter_removal import (LS_Filter, NLMS_filter, block_NLMS,            # n
 from .signal_utils import (deinterleave_IQ, frequency_shift, resample, frontend,            # noqa: F401
                            find_channel_offset, offset_compensation, shift, xcorr, decimate,
                            channel_preprocessing, normalize)
-from .target_detection import (CFAR_2D, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
+from .target_detection import (CFAR_2D, OS_CFAR_2D, os_cfar_frames, get_measurements, multitarget_tracker, simple_target_tracker,  # noqa: F401
                                multitarget_tracker_frames, simple_tracker_frames, cfar_track, TrackerPipeline,
                                kalman_filter_dtype, target_track_dtype, target_track_dtype_simple)
 from .recording import RecordingPipeline                                     # noqa: F401
@@ -26,7 +26,7 @@ from .spectrum import psd, psd_frames, SignalPreview                         # n
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
            "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
            "find_channel_offset", "offset_compensation", "shift", "xcorr", "decimate", "channel_preprocessing",
-           "normalize", "CFAR_2D",
+           "normalize", "CFAR_2D", "OS_CFAR_2D", "os_cfar_frames",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
            "simple_tracker_frames", "cfar_track", "TrackerPipeline", "RecordingPipeline", "persistence", "persistence_frames",
            "RenderPipeline", "psd", "psd_frames", "SignalPreview"]

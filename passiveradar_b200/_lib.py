@@ -99,6 +99,8 @@ SIGNATURES = {
                                  C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_cfar2d_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                     C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_os_cfar2d_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int,
+                                       C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_uint]),
     "prc_persistence_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_percentiles_frames": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,

@@ -30,7 +30,7 @@ const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply"
                                            "chanoff_fft", "chanoff_argmax", "svd_corr", "svd_eig", "svd_fir",
                                            "caf_combine", "frontend_chunks", "cfar_frames",
                                            "persistence", "percentile", "psd_segments", "psd_finish",
-                                           "decimate", "norm_sum", "norm_scale"};
+                                           "decimate", "norm_sum", "norm_scale", "os_cfar"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};

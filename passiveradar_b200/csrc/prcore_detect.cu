@@ -1,5 +1,5 @@
-// prcore_detect.cu -- detection and tracking in libprcore.so: CFAR_2D (single map and frames), the frame chain's
-// persistence and percentiles, and the Kalman trackers; their launches and C entry points.
+// prcore_detect.cu -- detection and tracking in libprcore.so: CFAR_2D (single map and frames), the ordered-statistic
+// CFAR, the frame chain's persistence and percentiles, and the Kalman trackers; their launches and C entry points.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -9,6 +9,7 @@
 
 #include "prcore_host.h"
 #include "detect.cuh"
+#include "oscfar.cuh"
 #include "render.cuh"
 
 namespace prcore {
@@ -62,6 +63,13 @@ int cfar_frames_device(Ctx* c, KernelId kid, CfarParams& p, int nframes) {
         launch_cfar(p, nframes, c->stream);
     }
     return check_launch("cfar_frames_kernel");
+}
+
+// ---- ordered-statistic CFAR (oscfar.cuh) ---------------------------------------------------------------
+// the cells of CFAR_2D's window: fw^2 minus the guard hole [e1, e2)^2 (empty when e2 <= e1)
+int os_cells(const CfarParams& p) {
+    const int hole = std::max(0, p.e2 - p.e1);
+    return p.fw * p.fw - hole * hole;
 }
 
 // ---- Kalman trackers (track.cuh) -----------------------------------------------------------------
@@ -256,6 +264,43 @@ int prc_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t fr
     p.cr_f64 = f64 ? 1 : 0;
     TRY(cfar_frames_device(c, K_CFAR_FRAMES, p, nframes));
     TRY(unstage(c, cr_out, p.cr, mem_kind, nframes, cells * oute, os * oute, flags));
+    return finish(c, flags);
+}
+
+int prc_os_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int fw, int gw, int k,
+                         void* cr_out, int64_t cr_stride, int device, void* stream, unsigned flags) {
+    if (!x || !cr_out) return fail(PRC_E_INVALID, "x and cr_out must not be NULL");
+    oscfar::OsParams p;
+    TRY(cfar_window(rows, cols, fw, gw, &p.c));
+    if (nframes < 0 || nframes > 65535) return fail(PRC_E_INVALID, "nframes=%d outside [0, 65535]", nframes);
+    const long long cells = (long long)rows * cols;
+    if (nframes > 1 && (frame_stride < cells || cr_stride < cells))
+        return fail(PRC_E_INVALID, "frame_stride=%lld / cr_stride=%lld smaller than the %lld cells of a map",
+                    (long long)frame_stride, (long long)cr_stride, cells);
+    const int n = os_cells(p.c);
+    if (n < 1) return fail(PRC_E_INVALID, "fw=%d gw=%d: the guard hole covers the whole window (N = 0 cells)", fw, gw);
+    if (k < 1 || k > n) return fail(PRC_E_INVALID, "k=%d outside [1, N = %d], the cells of the fw=%d gw=%d window", k, n,
+                                    fw, gw);
+    p.k = k;
+    p.h0 = p.c.e1;
+    p.h1 = std::max(p.c.e1, p.c.e2);
+    p.c.x = x;
+    p.c.is_complex = (flags & PRC_FLAG_ABS_C64) ? 1 : 0;
+    p.c.cr = cr_out;
+    p.c.cr_f64 = (flags & PRC_FLAG_CR_F64) ? 1 : 0;
+    p.c.frame_stride = nframes > 1 ? frame_stride : cells;
+    p.c.out_stride = nframes > 1 ? cr_stride : cells;
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    if (nframes == 0) return finish(c, flags);
+    TRY(c->rd_part.ensure((size_t)nframes * CFAR_MEAN_CTAS * sizeof(double)));
+    p.c.partial = c->rd_part.as<double>();
+    {
+        ProfScope ps(c, K_OS_CFAR);
+        oscfar::launch_os_cfar(p, nframes, c->stream);
+    }
+    TRY(check_launch("os_select_kernel"));
     return finish(c, flags);
 }
 

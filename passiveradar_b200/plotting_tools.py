@@ -79,6 +79,41 @@ def _np_dtype(t):
     return {torch.float32: np.float32, torch.float64: np.float64}[t.dtype]
 
 
+def _cfar_choice(cfar, os_rank, fw, gw):
+    """The pipelines' cfar / os_rank options -> (cfar, k): k is the ordered-statistic rank, None for CFAR_2D."""
+    if cfar not in ("ca", "os"):
+        raise ValueError(f"cfar must be 'ca' (CFAR_2D) or 'os' (OS_CFAR_2D), got {cfar!r}")
+    if cfar == "ca":
+        if os_rank is not None:
+            raise ValueError("os_rank applies to cfar='os' only")
+        return cfar, None
+    from .target_detection import os_rank as rank, os_window_cells
+    if not (1 <= fw <= 64) or gw < 0 or fw * fw == gw * gw:
+        raise ValueError(f"fw={fw} gw={gw}: OS_CFAR_2D needs 1 <= fw <= 64, gw >= 0 and fw != gw")
+    n = os_window_cells(fw, gw)
+    k = rank(fw, gw, os_rank)
+    if not 1 <= k <= n:
+        raise ValueError(f"os_rank={k} outside [1, N = {n}], the cells of the fw={fw} gw={gw} window")
+    return cfar, k
+
+
+def _cfar_frames_into(lib, cfar, k, maps_d, cf, fw, gw, dev, stream):
+    """The float64 CR of every map of maps_d (T compact complex64 / float32 device maps) into cf (T maps): CFAR_2D
+    (prc_cfar2d_frames) or, with cfar == "os", the ordered-statistic CFAR of rank k (prc_os_cfar2d_frames)."""
+    import torch
+    T, F, R1 = maps_d.shape
+    cells = F * R1
+    flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if maps_d.dtype == torch.complex64 else 0)
+    for t0 in range(0, T, MAX_CFAR_FRAMES):
+        nb = min(MAX_CFAR_FRAMES, T - t0)
+        if cfar == "os":
+            _lib.check(lib.prc_os_cfar2d_frames(maps_d[t0].data_ptr(), F, R1, nb, cells, fw, gw, k,
+                                                cf[t0].data_ptr(), cells, dev, stream, flags))
+        else:
+            _lib.check(lib.prc_cfar2d_frames(maps_d[t0].data_ptr(), F, R1, nb, cells, fw, gw,
+                                             cf[t0].data_ptr(), cells, _lib.MEM_DEVICE, dev, stream, flags))
+
+
 def _frames_for(prod, dtype):
     """The dtype the kernel reads a stack in: float32 when the products are float32 (exact for every dtype that
     promotes to them), else the stack's own float dtype, float64 for integers."""
@@ -177,10 +212,14 @@ class RenderPipeline:
     ``run_device`` takes (T, F, R+1) complex64 or float32 CUDA tensors (``RecordingPipeline.run_device`` /
     ``FramePipeline.run_device`` output) and carries the last hold - 1 CFAR frames to the next call, so a stack cut
     into batches of any size renders bit-identically to one call; ``reset()`` starts a new sequence.  ``run`` takes
-    main.py's host layout (F, R+1, nframes)."""
+    main.py's host layout (F, R+1, nframes).
 
-    def __init__(self, fw=18, gw=4, hold=20, decay=0.90, *, device=None, batch=64):
+    ``cfar="os"`` replaces CFAR_2D by the ordered-statistic CFAR on the same window (``OS_CFAR_2D``): the k-th smallest
+    window cell, k = ``os_rank`` or ceil(3N / 4), is the noise estimate instead of the window mean."""
+
+    def __init__(self, fw=18, gw=4, hold=20, decay=0.90, *, device=None, batch=64, cfar="ca", os_rank=None):
         self.fw, self.gw, self.hold, self.decay = int(fw), int(gw), int(hold), decay
+        self.cfar, self.os_rank = _cfar_choice(cfar, os_rank, self.fw, self.gw)
         if self.hold < 1:
             raise ValueError("hold must be >= 1")
         if int(batch) < 1:
@@ -226,12 +265,8 @@ class RenderPipeline:
         cf = torch.empty((nc + T, F, R1), dtype=torch.float64, device=maps_d.device)
         if nc:
             cf[:nc] = self._carry
-        flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if maps_d.dtype == torch.complex64 else 0)
         cells = F * R1
-        for t0 in range(0, T, MAX_CFAR_FRAMES):
-            nb = min(MAX_CFAR_FRAMES, T - t0)
-            _lib.check(lib.prc_cfar2d_frames(maps_d[t0].data_ptr(), F, R1, nb, cells, self.fw, self.gw,
-                                             cf[nc + t0].data_ptr(), cells, _lib.MEM_DEVICE, dev, stream, flags))
+        _cfar_frames_into(lib, self.cfar, self.os_rank, maps_d, cf[nc:], self.fw, self.gw, dev, stream)
         _lib.check(lib.prc_persistence_frames(cf.data_ptr(), F, R1, T, cells, nc, self.hold, self.weights.ctypes.data,
                                               data.data_ptr(), _lib.MEM_DEVICE, dev, stream,
                                               _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64 | _lib.FLAG_ORIENT))

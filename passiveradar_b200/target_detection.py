@@ -40,6 +40,101 @@ def CFAR_2D(X, fw, gw, thresh=None, *, device=None):
     return det.astype(bool)
 
 
+# ---------------------------------------------------------------------------------------------- ordered-statistic CFAR
+MAX_OS_FRAMES = 65535          # frames of one prc_os_cfar2d_frames call
+
+
+def os_window_cells(fw, gw):
+    """N, the cells of CFAR_2D's window (fw x fw minus the reference's guard hole, NumPy slice rules)."""
+    T = np.ones((fw, fw), dtype=np.int64)
+    e1 = (fw - gw) // 2
+    e2 = fw - e1 + 1
+    T[e1:e2, e1:e2] = 0
+    return int(T.sum())
+
+
+def os_rank(fw, gw, k=None):
+    """The rank OS_CFAR_2D uses: k, or ceil(3N / 4) when k is None.  Out-of-range windows and ranks are left for the
+    library to refuse with its message."""
+    if k is not None:
+        return int(k)
+    fw, gw = int(fw), int(gw)
+    if not (1 <= fw <= 64 and gw >= 0):
+        return 1
+    return -(-3 * os_window_cells(fw, gw) // 4)
+
+
+def _os_launch(x, rows, cols, nframes, fw, gw, k, out, flags, dev, stream):
+    """prc_os_cfar2d_frames over device tensors x (nframes compact float32 / complex64 maps) -> out (float64)."""
+    lib = _lib.load()
+    cells = rows * cols
+    for t0 in range(0, nframes, MAX_OS_FRAMES):
+        nb = min(MAX_OS_FRAMES, nframes - t0)
+        _lib.check(lib.prc_os_cfar2d_frames(x[t0].data_ptr(), rows, cols, nb, cells, fw, gw, k, out[t0].data_ptr(),
+                                            cells, dev, stream, flags))
+
+
+def OS_CFAR_2D(X, fw, gw, k=None, thresh=None, *, device=None):
+    '''ordered-statistic constant false alarm rate target detection (Rohling) on CFAR_2D's window
+
+    Parameters:
+        fw: CFAR kernel width
+        gw: number of guard cells
+        k: rank of the noise estimate among the N window cells, 1 <= k <= N (default ceil(3N / 4))
+        thresh: detection threshold
+
+    Returns:
+        (X / mean|X|) / (k-th smallest window cell + 1e-10) as float64; bool array when ``thresh`` is given'''
+    import torch
+    X = np.asarray(X)
+    if X.ndim != 2:
+        raise ValueError("X must be two-dimensional")
+    if np.iscomplexobj(X):
+        raise TypeError("OS_CFAR_2D expects a real map (the reference is called with np.abs(xambg))")
+    x = np.ascontiguousarray(X, dtype=np.float32)
+    rows, cols = x.shape
+    fw, gw = int(fw), int(gw)
+    dev = _lib.current_device() if device is None else int(device)
+    tdev = torch.device("cuda", dev)
+    xd = torch.from_numpy(x).to(tdev)[None]
+    cr = torch.empty((1, rows, cols), dtype=torch.float64, device=tdev)
+    with torch.cuda.device(tdev):
+        _os_launch(xd, rows, cols, 1, fw, gw, os_rank(fw, gw, k), cr, _lib.FLAG_CR_F64, dev,
+                   torch.cuda.current_stream(tdev).cuda_stream or 1)
+    out = cr[0].cpu().numpy()
+    return out if thresh is None else out > thresh
+
+
+def os_cfar_frames(stack, fw, gw, k=None, *, device=None):
+    '''OS_CFAR_2D of every frame of a (T, rows, cols) float32 or complex64 stack (complex maps: their magnitude) in one
+    launch per 65 535 frames.  A host array gives a host float64 CR stack; a CUDA tensor gives a float64 CUDA tensor,
+    ordered on the current torch stream.  Frame b's CR is bit-identical to a one-frame call on it.'''
+    import torch
+    host = not (hasattr(stack, "is_cuda") and stack.is_cuda)
+    if host:
+        a = np.asarray(stack)
+        if a.dtype not in (np.float32, np.complex64):
+            raise TypeError(f"stack must be float32 or complex64, got {a.dtype}")
+        dev = _lib.current_device() if device is None else int(device)
+        t = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", dev))
+    else:
+        if stack.dtype not in (torch.float32, torch.complex64):
+            raise TypeError(f"stack must be float32 or complex64, got {stack.dtype}")
+        t = stack.contiguous()
+        dev = t.device.index if device is None else int(device)
+    if t.dim() != 3:
+        raise ValueError(f"stack must be three-dimensional (T, rows, cols), got {t.dim()} dimensions")
+    T, rows, cols = t.shape
+    fw, gw = int(fw), int(gw)
+    out = torch.empty((T, rows, cols), dtype=torch.float64, device=t.device)
+    flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if t.dtype == torch.complex64 else 0)
+    if T:
+        with torch.cuda.device(t.device):
+            _os_launch(t, rows, cols, T, fw, gw, os_rank(fw, gw, k), out, flags, dev,
+                       torch.cuda.current_stream(t.device).cuda_stream or 1)
+    return out.cpu().numpy() if host else out
+
+
 # ---------------------------------------------------------------------------------------------- Kalman trackers
 # The reference's record dtypes (target_detection.py:9-17, :151-162, :530-537) with np.float -> float64 and
 # np.int -> int64 (the aliases NumPy >= 1.24 removed).  Packed, every field 8 bytes: the C structs prc_kalman,
@@ -313,11 +408,14 @@ class TrackerPipeline:
     The trackers read the float64 CF itself, as the scripts do.  ``run_device`` carries the last tracker records
     (continued with PRC_FLAG_TRACK_RESUME) and the last hold - 1 CF frames to the next call, so a stack cut into
     batches of any size, one map per call included, gives the same bytes as one call; ``reset()`` starts a new
-    sequence.  ``run`` takes the scripts' host layout (F, R+1, nframes).  Plotting stays with the caller."""
+    sequence.  ``run`` takes the scripts' host layout (F, R+1, nframes).  Plotting stays with the caller.
+
+    ``cfar="os"`` replaces CFAR_2D by the ordered-statistic CFAR on the same window (``OS_CFAR_2D``, rank ``os_rank``
+    or ceil(3N / 4)); the trackers and the phosphor frames then read its CR."""
 
     def __init__(self, max_range, max_doppler, *, tracker="multi", n_tracks=10, fw=18, gw=4, hold=20, decay=0.90,
-                 render=True, batch=64, device=None):
-        from .plotting_tools import _decay_plan
+                 render=True, batch=64, device=None, cfar="ca", os_rank=None):
+        from .plotting_tools import _cfar_choice, _decay_plan
         if tracker not in ("multi", "simple"):
             raise ValueError(f"tracker must be 'multi' or 'simple', got {tracker!r}")
         self.tracker = tracker
@@ -328,6 +426,7 @@ class TrackerPipeline:
         self.fw, self.gw, self.hold, self.decay = int(fw), int(gw), int(hold), decay
         if not (1 <= self.fw <= 64) or self.gw < 0 or self.fw * self.fw == self.gw * self.gw:
             raise ValueError(f"fw={fw} gw={gw}: CFAR_2D needs 1 <= fw <= 64, gw >= 0 and fw != gw")
+        self.cfar, self.os_rank = _cfar_choice(cfar, os_rank, self.fw, self.gw)
         if self.hold < 1:
             raise ValueError("hold must be >= 1")
         if int(batch) < 1:
@@ -375,7 +474,7 @@ class TrackerPipeline:
         * with render=True: ``data`` (T, R+1, F) float64 and ``limits`` (T, 2) = [vmin, vmax], as
           ``RenderPipeline.run_device`` gives them."""
         import torch
-        from .plotting_tools import MAX_CFAR_FRAMES, PERCENTILES, VMAX_SCALE, _stream_arg
+        from .plotting_tools import PERCENTILES, VMAX_SCALE, _cfar_frames_into, _stream_arg
         if not (_is_tensor(maps_d) and maps_d.is_cuda and maps_d.dim() == 3):
             raise TypeError("maps_d must be a (T, F, R+1) CUDA tensor")
         if maps_d.dtype not in (torch.complex64, torch.float32):
@@ -405,11 +504,7 @@ class TrackerPipeline:
         cf = torch.empty((nc + T, F, R1), dtype=torch.float64, device=tdev)
         if nc:
             cf[:nc] = self._carry
-        flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if maps_d.dtype == torch.complex64 else 0)
-        for t0 in range(0, T, MAX_CFAR_FRAMES):
-            nb = min(MAX_CFAR_FRAMES, T - t0)
-            _lib.check(lib.prc_cfar2d_frames(maps_d[t0].data_ptr(), F, R1, nb, cells, self.fw, self.gw,
-                                             cf[nc + t0].data_ptr(), cells, _lib.MEM_DEVICE, dev, stream, flags))
+        _cfar_frames_into(lib, self.cfar, self.os_rank, maps_d, cf[nc:], self.fw, self.gw, dev, stream)
         hist = out["history"]
         flags = _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64
         if self._state is not None:
