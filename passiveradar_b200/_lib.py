@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import sys
 import threading
 
 import numpy as np
@@ -243,13 +244,62 @@ def profile_read():
     return out
 
 
-def current_device() -> int:
-    """Device used by the drop-in operators: PRC_DEVICE, else LOCAL_RANK (torchrun), else 0."""
+def current_device(device=None) -> int:
+    """Device used by the drop-in operators: ``device`` when given, else PRC_DEVICE, else LOCAL_RANK (torchrun), else 0."""
+    if device is not None:
+        return int(device)
     for key in ("PRC_DEVICE", "LOCAL_RANK"):
         v = os.environ.get(key)
         if v not in (None, ""):
             return int(v)
     return 0
+
+
+# ---------------------------------------------------------------------------------------------- torch <-> library
+# NumPy dtype -> the PRC_DT_* code of an input the library reads natively, and -> the PRC_IQ_* kind of raw IQ
+DT_CODES = {np.dtype(np.int8): DT_I8, np.dtype(np.uint8): DT_U8, np.dtype(np.int16): DT_I16,
+            np.dtype(np.float32): DT_F32, np.dtype(np.float64): DT_F64,
+            np.dtype(np.complex64): DT_C64, np.dtype(np.complex128): DT_C128}
+IQ_KINDS = {np.dtype(np.int8): IQ_I8, np.dtype(np.int16): IQ_I16, np.dtype(np.float32): IQ_C64}
+
+
+def np_dtype(torch_dtype):
+    """The NumPy dtype of a torch dtype; None for the ones NumPy has no name for (bfloat16, complex32, ...)."""
+    try:
+        return np.dtype(str(torch_dtype).removeprefix("torch."))
+    except TypeError:
+        return None
+
+
+def torch_dtype(dtype):
+    """The torch dtype of a NumPy dtype."""
+    import torch
+    return getattr(torch, np.dtype(dtype).name)
+
+
+def is_cuda_tensor(x) -> bool:
+    """Is ``x`` a torch tensor on a CUDA device?  Without torch imported, nothing is."""
+    torch = sys.modules.get("torch")
+    return torch is not None and isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def stream_arg(device):
+    """The current torch stream of ``device`` as the library's ``stream`` argument.  torch's default stream is CUDA's
+    legacy default stream, whose handle is 0; the library takes 0 for "my own stream", which is non-blocking and so
+    not ordered after work queued on torch's, so the default stream is passed as cudaStreamLegacy."""
+    import torch
+    return torch.cuda.current_stream(device).cuda_stream or 1       # 1 == cudaStreamLegacy
+
+
+def forked(device, call):
+    """Run ``call(stream)``, one library call that returns a status, on a side stream forked from, and joined back
+    into, the current torch stream of ``device``."""
+    import torch
+    cur = torch.cuda.current_stream(device)
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(cur)
+    check(call(side.cuda_stream))
+    cur.wait_stream(side)
 
 
 def ptr(a) -> int:

@@ -39,7 +39,7 @@ def LS_Filter(refChannel, srvChannel, filterLen, reg=1.0, peek=10, return_filter
     out = np.empty(n, dtype=np.complex64)
     taps = np.empty(max(ntaps, 0), dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_ls_filter_c64(ref.ctypes.data, srv.ctypes.data, n, filterLen, peek, float(reg),
                                out.ctypes.data, taps.ctypes.data, _lib.MEM_HOST, dev, None, 0)
     _lib.check(st)
@@ -65,7 +65,7 @@ def _nlms(refChannel, srvChannel, filterLen, mu, peek, blockLen, initialTaps, re
     out = np.empty(n, dtype=np.complex64)
     taps = np.empty(max(ntaps, 0), dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_nlms_c64(ref.ctypes.data, srv.ctypes.data, n, filterLen, peek, float(mu), int(blockLen),
                           None if init is None else init.ctypes.data, out.ctypes.data, taps.ctypes.data,
                           _lib.MEM_HOST, dev, None, 0)
@@ -131,7 +131,7 @@ def GAL_JPE(refChannel, srvChannel, latticeLen, delayLineLen, mu1, mu2, peek=10,
         h[:] = 0
     else:
         lib = _lib.load()
-        dev = _lib.current_device() if device is None else int(device)
+        dev = _lib.current_device(device)
         st = lib.prc_gal_jpe_frames_c64(ref.ctypes.data, srv.ctypes.data, n, 1, n, latticeLen, delayLineLen,
                                         float(mu1), float(mu2), peek, out.ctypes.data, k.ctypes.data, h.ctypes.data,
                                         _lib.MEM_HOST, dev, None, 0)
@@ -165,7 +165,7 @@ def gal_jpe_frames(ref_frames, srv_frames, latticeLen, delayLineLen, mu1, mu2, p
     h = np.zeros((nframes, delayLineLen), dtype=np.complex64)
     if nframes > 0 and n > 0:
         lib = _lib.load()
-        dev = _lib.current_device() if device is None else int(device)
+        dev = _lib.current_device(device)
         st = lib.prc_gal_jpe_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nframes, n, latticeLen, delayLineLen,
                                         float(mu1), float(mu2), peek, out.ctypes.data, k.ctypes.data, h.ctypes.data,
                                         _lib.MEM_HOST, dev, None, 0)
@@ -190,7 +190,7 @@ def LS_Filter_Toeplitz(refChannel, srvChannel, filterLen, peek=10, return_filter
     out = np.empty(n, dtype=np.complex64)
     taps = np.empty(max(filterLen + peek, 0), dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_ls_toeplitz_c64(ref.ctypes.data, srv.ctypes.data, n, filterLen, peek, out.ctypes.data,
                                  taps.ctypes.data, _lib.MEM_HOST, dev, None, 0)
     _lib.check(st)
@@ -215,7 +215,7 @@ def LS_Filter_Multiple(refChannel, srvChannel, filterLen, sampleRate, dopplerBin
     n = ref.shape[0]
     out = np.empty(n, dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_ls_multiple_c64(ref.ctypes.data, srv.ctypes.data, n, int(filterLen), 10, float(sampleRate),
                                  bins.ctypes.data, bins.shape[0], out.ctypes.data, None, _lib.MEM_HOST, dev, None, 0)
     _lib.check(st)
@@ -244,7 +244,7 @@ def _ls_svd(ref, srv, filterLen, peek, device):
     if n == 0:
         return out, taps, rank
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_ls_svd_frames_c64(ref.ctypes.data, srv.ctypes.data, n, nframes, n, filterLen, peek, out.ctypes.data,
                                    taps.ctypes.data, rank.ctypes.data, _lib.MEM_HOST, dev, None, 0)
     _lib.check(st)

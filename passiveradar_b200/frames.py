@@ -21,18 +21,12 @@ import scipy.signal as signal
 from . import _lib
 
 
-def _torch():
-    import torch
-    return torch
-
-
 def pinned_empty(shape, dtype=np.complex64):
     """Host ndarray backed by page-locked memory (so copies to the GPU are truly async).  The array owns its
     memory: it is released when the last reference to the array goes away."""
-    torch = _torch()
-    tdt = {np.dtype(np.complex64): torch.complex64, np.dtype(np.float32): torch.float32,
-           np.dtype(np.float64): torch.float64}[np.dtype(dtype)]
-    t = torch.empty(tuple(shape) if not isinstance(shape, int) else (shape,), dtype=tdt, pin_memory=True)
+    import torch
+    t = torch.empty(tuple(shape) if not isinstance(shape, int) else (shape,), dtype=_lib.torch_dtype(dtype),
+                    pin_memory=True)
     return t.numpy()          # the ndarray keeps the tensor (its base object) alive
 
 
@@ -43,7 +37,7 @@ class FramePipeline:
 
     def __init__(self, n, range_bins, freq_bins, filter_len=None, reg=1.0, peek=10,
                  window=("kaiser", 5.0), device=None, nslots=4, batch=16):
-        torch = _torch()
+        import torch
         if not torch.cuda.is_available():
             raise _lib.PrcoreError(_lib.PRC_E_CUDA, "FramePipeline needs a CUDA device (no CPU fallback)")
         self.lib = _lib.load()
@@ -53,7 +47,7 @@ class FramePipeline:
         self.filter_len = self.R if filter_len is None else int(filter_len)
         self.peek = int(peek)
         self.reg = float(reg)
-        self.device = _lib.current_device() if device is None else int(device)
+        self.device = _lib.current_device(device)
         self.tdev = torch.device("cuda", self.device)
         self.nslots = max(1, int(nslots))
         self.batch = max(1, int(batch))
@@ -102,7 +96,7 @@ class FramePipeline:
         Work is forked from, and joined back into, the current torch stream.  ``check=True`` synchronises and raises
         ``LinAlgError`` for a frame whose normal equations were singular; otherwise the caller may query
         :meth:`ls_status`."""
-        torch = _torch()
+        import torch
         nf = ref_d.shape[0]
         stride = ref_d.stride(0) if nf > 1 else self.n
         if nf > 1 and srv_d.stride(0) != stride:
@@ -137,7 +131,7 @@ class FramePipeline:
         Returns (nframes, F, R+1, 1) complex64 host array; synchronises before returning and raises ``LinAlgError``
         if a frame's normal equations were singular (as the synchronous ``LS_Filter`` does).  Pass a preallocated
         (ideally pinned) ``out`` when streaming: without it a new pinned array is allocated per call."""
-        torch = _torch()
+        import torch
         ref_frames = np.asarray(ref_frames)
         srv_frames = np.asarray(srv_frames)
         if ref_frames.shape != srv_frames.shape:

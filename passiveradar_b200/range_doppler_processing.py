@@ -67,7 +67,7 @@ def fast_xambg(refChannel, srvChannel, rangeBins, freqBins, inputLen=None, windo
                                      dtype=np.float64)
     out = np.empty((freqBins, rangeBins + 1, 1), dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     st = lib.prc_xambg_c64(ref.ctypes.data, srv.ctypes.data, n, rangeBins, freqBins,
                            None if w is None else w.ctypes.data,
                            None if dtaps is None else dtaps.ctypes.data,
@@ -93,7 +93,7 @@ def direct_xambg(refChannel, srvChannel, rangeBins, freqBins, sampleRate, *, dev
     rangeBins, freqBins = int(rangeBins), int(freqBins)
     out = np.empty((freqBins, rangeBins + 1, 1), dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(lib.prc_direct_xambg_c64(ref.ctypes.data, srv.ctypes.data, ref.shape[0], rangeBins, freqBins,
                                         float(sampleRate), out.ctypes.data, _lib.MEM_HOST, dev, None, 0))
     return out

@@ -56,18 +56,13 @@ import numpy as np
 import scipy.signal as signal
 
 from . import _lib
-from .signal_utils import _decimate_sos, _mix_mode, _OFFSET_DTYPES, _PADLEN, _resample_taps, find_channel_offset
+from .signal_utils import (_mix_mode, _offset_sections, _PADLEN, _raw_iq_kind, _raw_sources, _resample_taps,
+                           find_channel_offset)
 
-_IQ_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.dtype(np.float32): _lib.IQ_C64}
 DOPPLER_BINS = (0, 1, -1, 2, -2)         # main.py:174: clutter at 0 Hz, +/-1 Hz, +/-2 Hz
 LS_PEEK = 10                             # LS_Filter_Multiple's default (clutter_removal.py:162)
 RS_THREADS = 256                         # outputs per resample CTA (frontend.cuh)
 SMEM_LIMIT = 200 * 1024                  # shared memory a front-end CTA may use (prcore_host.h)
-
-
-def _torch():
-    import torch
-    return torch
 
 
 def resample_smem_refusal(up, dn):
@@ -205,7 +200,7 @@ class RecordingPipeline:
 
         Row r of the channel buffers holds chunk c0 - 2 + r: rows 0 and 1 are carried from the previous batch (zeros
         before the first), and the row after the batch is zero for the last one, as overlap(boundary=0) pads."""
-        torch = _torch()
+        import torch
         B, Lc, d = self.batch, self.Lc, self.depth
         bufs = [torch.zeros((B + 3) * Lc, dtype=torch.complex64, device=torch_device) for _ in range(2)]
         frames = [torch.zeros(B + 1, self.cpi, dtype=torch.complex64, device=torch_device) for _ in range(2)]
@@ -230,11 +225,11 @@ class RecordingPipeline:
 
     # ------------------------------------------------------------------ device work of one batch
     def _setup(self):
-        torch = _torch()
+        import torch
         if not torch.cuda.is_available():
             raise _lib.PrcoreError(_lib.PRC_E_CUDA, "RecordingPipeline needs a CUDA device (no CPU fallback)")
         self.lib = _lib.load()
-        self.dev = _lib.current_device() if self.device is None else int(self.device)
+        self.dev = _lib.current_device(self.device)
         self.tdev = torch.device("cuda", self.dev)
         with torch.cuda.device(self.tdev):
             self.stream = torch.cuda.Stream(device=self.tdev)
@@ -265,12 +260,10 @@ class RecordingPipeline:
 
     def _offset_device(self, ref_d, srv_d):
         """find_channel_offset(ref[:10 cpi], srv[:10 cpi], 1, 5_000_000) (main.py:81-83) on device-resident raw data."""
-        torch = _torch()
+        import torch
         a, b = ref_d[:10 * self.cpi], srv_d[:10 * self.cpi]
-        dt = [_OFFSET_DTYPES[np.dtype(str(t.dtype).replace("torch.", ""))] for t in (a, b)]
-        single = [t.dtype == torch.float32 for t in (a, b)]
-        sos = np.ascontiguousarray(np.stack([_decimate_sos(1, s)[0] for s in single]))
-        zi = np.ascontiguousarray(np.stack([_decimate_sos(1, s)[1] for s in single]))
+        dt = [_lib.DT_CODES[_lib.np_dtype(t.dtype)] for t in (a, b)]
+        sos, zi = _offset_sections(1, a.dtype == torch.float32, b.dtype == torch.float32)
         off = torch.zeros(1, dtype=torch.int64, device=self.tdev)
         _lib.check(self.lib.prc_channel_offset(a.data_ptr(), dt[0], a.shape[0], b.data_ptr(), dt[1], b.shape[0], 1,
                                                5_000_000, sos.ctypes.data, zi.ctypes.data, off.data_ptr(), None,
@@ -281,7 +274,7 @@ class RecordingPipeline:
         """find_channel_offset(refc1, srvc1, 1, 5_000_000) (main.py:50-54) for device-resident raw data head =
         stream[0:20 cpi]: refc1 and srvc1 are [0::2] and [1::2] of deinterleave_IQ(head), complex64, so the offset is
         in complex samples.  Both channels are read out of the stream in place."""
-        torch = _torch()
+        import torch
         m = head.shape[0] // 2                                    # deinterleave_IQ's complex samples
         lens = ((m + 1) // 2, m // 2)
         if min(lens) <= _PADLEN:
@@ -292,24 +285,13 @@ class RecordingPipeline:
                                                _lib.MIX_NONE, 0.0, 1.0, 0.0, chans[q].data_ptr(), _lib.MEM_DEVICE,
                                                self.dev, self.stream.cuda_stream,
                                                _lib.FLAG_ASYNC | _lib.FLAG_CHANNEL_PAIR))
-        sos, zi = _decimate_sos(1, True)
-        sos, zi = np.ascontiguousarray(np.stack([sos, sos])), np.ascontiguousarray(np.stack([zi, zi]))
+        sos, zi = _offset_sections(1, True, True)
         off = torch.zeros(1, dtype=torch.int64, device=self.tdev)
         _lib.check(self.lib.prc_channel_offset(chans[0].data_ptr(), _lib.DT_C64, lens[0], chans[1].data_ptr(),
                                                _lib.DT_C64, lens[1], 1, 5_000_000, sos.ctypes.data, zi.ctypes.data,
                                                off.data_ptr(), None, _lib.MEM_DEVICE, self.dev,
                                                self.stream.cuda_stream, 0))
         return int(off.item())
-
-    def _sources(self, ref_raw, srv_raw):
-        """The raw sources of a run: the one stream of an interleaved pipeline, or ref_raw and srv_raw."""
-        if self.interleaved:
-            if srv_raw is not None:
-                raise ValueError("interleaved_input_channels is True: pass the one interleaved source only")
-            return (ref_raw,)
-        if srv_raw is None:
-            raise ValueError("interleaved_input_channels is False: pass ref_raw and srv_raw")
-        return ref_raw, srv_raw
 
     def _reads(self, p):
         """Where the front end reads a plan's chunks: for each channel the raw element of its source where its chunk 0
@@ -325,19 +307,10 @@ class RecordingPipeline:
         is in complex samples.  Writes the maps as (nframes, F, R+1) complex64 into ``maps`` (allocated when None) on
         the device and returns it.  Work is forked from, and joined back into, the current torch stream: the raw tensors
         may still be being written by work queued there, and the maps are ready for work queued there after the call."""
-        torch = _torch()
-        srcs = self._sources(ref_raw, srv_raw)
+        import torch
+        srcs = _raw_sources(self.interleaved, ref_raw, srv_raw)
         self._setup()
-        kinds = []
-        for name, t in zip(("ref_raw", "srv_raw"), srcs):
-            if not isinstance(t, torch.Tensor) or t.device != self.tdev:
-                raise ValueError(f"{name} must be a tensor on {self.tdev}")
-            if t.dim() != 1 or not t.is_contiguous():
-                raise ValueError(f"{name} must be one-dimensional and contiguous")
-            dt = {torch.int8: np.int8, torch.int16: np.int16, torch.float32: np.float32}.get(t.dtype)
-            if dt is None:
-                raise TypeError(f"{name} must be int8, int16 or float32 raw IQ, got {t.dtype}")
-            kinds.append(_IQ_KINDS[np.dtype(dt)])
+        kinds = [_raw_iq_kind(name, t, self.tdev) for name, t in zip(("ref_raw", "srv_raw"), srcs)]
         cur = torch.cuda.current_stream(self.tdev)
         self.stream.wait_stream(cur)
         if offset is None:
@@ -373,12 +346,12 @@ class RecordingPipeline:
         """ref_raw, srv_raw: 1-D raw interleaved IQ sources (ndarray, np.memmap, h5py dataset: anything sliceable),
         int8, int16 or float32; for an interleaved pipeline ref_raw is the one two-channel stream and srv_raw is None,
         and ``offset`` is in complex samples.  Returns main.py's ``xambg``: (F, R+1, nframes) complex64 on the host."""
-        torch = _torch()
+        import torch
         from .frames import pinned_empty
-        srcs = self._sources(ref_raw, srv_raw)
+        srcs = _raw_sources(self.interleaved, ref_raw, srv_raw)
         self._setup()
         dtypes = [np.dtype(x.dtype) for x in srcs]
-        kinds = [_IQ_KINDS[dt] for dt in dtypes]
+        kinds = [_lib.IQ_KINDS[dt] for dt in dtypes]
         if offset is None and self.interleaved:
             with torch.cuda.stream(self.stream):             # the head's copy is ordered before its reads
                 head = torch.from_numpy(np.ascontiguousarray(ref_raw[0:20 * self.cpi])).to(self.tdev)
@@ -395,11 +368,11 @@ class RecordingPipeline:
         out = np.empty((self.F, self.R + 1, N), dtype=np.complex64)
         # two slots of raw batches (pinned host, device), of maps (device, pinned host); kept for the next run, since
         # page-locking them costs more than a short recording takes
-        tdt = {np.dtype(np.int8): torch.int8, np.dtype(np.int16): torch.int16, np.dtype(np.float32): torch.float32}
+        tdt = [_lib.torch_dtype(dt) for dt in dtypes]
         slot = B * step + extra
         if getattr(self, "_ring_key", None) != (tuple(dtypes), slot, self.dev):
-            self._ring = ([[torch.empty(slot, dtype=tdt[dt], pin_memory=True) for dt in dtypes] for _ in range(2)],
-                          [[torch.empty(slot, dtype=tdt[dt], device=self.tdev) for dt in dtypes] for _ in range(2)],
+            self._ring = ([[torch.empty(slot, dtype=t, pin_memory=True) for t in tdt] for _ in range(2)],
+                          [[torch.empty(slot, dtype=t, device=self.tdev) for t in tdt] for _ in range(2)],
                           [torch.empty(B + 1, self.F, self.R + 1, dtype=torch.complex64, device=self.tdev)
                            for _ in range(2)],
                           [pinned_empty((B + 1, self.F, self.R + 1)) for _ in range(2)])

@@ -46,6 +46,30 @@ def _raw_iq(interleavedIQ):
     return np.ascontiguousarray(x, dtype=np.float32), _lib.IQ_C64, n
 
 
+def _raw_sources(interleaved, ref_raw, srv_raw):
+    """The raw sources of a run: the one stream of an interleaved configuration, or ref_raw and srv_raw."""
+    if interleaved:
+        if srv_raw is not None:
+            raise ValueError("interleaved_input_channels is True: pass the one interleaved source only")
+        return (ref_raw,)
+    if srv_raw is None:
+        raise ValueError("interleaved_input_channels is False: pass ref_raw and srv_raw")
+    return ref_raw, srv_raw
+
+
+def _raw_iq_kind(name, t, tdev):
+    """The PRC_IQ_* kind of a raw interleaved IQ source tensor, which must be one-dimensional and contiguous on tdev."""
+    import torch
+    if not isinstance(t, torch.Tensor) or t.device != tdev:
+        raise ValueError(f"{name} must be a tensor on {tdev}")
+    if t.dim() != 1 or not t.is_contiguous():
+        raise ValueError(f"{name} must be one-dimensional and contiguous")
+    kind = _lib.IQ_KINDS.get(_lib.np_dtype(t.dtype))
+    if kind is None:
+        raise TypeError(f"{name} must be int8, int16 or float32 raw IQ, got {t.dtype}")
+    return kind
+
+
 def _mix_mode(fc, Fs, phase_offset):
     po = np.asarray(phase_offset)
     if po.size != 1:
@@ -68,7 +92,7 @@ def deinterleave_IQ(interleavedIQ, *, device=None):
     if n == 0:
         return out
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(lib.prc_iq_mix_c64(buf.ctypes.data, kind, n, _lib.MIX_NONE, 0.0, 1.0, 0.0, out.ctypes.data,
                                   _lib.MEM_HOST, dev, None, 0))
     return out
@@ -90,7 +114,7 @@ def frequency_shift(x, fc, Fs, phase_offset=0, *, device=None):
     out = np.empty(n, dtype=np.complex64)
     if n:
         lib = _lib.load()
-        dev = _lib.current_device() if device is None else int(device)
+        dev = _lib.current_device(device)
         _lib.check(lib.prc_iq_mix_c64(xin.ctypes.data, _lib.IQ_C64, n, mode, float(fc), float(Fs), po,
                                       out.ctypes.data, _lib.MEM_HOST, dev, None, 0))
     narrow = mode == _lib.MIX_C64 and x.dtype in (np.complex64, np.float32, np.float16)
@@ -130,7 +154,7 @@ def _run_frontend(buf, kind, n, mode, fc, Fs, po, up, dn, single, device):
     n_out = n_out // dn + bool(n_out % dn)
     out = np.empty(n_out, dtype=np.complex64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(lib.prc_frontend_c64(buf.ctypes.data, kind, n, mode, float(fc), float(Fs), po, up, dn,
                                     h.ctypes.data, h.shape[0], out.ctypes.data, n_out, _lib.MEM_HOST, dev, None, 0))
     return out
@@ -166,7 +190,7 @@ def frontend(interleavedIQ, fc, Fs, phase_offset, up, dn, *, device=None):
     if up == dn == 1:
         out = np.empty(n, dtype=np.complex64)
         lib = _lib.load()
-        dev = _lib.current_device() if device is None else int(device)
+        dev = _lib.current_device(device)
         _lib.check(lib.prc_iq_mix_c64(buf.ctypes.data, kind, n, mode, float(fc), float(Fs), po, out.ctypes.data,
                                       _lib.MEM_HOST, dev, None, 0))
         return out
@@ -175,9 +199,6 @@ def frontend(interleavedIQ, fc, Fs, phase_offset, up, dn, *, device=None):
 
 
 # ---- channel offset (reference signal_utils.py:29-78) ------------------------------------------------------------
-_OFFSET_DTYPES = {np.dtype(np.int8): _lib.DT_I8, np.dtype(np.uint8): _lib.DT_U8, np.dtype(np.int16): _lib.DT_I16,
-                  np.dtype(np.float32): _lib.DT_F32, np.dtype(np.float64): _lib.DT_F64,
-                  np.dtype(np.complex64): _lib.DT_C64, np.dtype(np.complex128): _lib.DT_C128}
 _PADLEN = 27
 
 
@@ -188,9 +209,9 @@ def _offset_input(x):
     if a.ndim != 1:
         raise ValueError("the signals must be one-dimensional")
     single = a.dtype in (np.float32, np.complex64)
-    if a.dtype not in _OFFSET_DTYPES:
+    if a.dtype not in _lib.DT_CODES:
         a = a.astype(np.complex128 if np.iscomplexobj(a) else np.float64)
-    return np.ascontiguousarray(a), _OFFSET_DTYPES[a.dtype], single
+    return np.ascontiguousarray(a), _lib.DT_CODES[a.dtype], single
 
 
 @functools.lru_cache(maxsize=64)
@@ -203,6 +224,13 @@ def _decimate_sos(nd, single):
         sos = sos.astype(np.float32)
     zi = sosfilt_zi(sos)
     return np.ascontiguousarray(sos, dtype=np.float64), np.ascontiguousarray(zi, dtype=np.float64)
+
+
+def _offset_sections(nd, single1, single2):
+    """prc_channel_offset's sos and zi arguments: decimate's sections and sosfilt_zi for each of the two signals
+    (float32-rounded for a float32 / complex64 one), stacked."""
+    (sos1, zi1), (sos2, zi2) = _decimate_sos(nd, single1), _decimate_sos(nd, single2)
+    return np.ascontiguousarray(np.stack([sos1, sos2])), np.ascontiguousarray(np.stack([zi1, zi2]))
 
 
 def _pad_width(v):
@@ -225,13 +253,12 @@ def _channel_offset(s1, s2, nd, nl, device=None, want_xc=False):
     a2, d2, single2 = _offset_input(s2)
     if min(a1.shape[0], a2.shape[0]) <= _PADLEN:
         raise ValueError(f"The length of the input vector x must be greater than padlen, which is {_PADLEN}.")
-    sos = np.ascontiguousarray(np.stack([_decimate_sos(nd, single1)[0], _decimate_sos(nd, single2)[0]]))
-    zi = np.ascontiguousarray(np.stack([_decimate_sos(nd, single1)[1], _decimate_sos(nd, single2)[1]]))
+    sos, zi = _offset_sections(nd, single1, single2)
     n1d, n2d = -(-a1.shape[0] // nd), -(-a2.shape[0] // nd)
     xc = np.empty(abs(n1d - (n2d + 2 * nl)) + 1, dtype=np.float64) if want_xc else None
     off = np.zeros(1, dtype=np.int64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(lib.prc_channel_offset(a1.ctypes.data, d1, a1.shape[0], a2.ctypes.data, d2, a2.shape[0], nd, nl,
                                       sos.ctypes.data, zi.ctypes.data, off.ctypes.data,
                                       None if xc is None else xc.ctypes.data, _lib.MEM_HOST, dev, None, 0))
@@ -284,7 +311,7 @@ def xcorr(s1, s2, nlead, nlag, *, device=None):
     cplx = np.iscomplexobj(a1) or np.iscomplexobj(a2)
     out = np.empty(abs(a1.shape[0] - (a2.shape[0] + nlag + nlead)) + 1, dtype=np.complex128 if cplx else np.float64)
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(lib.prc_xcorr(a1.ctypes.data, d1, a1.shape[0], a2.ctypes.data, d2, a2.shape[0], nlead, nlag,
                              out.ctypes.data, _lib.MEM_HOST, dev, None, 0))
     if rt.kind in "iu":
@@ -293,44 +320,10 @@ def xcorr(s1, s2, nlead, nlag, *, device=None):
 
 
 # ---- decimate, channel_preprocessing, normalize (reference signal_utils.py:7-13, :80-85) ---------------------------
-_NATIVE = {np.dtype(np.int8): _lib.DT_I8, np.dtype(np.uint8): _lib.DT_U8, np.dtype(np.int16): _lib.DT_I16,
-           np.dtype(np.float32): _lib.DT_F32, np.dtype(np.float64): _lib.DT_F64,
-           np.dtype(np.complex64): _lib.DT_C64, np.dtype(np.complex128): _lib.DT_C128}
-_RAW_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.dtype(np.float32): _lib.IQ_C64}
-
-
-def _torch():
-    import torch
-    return torch
-
-
-def _np_dtype_of(torch, t):
-    """NumPy dtype of a tensor's elements (None for the ones NumPy has no name for here, e.g. bfloat16)."""
-    return {torch.bool: np.bool_, torch.int8: np.int8, torch.uint8: np.uint8, torch.int16: np.int16,
-            torch.int32: np.int32, torch.int64: np.int64, torch.float16: np.float16, torch.float32: np.float32,
-            torch.float64: np.float64, torch.complex64: np.complex64, torch.complex128: np.complex128}.get(t.dtype)
-
-
-def _torch_dtype(torch, dt):
-    return {np.dtype(np.int8): torch.int8, np.dtype(np.uint8): torch.uint8, np.dtype(np.int16): torch.int16,
-            np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
-            np.dtype(np.complex64): torch.complex64, np.dtype(np.complex128): torch.complex128}[np.dtype(dt)]
-
-
 def _device_of(torch, device):
     if not torch.cuda.is_available():
         raise _lib.PrcoreError(_lib.PRC_E_CUDA, "no CUDA device available; libprcore has no CPU fallback")
-    return torch.device("cuda", _lib.current_device() if device is None else int(device))
-
-
-def _forked(torch, tdev, call):
-    """Run one library call on a side stream forked from, and joined back into, the current torch stream.  The library
-    gives a NULL stream (torch's default stream) a stream of its own, so the call is never enqueued on it directly."""
-    cur = torch.cuda.current_stream(tdev)
-    side = torch.cuda.Stream(device=tdev)
-    side.wait_stream(cur)
-    _lib.check(call(side.cuda_stream))
-    cur.wait_stream(side)
+    return torch.device("cuda", _lib.current_device(device))
 
 
 @functools.lru_cache(maxsize=32)
@@ -357,7 +350,7 @@ def _decimation_factor(q):
 def _decimate_dtype(dt):
     """scipy.signal.decimate's result dtype: x's own when inexact, float64 for integers, bools and float16."""
     dt = np.dtype(dt)
-    if dt in (np.dtype(np.longdouble), np.dtype(np.clongdouble)) and dt not in _NATIVE:
+    if dt in (np.dtype(np.longdouble), np.dtype(np.clongdouble)) and dt not in _lib.DT_CODES:
         raise TypeError("No matching signature found")
     if dt.kind == "c":
         return dt
@@ -369,12 +362,12 @@ def _decimate_dtype(dt):
 def _run_decimate(torch, rows, src, n, mode, fc, Fs, po, q, single, out_dtype, tdev):
     """One prc_decimate_rows call on the current torch stream: rows (k, n) contiguous on tdev -> (k, ceil(n/q))."""
     k = rows.shape[0]
-    out = torch.empty(k, -(-n // q), dtype=_torch_dtype(torch, out_dtype), device=tdev)
+    out = torch.empty(k, -(-n // q), dtype=_lib.torch_dtype(out_dtype), device=tdev)
     taps = _decimate_taps(q, single)
     lib = _lib.load()
-    _forked(torch, tdev, lambda st: lib.prc_decimate_rows(rows.data_ptr(), src, n, k, n, mode, float(fc), float(Fs), po,
-                                                          taps.ctypes.data, q, out.data_ptr(), out.shape[1], tdev.index,
-                                                          st, _lib.FLAG_ASYNC))
+    _lib.forked(tdev, lambda st: lib.prc_decimate_rows(rows.data_ptr(), src, n, k, n, mode, float(fc), float(Fs), po,
+                                                       taps.ctypes.data, q, out.data_ptr(), out.shape[1], tdev.index, st,
+                                                       _lib.FLAG_ASYNC))
     return out
 
 
@@ -385,14 +378,13 @@ def decimate(x, q, *, device=None):
     Hamming taps along axis 0 of an array of any shape, in SciPy's dtype (x's own when inexact, float64 otherwise;
     float32 taps and sums for float32 and complex64, float64 for the rest).  A NumPy (or array-like) x gives NumPy; a
     CUDA tensor gives a tensor on its device, ordered on the current torch stream.'''
+    import torch
     q = _decimation_factor(q)
-    torch = None
-    if type(x).__module__.startswith("torch"):
-        torch = _torch()
-    if torch is not None and isinstance(x, torch.Tensor):
+    is_t = isinstance(x, torch.Tensor)
+    if is_t:
         if not x.is_cuda:
             raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
-        ndt = _np_dtype_of(torch, x)
+        ndt = _lib.np_dtype(x.dtype)
         if ndt is None:
             raise TypeError(f"decimate takes numeric tensors, got {x.dtype}")
         shape, rd = tuple(x.shape), _decimate_dtype(ndt)
@@ -405,23 +397,20 @@ def decimate(x, q, *, device=None):
     k = int(np.prod(shape[1:], dtype=np.int64))
     nout = -(-n // q)
     if n == 0 or k == 0:
-        if torch is not None and isinstance(x, torch.Tensor):
-            return torch.empty((nout,) + shape[1:], dtype=_torch_dtype(torch, rd), device=x.device)
+        if is_t:
+            return torch.empty((nout,) + shape[1:], dtype=_lib.torch_dtype(rd), device=x.device)
         return np.empty((nout,) + shape[1:], dtype=rd)
     single = rd in (np.float32, np.complex64)
-    if torch is not None and isinstance(x, torch.Tensor):
-        t = x
-        if np.dtype(ndt) not in _NATIVE:
-            t = t.to(torch.float64)
+    if is_t:
+        t = x if ndt in _lib.DT_CODES else x.to(torch.float64)
         rows = t.reshape(n, k).T.contiguous()
-        out = _run_decimate(torch, rows, _NATIVE[np.dtype(_np_dtype_of(torch, rows))], n, _lib.MIX_NONE, 0.0, 1.0, 0.0,
+        out = _run_decimate(torch, rows, _lib.DT_CODES[_lib.np_dtype(rows.dtype)], n, _lib.MIX_NONE, 0.0, 1.0, 0.0,
                             q, single, rd, x.device)
         return out.T.reshape((nout,) + shape[1:])
-    a = x if x.dtype in _NATIVE else x.astype(rd)
-    torch = _torch()
+    a = x if x.dtype in _lib.DT_CODES else x.astype(rd)
     tdev = _device_of(torch, device)
     rows = torch.from_numpy(np.ascontiguousarray(a.reshape(n, k).T)).to(tdev)
-    out = _run_decimate(torch, rows, _NATIVE[a.dtype], n, _lib.MIX_NONE, 0.0, 1.0, 0.0, q, single, rd, tdev)
+    out = _run_decimate(torch, rows, _lib.DT_CODES[a.dtype], n, _lib.MIX_NONE, 0.0, 1.0, 0.0, q, single, rd, tdev)
     return np.ascontiguousarray(out.cpu().numpy().T).reshape((nout,) + shape[1:])
 
 
@@ -432,29 +421,26 @@ def channel_preprocessing(sig, dec, fc, Fs, *, device=None):
     float32 I/Q is deinterleaved (I = sig[0:-1:2], Q = sig[1::2]) and mixed as it is staged, so the tuned signal is never
     stored.  complex64 when the reference's is (Python-scalar fc and Fs), complex128 otherwise.  A CUDA tensor of raw
     samples gives a tensor on its device, ordered on the current torch stream.'''
+    import torch
     q = _decimation_factor(dec)
     mode, po = _mix_mode(fc, Fs, 0)
     rd = np.dtype(np.complex64) if mode == _lib.MIX_C64 else np.dtype(np.complex128)
-    torch = _torch() if type(sig).__module__.startswith("torch") else None
-    if torch is not None and isinstance(sig, torch.Tensor):
+    if isinstance(sig, torch.Tensor):
         if not sig.is_cuda:
             raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
         if sig.dim() != 1:
             raise ValueError("interleaved IQ must be one-dimensional")
         n = sig.shape[0] // 2
         t = sig[:2 * n]
-        ndt = _np_dtype_of(torch, t)
-        if ndt is None or np.dtype(ndt) not in _RAW_KINDS:
+        if _lib.np_dtype(t.dtype) not in _lib.IQ_KINDS:
             t = t.to(torch.float32)
-            ndt = np.float32
         if n == 0:
-            return torch.empty(0, dtype=_torch_dtype(torch, rd), device=sig.device)
-        raw, kind, tdev = t.contiguous(), _RAW_KINDS[np.dtype(ndt)], sig.device
+            return torch.empty(0, dtype=_lib.torch_dtype(rd), device=sig.device)
+        raw, kind, tdev = t.contiguous(), _lib.IQ_KINDS[_lib.np_dtype(t.dtype)], sig.device
     else:
         buf, kind, n = _raw_iq(sig)
         if n == 0:
             return np.empty(0, dtype=rd)
-        torch = _torch()
         tdev = _device_of(torch, device)
         raw = torch.from_numpy(buf).to(tdev)
     out = _run_decimate(torch, raw.view(1, -1), _lib.DEC_RAW + kind, n, mode, fc, Fs, po, q, mode == _lib.MIX_C64, rd,
@@ -473,33 +459,31 @@ def normalize(x, *, device=None):
     complex128 x of any shape, in NumPy's result dtype (float64 for the integers).  The mean is summed in float64 in a
     fixed order.  An all-zero x gives NaN, an empty x an empty result.  A CUDA tensor gives a tensor on its device,
     ordered on the current torch stream.'''
-    torch = _torch() if type(x).__module__.startswith("torch") else None
-    is_t = torch is not None and isinstance(x, torch.Tensor)
+    import torch
+    is_t = isinstance(x, torch.Tensor)
     if is_t:
         if not x.is_cuda:
             raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
-        dt = _np_dtype_of(torch, x)
-        dt = None if dt is None else np.dtype(dt)
+        dt = _lib.np_dtype(x.dtype)
     else:
         x = np.asarray(x)
         dt = x.dtype
-    if dt not in _NATIVE:
+    if dt not in _lib.DT_CODES:
         raise TypeError(f"normalize takes int8, uint8, int16, float32, float64, complex64 or complex128, got {dt}")
     rd = _NORM_OUT.get(dt, np.dtype(np.float64))
     shape = tuple(x.shape)
     n = int(np.prod(shape, dtype=np.int64))
     if n == 0:
         if is_t:
-            return torch.empty(shape, dtype=_torch_dtype(torch, rd), device=x.device)
+            return torch.empty(shape, dtype=_lib.torch_dtype(rd), device=x.device)
         return np.empty(shape, dtype=rd)
     if is_t:
         src, tdev = x.contiguous(), x.device
     else:
-        torch = _torch()
         tdev = _device_of(torch, device)
         src = torch.from_numpy(np.ascontiguousarray(x).reshape(-1)).to(tdev)
-    out = torch.empty(shape, dtype=_torch_dtype(torch, rd), device=tdev)
+    out = torch.empty(shape, dtype=_lib.torch_dtype(rd), device=tdev)
     lib = _lib.load()
-    _forked(torch, tdev, lambda st: lib.prc_normalize(src.data_ptr(), _NATIVE[dt], n, out.data_ptr(), tdev.index, st,
-                                                      _lib.FLAG_ASYNC))
+    _lib.forked(tdev, lambda st: lib.prc_normalize(src.data_ptr(), _lib.DT_CODES[dt], n, out.data_ptr(), tdev.index, st,
+                                                   _lib.FLAG_ASYNC))
     return out if is_t else out.cpu().numpy()

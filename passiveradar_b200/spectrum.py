@@ -17,16 +17,10 @@ import operator
 import numpy as np
 
 from . import _lib
-from .signal_utils import _decimate_sos, _mix_mode, _resample_taps
+from .signal_utils import _mix_mode, _offset_sections, _raw_iq_kind, _raw_sources, _resample_taps
 
 MIN_PAD_TO, MAX_PAD_TO = 16, 8192
-_DTYPES = {np.dtype(np.float32): _lib.DT_F32, np.dtype(np.float64): _lib.DT_F64,
-           np.dtype(np.complex64): _lib.DT_C64, np.dtype(np.complex128): _lib.DT_C128}
-
-
-def _torch():
-    import torch
-    return torch
+_DTYPES = {dt: _lib.DT_CODES[dt] for dt in map(np.dtype, (np.float32, np.float64, np.complex64, np.complex128))}
 
 
 def _host_dtype(dt):
@@ -91,41 +85,30 @@ def _plan(dtype, NFFT, Fs, Fc, detrend, window, noverlap, pad_to, sides, scale_b
     return NFFT, noverlap, pad_to, w, scale, onesided, freqs + Fc
 
 
-def _run(lib, dev, x, dtype_code, n, nframes, row_stride, plan, out, stream):
-    """One prc_psd_frames call on device tensors (x: nframes rows of n samples, row_stride elements apart)."""
-    nfft, noverlap, pad_to, w_dev, scale, onesided = plan
-    _lib.check(lib.prc_psd_frames(x.data_ptr(), dtype_code, n, nframes, row_stride, nfft, noverlap, pad_to,
-                                  w_dev.data_ptr(), scale, int(onesided), out.data_ptr(), out.stride(0), dev,
-                                  stream.cuda_stream, _lib.FLAG_ASYNC))
-
-
 def _device_rows(torch, frames, device):
-    """A CUDA tensor, or a host array (staged with torch), as (tensor of rows with unit element stride, dtype code, host?)."""
+    """A CUDA tensor, or a host array (staged with torch), as (tensor of rows with unit element stride, host?)."""
     if isinstance(frames, torch.Tensor):
         if not frames.is_cuda:
             raise ValueError("a tensor input must be a CUDA tensor; pass host data as a NumPy array")
         t = frames
-        tdt = {torch.complex64: np.complex64, torch.complex128: np.complex128, torch.float32: np.float32,
-               torch.float64: np.float64}.get(t.dtype)
-        if tdt is None:
+        if _lib.np_dtype(t.dtype) not in _DTYPES:
             t = t.to(torch.complex128 if t.is_complex() else torch.float64)
-            tdt = np.complex128 if t.is_complex() else np.float64
         if t.dim() >= 1 and t.shape[-1] > 0 and t.stride(-1) != 1:
             t = t.contiguous()
-        return t, _DTYPES[np.dtype(tdt)], False
+        return t, False
     if not torch.cuda.is_available():
         raise _lib.PrcoreError(_lib.PRC_E_CUDA, "psd needs a CUDA device (no CPU fallback)")
     a = np.asarray(frames)
     a = np.ascontiguousarray(a, dtype=_host_dtype(a.dtype))
-    dev = _lib.current_device() if device is None else int(device)
-    return torch.from_numpy(a).to(torch.device("cuda", dev)), _DTYPES[a.dtype], True
+    return torch.from_numpy(a).to(torch.device("cuda", _lib.current_device(device))), True
 
 
 def _psd_rows(frames, NFFT, Fs, Fc, detrend, window, noverlap, pad_to, sides, scale_by_freq, device, ndim):
-    torch = _torch()
+    import torch
     if isinstance(frames, torch.Tensor):
-        dtype = {torch.complex64: np.complex64, torch.complex128: np.complex128, torch.float32: np.float32}.get(
-            frames.dtype, np.complex128 if frames.is_complex() else np.float64)
+        dtype = _lib.np_dtype(frames.dtype)
+        if dtype not in _DTYPES:
+            dtype = np.dtype(np.complex128 if frames.is_complex() else np.float64)
         shape = tuple(frames.shape)
     else:
         a = np.asarray(frames)
@@ -136,18 +119,17 @@ def _psd_rows(frames, NFFT, Fs, Fc, detrend, window, noverlap, pad_to, sides, sc
         raise ValueError("x must not be empty")
     nfft, noverlap, pad_to, w, scale, onesided, freqs = _plan(dtype, NFFT, Fs, Fc, detrend, window, noverlap, pad_to,
                                                               sides, scale_by_freq)
-    t, code, host = _device_rows(torch, frames, device)
+    t, host = _device_rows(torch, frames, device)
     tdev = t.device
     rows = t.view(1, -1) if ndim == 1 else t
     lib = _lib.load()
-    cur = torch.cuda.current_stream(tdev)
-    side = torch.cuda.Stream(device=tdev)
     w_dev = torch.from_numpy(w).to(tdev)
     out = torch.empty(rows.shape[0], pad_to // 2 + 1 if onesided else pad_to, dtype=torch.float64, device=tdev)
-    side.wait_stream(cur)
-    _run(lib, tdev.index, rows, code, rows.shape[1], rows.shape[0], rows.stride(0) if rows.shape[0] > 1 else rows.shape[1],
-         (nfft, noverlap, pad_to, w_dev, scale, onesided), out, side)
-    cur.wait_stream(side)
+    n, nframes = rows.shape[1], rows.shape[0]
+    _lib.forked(tdev, lambda st: lib.prc_psd_frames(
+        rows.data_ptr(), _DTYPES[_lib.np_dtype(rows.dtype)], n, nframes, rows.stride(0) if nframes > 1 else n,
+        nfft, noverlap, pad_to, w_dev.data_ptr(), scale, int(onesided), out.data_ptr(), out.stride(0), tdev.index, st,
+        _lib.FLAG_ASYNC))
     out = out[0] if ndim == 1 else out
     if host:
         return out.cpu().numpy(), freqs
@@ -181,7 +163,6 @@ PREVIEW_NFFT_INPUT = 8192            # signal_preview.py:52-55
 PREVIEW_NFFT_CHANNEL = 2048          # signal_preview.py:68-71
 PREVIEW_OFFSET_ND, PREVIEW_OFFSET_NL = 4, 50000          # find_channel_offset(ref, srv, 4, 50000)
 PREVIEW_XCORR_LAGS = 2000            # xcorr(ref, srv, 2000, 2000)
-_IQ_KINDS = {np.dtype(np.int8): _lib.IQ_I8, np.dtype(np.int16): _lib.IQ_I16, np.dtype(np.float32): _lib.IQ_C64}
 
 
 class SignalPreview:
@@ -244,26 +225,15 @@ class SignalPreview:
 
     # ------------------------------------------------------------------ device chain
     def _setup(self, tdev=None):
-        torch = _torch()
+        import torch
         if not torch.cuda.is_available():
             raise _lib.PrcoreError(_lib.PRC_E_CUDA, "SignalPreview needs a CUDA device (no CPU fallback)")
         self.lib = _lib.load()
         if tdev is None:
-            tdev = torch.device("cuda", _lib.current_device() if self.device is None else int(self.device))
+            tdev = torch.device("cuda", _lib.current_device(self.device))
         self.tdev = tdev
         self.dev = tdev.index
         self.stream = torch.cuda.Stream(device=tdev)
-
-    def _check_raw(self, name, t):
-        torch = _torch()
-        if not isinstance(t, torch.Tensor) or t.device != self.tdev:
-            raise ValueError(f"{name} must be a tensor on {self.tdev}")
-        if t.dim() != 1 or not t.is_contiguous():
-            raise ValueError(f"{name} must be one-dimensional and contiguous")
-        dt = {torch.int8: np.int8, torch.int16: np.int16, torch.float32: np.float32}.get(t.dtype)
-        if dt is None:
-            raise TypeError(f"{name} must be int8, int16 or float32 raw IQ, got {t.dtype}")
-        return _IQ_KINDS[np.dtype(dt)]
 
     def _deinterleave(self, raw, kind, out):
         n = raw.shape[0] // 2
@@ -285,10 +255,11 @@ class SignalPreview:
                                            self.stream.cuda_stream, _lib.FLAG_ASYNC))
 
     def _window(self, nfft):
+        import torch
         cache = self.__dict__.setdefault("_windows", {})
         if (nfft, self.dev) not in cache:
             w = np.hanning(nfft)
-            cache[(nfft, self.dev)] = (_torch().from_numpy(w).to(self.tdev), w)
+            cache[(nfft, self.dev)] = (torch.from_numpy(w).to(self.tdev), w)
         return cache[(nfft, self.dev)]
 
     def _spectra(self, chans, lens, nfft, Fs, out):
@@ -299,23 +270,20 @@ class SignalPreview:
                 self._psd(chans[q:q + 1], lens[q], nfft, Fs, out[q:q + 1])
 
     def _chain(self, ref_raw, srv_raw):
-        torch = _torch()
+        import torch
+        srcs = _raw_sources(self.interleaved, ref_raw, srv_raw)
+        names = ("data",) if self.interleaved else ("ref_raw", "srv_raw")
+        kinds = [_raw_iq_kind(name, t, self.tdev) for name, t in zip(names, srcs)]
         if self.interleaved:
-            if srv_raw is not None:
-                raise ValueError("interleaved_input_channels is True: pass the one interleaved source only")
-            k = self._check_raw("data", ref_raw)
             data = ref_raw[:self.icl]
             m = data.shape[0] // 2                                 # deinterleave_IQ's complex samples
             n_ref, n_srv = (m + 1) // 2, m // 2
             chans = torch.zeros(2, n_ref, dtype=torch.complex64, device=self.tdev)
             for q, n in enumerate((n_ref, n_srv)):
                 if n:
-                    self._channel(data, k, q, n, chans[q])
+                    self._channel(data, kinds[0], q, n, chans[q])
         else:
-            if srv_raw is None:
-                raise ValueError("interleaved_input_channels is False: pass ref_raw and srv_raw")
-            kinds = [self._check_raw("ref_raw", ref_raw), self._check_raw("srv_raw", srv_raw)]
-            raws = [ref_raw[:self.icl], srv_raw[:self.icl]]
+            raws = [t[:self.icl] for t in srcs]
             n_ref, n_srv = raws[0].shape[0] // 2, raws[1].shape[0] // 2
             chans = torch.zeros(2, max(n_ref, n_srv), dtype=torch.complex64, device=self.tdev)
             for q in range(2):
@@ -340,12 +308,11 @@ class SignalPreview:
                                                      _lib.FLAG_ASYNC))
         channel_psd = torch.empty(2, PREVIEW_NFFT_CHANNEL, dtype=torch.float64, device=self.tdev)
         self._spectra(res, rs, PREVIEW_NFFT_CHANNEL, self.bw, channel_psd)
-        sos, zi = _decimate_sos(PREVIEW_OFFSET_ND, True)           # decimate's sections for complex64 signals
-        sos2, zi2 = np.ascontiguousarray(np.stack([sos, sos])), np.ascontiguousarray(np.stack([zi, zi]))
+        sos, zi = _offset_sections(PREVIEW_OFFSET_ND, True, True)      # decimate's sections for complex64 signals
         off = torch.zeros(1, dtype=torch.int64, device=self.tdev)
         _lib.check(self.lib.prc_channel_offset(chans[0].data_ptr(), _lib.DT_C64, n_ref, chans[1].data_ptr(),
                                                _lib.DT_C64, n_srv, PREVIEW_OFFSET_ND, PREVIEW_OFFSET_NL,
-                                               sos2.ctypes.data, zi2.ctypes.data, off.data_ptr(), None,
+                                               sos.ctypes.data, zi.ctypes.data, off.data_ptr(), None,
                                                _lib.MEM_DEVICE, self.dev, self.stream.cuda_stream, _lib.FLAG_ASYNC))
         L = PREVIEW_XCORR_LAGS
         xc = torch.empty(abs(n_ref - (n_srv + 2 * L)) + 1, dtype=torch.complex128, device=self.tdev)
@@ -357,7 +324,7 @@ class SignalPreview:
     def run_device(self, ref_raw, srv_raw=None):
         """CUDA tensors of raw interleaved IQ -> the preview's results as tensors on their device (``offset`` an int).
         Work is forked from, and joined back into, the current torch stream."""
-        torch = _torch()
+        import torch
         self._setup(ref_raw.device if isinstance(ref_raw, torch.Tensor) and ref_raw.is_cuda else None)
         cur = torch.cuda.current_stream(self.tdev)
         self.stream.wait_stream(cur)
@@ -376,12 +343,12 @@ class SignalPreview:
     def run(self, ref_raw, srv_raw=None):
         """Host sources (ndarray, np.memmap, h5py dataset; int8, int16 or float32 raw interleaved IQ) -> the preview's
         results as NumPy arrays (``offset`` an int).  Only ``[0:input_chunk_length]`` of each source is read."""
-        torch = _torch()
+        import torch
         self._setup()
 
         def stage(src):
             a = np.ascontiguousarray(np.asarray(src[0:self.icl]))
-            if a.dtype not in _IQ_KINDS:
+            if a.dtype not in _lib.IQ_KINDS:
                 raise TypeError(f"raw IQ must be int8, int16 or float32, got {a.dtype}")
             return torch.from_numpy(a).to(self.tdev)
 

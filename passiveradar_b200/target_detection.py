@@ -27,7 +27,7 @@ def CFAR_2D(X, fw, gw, thresh=None, *, device=None):
     x = np.ascontiguousarray(X, dtype=np.float32)
     rows, cols = x.shape
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     if thresh is None:
         cr = np.empty((rows, cols), dtype=np.float32)
         _lib.check(lib.prc_cfar2d_f32(x.ctypes.data, rows, cols, int(fw), int(gw), None, cr.ctypes.data, None,
@@ -40,8 +40,8 @@ def CFAR_2D(X, fw, gw, thresh=None, *, device=None):
     return det.astype(bool)
 
 
-# ---------------------------------------------------------------------------------------------- ordered-statistic CFAR
-MAX_OS_FRAMES = 65535          # frames of one prc_os_cfar2d_frames call
+# ---------------------------------------------------------------------------------------------- batched CFAR
+MAX_CFAR_FRAMES = 65535        # frames of one prc_cfar2d_frames / prc_os_cfar2d_frames call
 
 
 def os_window_cells(fw, gw):
@@ -64,14 +64,25 @@ def os_rank(fw, gw, k=None):
     return -(-3 * os_window_cells(fw, gw) // 4)
 
 
-def _os_launch(x, rows, cols, nframes, fw, gw, k, out, flags, dev, stream):
-    """prc_os_cfar2d_frames over device tensors x (nframes compact float32 / complex64 maps) -> out (float64)."""
+def _cfar_frames_into(maps_d, cr, fw, gw, k, dev):
+    """The CR of every map of maps_d (T compact float32 / complex64 device maps; complex maps: their magnitude) into cr
+    (T compact float64 or float32 maps), on the current torch stream: CFAR_2D (prc_cfar2d_frames) or, with a rank k,
+    the ordered-statistic CFAR (prc_os_cfar2d_frames, float64 CR only)."""
+    import torch
     lib = _lib.load()
+    T, rows, cols = maps_d.shape
     cells = rows * cols
-    for t0 in range(0, nframes, MAX_OS_FRAMES):
-        nb = min(MAX_OS_FRAMES, nframes - t0)
-        _lib.check(lib.prc_os_cfar2d_frames(x[t0].data_ptr(), rows, cols, nb, cells, fw, gw, k, out[t0].data_ptr(),
-                                            cells, dev, stream, flags))
+    stream = _lib.stream_arg(maps_d.device)
+    flags = (_lib.FLAG_ASYNC | (_lib.FLAG_CR_F64 if cr.dtype == torch.float64 else 0) |
+             (_lib.FLAG_ABS_C64 if maps_d.dtype == torch.complex64 else 0))
+    for t0 in range(0, T, MAX_CFAR_FRAMES):
+        nb = min(MAX_CFAR_FRAMES, T - t0)
+        if k is None:
+            _lib.check(lib.prc_cfar2d_frames(maps_d[t0].data_ptr(), rows, cols, nb, cells, fw, gw, cr[t0].data_ptr(),
+                                             cells, _lib.MEM_DEVICE, dev, stream, flags))
+        else:
+            _lib.check(lib.prc_os_cfar2d_frames(maps_d[t0].data_ptr(), rows, cols, nb, cells, fw, gw, k,
+                                                cr[t0].data_ptr(), cells, dev, stream, flags))
 
 
 def OS_CFAR_2D(X, fw, gw, k=None, thresh=None, *, device=None):
@@ -94,13 +105,10 @@ def OS_CFAR_2D(X, fw, gw, k=None, thresh=None, *, device=None):
     x = np.ascontiguousarray(X, dtype=np.float32)
     rows, cols = x.shape
     fw, gw = int(fw), int(gw)
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     tdev = torch.device("cuda", dev)
-    xd = torch.from_numpy(x).to(tdev)[None]
     cr = torch.empty((1, rows, cols), dtype=torch.float64, device=tdev)
-    with torch.cuda.device(tdev):
-        _os_launch(xd, rows, cols, 1, fw, gw, os_rank(fw, gw, k), cr, _lib.FLAG_CR_F64, dev,
-                   torch.cuda.current_stream(tdev).cuda_stream or 1)
+    _cfar_frames_into(torch.from_numpy(x).to(tdev)[None], cr, fw, gw, os_rank(fw, gw, k), dev)
     out = cr[0].cpu().numpy()
     return out if thresh is None else out > thresh
 
@@ -110,12 +118,12 @@ def os_cfar_frames(stack, fw, gw, k=None, *, device=None):
     launch per 65 535 frames.  A host array gives a host float64 CR stack; a CUDA tensor gives a float64 CUDA tensor,
     ordered on the current torch stream.  Frame b's CR is bit-identical to a one-frame call on it.'''
     import torch
-    host = not (hasattr(stack, "is_cuda") and stack.is_cuda)
+    host = not _lib.is_cuda_tensor(stack)
     if host:
         a = np.asarray(stack)
         if a.dtype not in (np.float32, np.complex64):
             raise TypeError(f"stack must be float32 or complex64, got {a.dtype}")
-        dev = _lib.current_device() if device is None else int(device)
+        dev = _lib.current_device(device)
         t = torch.from_numpy(np.ascontiguousarray(a)).to(torch.device("cuda", dev))
     else:
         if stack.dtype not in (torch.float32, torch.complex64):
@@ -124,14 +132,9 @@ def os_cfar_frames(stack, fw, gw, k=None, *, device=None):
         dev = t.device.index if device is None else int(device)
     if t.dim() != 3:
         raise ValueError(f"stack must be three-dimensional (T, rows, cols), got {t.dim()} dimensions")
-    T, rows, cols = t.shape
     fw, gw = int(fw), int(gw)
-    out = torch.empty((T, rows, cols), dtype=torch.float64, device=t.device)
-    flags = _lib.FLAG_ASYNC | _lib.FLAG_CR_F64 | (_lib.FLAG_ABS_C64 if t.dtype == torch.complex64 else 0)
-    if T:
-        with torch.cuda.device(t.device):
-            _os_launch(t, rows, cols, T, fw, gw, os_rank(fw, gw, k), out, flags, dev,
-                       torch.cuda.current_stream(t.device).cuda_stream or 1)
+    out = torch.empty(t.shape, dtype=torch.float64, device=t.device)
+    _cfar_frames_into(t, out, fw, gw, os_rank(fw, gw, k), dev)
     return out.cpu().numpy() if host else out
 
 
@@ -187,25 +190,18 @@ def _extent(frame_extent):
     return float(fe[0]), float(fe[1])
 
 
-def _is_tensor(x):
-    return hasattr(x, "data_ptr") and hasattr(x, "is_cuda")
-
-
 def _frames_layout(maps, name):
     """(S, T, rows, cols) numpy array or CUDA tensor -> (array, S, T, rows, cols, seq_stride, frame_stride, f64)."""
-    if _is_tensor(maps):
-        if not maps.is_cuda:
-            maps = maps.numpy()
-        else:
-            import torch
-            if maps.dim() != 4:
-                raise ValueError(f"{name} must have shape (S, T, rows, cols)")
-            if maps.dtype not in (torch.float32, torch.float64):
-                raise TypeError(f"{name} must be a float32 or float64 CUDA tensor")
-            S, T, rows, cols = maps.shape
-            if maps.stride(3) != 1 or maps.stride(2) != cols:
-                raise ValueError(f"{name} frames must be contiguous (row-major rows x cols)")
-            return maps, S, T, rows, cols, maps.stride(0), maps.stride(1), maps.dtype == torch.float64
+    if _lib.is_cuda_tensor(maps):
+        import torch
+        if maps.dim() != 4:
+            raise ValueError(f"{name} must have shape (S, T, rows, cols)")
+        if maps.dtype not in (torch.float32, torch.float64):
+            raise TypeError(f"{name} must be a float32 or float64 CUDA tensor")
+        S, T, rows, cols = maps.shape
+        if maps.stride(3) != 1 or maps.stride(2) != cols:
+            raise ValueError(f"{name} frames must be contiguous (row-major rows x cols)")
+        return maps, S, T, rows, cols, maps.stride(0), maps.stride(1), maps.dtype == torch.float64
     a = _real_maps(np.asarray(maps), name)
     if a.ndim != 4:
         raise ValueError(f"{name} must have shape (S, T, rows, cols)")
@@ -235,19 +231,18 @@ def _launch(fn, maps, S, T, rows, cols, ss, fs, f64, args, out_dtype, out_shape,
     if initial_state is not None:
         hist[:, 0] = initial_state
         flags |= _lib.FLAG_TRACK_RESUME
-    if _is_tensor(maps):
+    if _lib.is_cuda_tensor(maps):
         import torch
         dev = maps.device.index if device is None else int(device)
         if initial_state is not None:
             hd = torch.from_numpy(hist.view(np.uint8).reshape(-1)).to(maps.device)
         else:
             hd = torch.empty(hist.nbytes, dtype=torch.uint8, device=maps.device)
-        stream = torch.cuda.current_stream(maps.device).cuda_stream
         _lib.check(getattr(lib, fn)(maps.data_ptr(), rows, cols, S, T, ss, fs, *args, hd.data_ptr(),
-                                    _lib.MEM_DEVICE, dev, stream, flags))
+                                    _lib.MEM_DEVICE, dev, _lib.stream_arg(maps.device), flags))
         hist.view(np.uint8).reshape(-1)[:] = hd.cpu().numpy()
         return hist
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     _lib.check(getattr(lib, fn)(maps.ctypes.data, rows, cols, S, T, ss, fs, *args, hist.ctypes.data,
                                 _lib.MEM_HOST, dev, None, flags))
     return hist
@@ -273,7 +268,7 @@ def get_measurements(dataFrame, p, frame_extent, *, device=None):
     rows, cols = x.shape
     n = rows * cols
     lib = _lib.load()
-    dev = _lib.current_device() if device is None else int(device)
+    dev = _lib.current_device(device)
     counts = np.zeros(1, dtype=np.int32)
     meas = np.empty((3, n), dtype=np.float64)
     _lib.check(lib.prc_get_measurements_frames(x.ctypes.data, rows, cols, 1, 1, n, n, dext, rext, n,
@@ -369,7 +364,7 @@ def cfar_track(maps_d, fw, gw, frame_extent, n_tracks, *, device=None):
     multitarget_tracker.  maps_d: (T, F, R+1) complex64 CUDA tensor (FramePipeline.run_device output); the maps are
     never copied to the host.  Returns the (T, n_tracks) target_track_dtype history.'''
     import torch
-    if not (_is_tensor(maps_d) and maps_d.is_cuda and maps_d.dtype == torch.complex64 and maps_d.dim() == 3):
+    if not (_lib.is_cuda_tensor(maps_d) and maps_d.dtype == torch.complex64 and maps_d.dim() == 3):
         raise TypeError("maps_d must be a (T, F, R+1) complex64 CUDA tensor")
     dext, rext = _extent(frame_extent)
     n_tracks = int(n_tracks)
@@ -378,14 +373,9 @@ def cfar_track(maps_d, fw, gw, frame_extent, n_tracks, *, device=None):
     T, F, R1 = maps_d.shape
     if n_tracks == 0 or T == 0:
         return np.zeros((T, n_tracks), dtype=target_track_dtype)
-    maps_d = maps_d.contiguous()
-    lib = _lib.load()
     dev = maps_d.device.index if device is None else int(device)
     cf = torch.empty((1, T, F, R1), dtype=torch.float32, device=maps_d.device)
-    stream = torch.cuda.current_stream(maps_d.device).cuda_stream
-    for t in range(T):
-        _lib.check(lib.prc_cfar2d_f32(maps_d[t].data_ptr(), F, R1, int(fw), int(gw), None, cf[0, t].data_ptr(), None,
-                                      _lib.MEM_DEVICE, dev, stream, _lib.FLAG_ABS_C64 | _lib.FLAG_ASYNC))
+    _cfar_frames_into(maps_d.contiguous(), cf[0], int(fw), int(gw), None, dev)
     return _launch("prc_multitarget_track_frames", cf, 1, T, F, R1, T * F * R1, F * R1, False,
                    (dext, rext, n_tracks), target_track_dtype, (1, T, n_tracks), dev)[0]
 
@@ -415,7 +405,7 @@ class TrackerPipeline:
 
     def __init__(self, max_range, max_doppler, *, tracker="multi", n_tracks=10, fw=18, gw=4, hold=20, decay=0.90,
                  render=True, batch=64, device=None, cfar="ca", os_rank=None):
-        from .plotting_tools import _cfar_choice, _decay_plan
+        from .plotting_tools import RenderPipeline
         if tracker not in ("multi", "simple"):
             raise ValueError(f"tracker must be 'multi' or 'simple', got {tracker!r}")
         self.tracker = tracker
@@ -423,17 +413,10 @@ class TrackerPipeline:
         self.n_tracks = int(n_tracks) if tracker == "multi" else 1
         if not 0 <= self.n_tracks <= MAX_TRACKS:
             raise ValueError(f"n_tracks={n_tracks} outside [0, {MAX_TRACKS}]")
-        self.fw, self.gw, self.hold, self.decay = int(fw), int(gw), int(hold), decay
-        if not (1 <= self.fw <= 64) or self.gw < 0 or self.fw * self.fw == self.gw * self.gw:
-            raise ValueError(f"fw={fw} gw={gw}: CFAR_2D needs 1 <= fw <= 64, gw >= 0 and fw != gw")
-        self.cfar, self.os_rank = _cfar_choice(cfar, os_rank, self.fw, self.gw)
-        if self.hold < 1:
-            raise ValueError("hold must be >= 1")
-        if int(batch) < 1:
-            raise ValueError("batch must be >= 1")
-        self.render, self.batch, self.device = bool(render), int(batch), device
-        # CF is float64 in the scripts (np.zeros(xambg.shape)): the products are float64 whatever decay's type
-        self.weights, _ = _decay_plan(np.float64, decay, self.hold)
+        # the chain's CFAR stage and, with render=True, its phosphor stage; it checks fw, gw, cfar, hold, batch, decay
+        self._render = RenderPipeline(fw, gw, hold, decay, device=device, batch=batch, cfar=cfar, os_rank=os_rank)
+        self.cfar, self.os_rank = self._render.cfar, self._render.os_rank
+        self.render, self.batch, self.device = bool(render), self._render.batch, device
         self.dtype = target_track_dtype if tracker == "multi" else target_track_dtype_simple
         self.reset()
 
@@ -450,13 +433,13 @@ class TrackerPipeline:
         """Start a new sequence: the next map is frame 0 of the tracker and of the persistence."""
         self._shape = None
         self._state = None          # the last frame's tracker records (uint8 device tensor)
-        self._carry = None          # the last hold - 1 CF frames
+        self._render.reset()        # the last hold - 1 CF frames
 
     def records(self, history, T=None):
         """The ``history`` bytes of ``run_device`` (T maps) as the tracker's NumPy records: (T, n_tracks)
         target_track_dtype for the multi-target tracker, (T,) target_track_dtype_simple for the simple one.  T may be
         left out unless n_tracks is 0."""
-        raw = history.cpu().numpy() if _is_tensor(history) else np.asarray(history, dtype=np.uint8)
+        raw = np.asarray(history.cpu() if _lib.is_cuda_tensor(history) else history, dtype=np.uint8)
         a = np.frombuffer(raw.tobytes(), dtype=self.dtype).copy()
         return a.reshape(-1 if T is None else T, self.n_tracks) if self.tracker == "multi" else a
 
@@ -474,12 +457,7 @@ class TrackerPipeline:
         * with render=True: ``data`` (T, R+1, F) float64 and ``limits`` (T, 2) = [vmin, vmax], as
           ``RenderPipeline.run_device`` gives them."""
         import torch
-        from .plotting_tools import PERCENTILES, VMAX_SCALE, _cfar_frames_into, _stream_arg
-        if not (_is_tensor(maps_d) and maps_d.is_cuda and maps_d.dim() == 3):
-            raise TypeError("maps_d must be a (T, F, R+1) CUDA tensor")
-        if maps_d.dtype not in (torch.complex64, torch.float32):
-            raise TypeError(f"maps_d must be complex64 or float32, got {maps_d.dtype}")
-        T, F, R1 = maps_d.shape
+        T, F, R1 = self._render._check(maps_d)
         if self._shape is not None and self._shape != (F, R1):
             raise ValueError(f"maps of shape {(F, R1)} continue a sequence of {self._shape} maps; call reset() first")
         if F * R1 > 1 << 19:
@@ -491,20 +469,12 @@ class TrackerPipeline:
         if T == 0:
             out["cf"] = torch.empty((0, F, R1), dtype=torch.float64, device=tdev)
             if self.render:
-                out["data"] = torch.empty((0, R1, F), dtype=torch.float64, device=tdev)
-                out["limits"] = torch.empty((0, 2), dtype=torch.float64, device=tdev)
+                out["data"], out["limits"] = self._render.run_device(maps_d)
             return self._masks(out, 0, torch)
         lib = _lib.load()
-        # the scripts take np.abs of the stack before CFAR_2D, and the CFAR kernel keeps the sign of a real cell in its
-        # numerator: a float32 map is made |map| first (exact, and a no-op on magnitudes)
-        maps_d = (maps_d.abs() if maps_d.dtype == torch.float32 else maps_d).contiguous()
-        stream = _stream_arg(torch, tdev)
-        nc = 0 if self._carry is None else self._carry.shape[0]
+        cf, nc = self._render._cf(maps_d, dev)
         cells = F * R1
-        cf = torch.empty((nc + T, F, R1), dtype=torch.float64, device=tdev)
-        if nc:
-            cf[:nc] = self._carry
-        _cfar_frames_into(lib, self.cfar, self.os_rank, maps_d, cf[nc:], self.fw, self.gw, dev, stream)
+        stream = _lib.stream_arg(tdev)
         hist = out["history"]
         flags = _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64
         if self._state is not None:
@@ -520,18 +490,7 @@ class TrackerPipeline:
                                                    self.max_doppler, hist.data_ptr(), _lib.MEM_DEVICE, dev, stream,
                                                    flags))
         if self.render:
-            data = torch.empty((T, R1, F), dtype=torch.float64, device=tdev)
-            limits = torch.empty((T, 2), dtype=torch.float64, device=tdev)
-            q = np.array(PERCENTILES, dtype=np.float64)
-            scale = np.array([1.0, VMAX_SCALE], dtype=np.float64)
-            _lib.check(lib.prc_persistence_frames(cf.data_ptr(), F, R1, T, cells, nc, self.hold,
-                                                  self.weights.ctypes.data, data.data_ptr(), _lib.MEM_DEVICE, dev,
-                                                  stream, _lib.FLAG_ASYNC | _lib.FLAG_MAP_F64 | _lib.FLAG_ORIENT))
-            _lib.check(lib.prc_percentiles_frames(data.data_ptr(), cells, T, cells, q.ctypes.data, scale.ctypes.data,
-                                                  2, limits.data_ptr(), _lib.MEM_DEVICE, dev, stream, _lib.FLAG_ASYNC))
-            out["data"], out["limits"] = data, limits
-            keep = min(nc + T, self.hold - 1)
-            self._carry = cf[nc + T - keep:].clone() if keep else None
+            out["data"], out["limits"] = self._render._phosphor(cf, nc, dev)
         self._shape = (F, R1)
         self._state = hist[(T - 1) * rec:].clone() if rec else None
         out["cf"] = cf[nc:]
@@ -561,28 +520,14 @@ class TrackerPipeline:
         (CFAR_2D reads float32, as the drop-in does).  Starts a new sequence and streams it through in batches.
         Returns host arrays: ``history`` exactly as multitarget_tracker / simple_target_tracker return it, the masked
         estimates and, with render=True, ``data`` (nframes, R+1, F) and ``limits`` (nframes, 2)."""
-        import torch
-        xambg = np.asarray(xambg)
-        if xambg.ndim != 3:
-            raise ValueError(f"xambg must be (F, R+1, nframes), got {xambg.ndim} dimensions")
-        if xambg.dtype.kind == "c":
-            dt = np.complex64
-        elif xambg.dtype.kind in "biuf":
-            dt = np.float32
-        else:
-            raise TypeError(f"unsupported map dtype {xambg.dtype}")
-        N = xambg.shape[2]
-        dev = _lib.current_device() if self.device is None else int(self.device)
-        tdev = torch.device("cuda", dev)
+        from .plotting_tools import _host_batches
         self.reset()
-        parts = []
-        with torch.cuda.device(tdev):
-            for b0 in range(0, max(N, 1), self.batch):      # an empty stack still gives empty outputs
-                b1 = min(N, b0 + self.batch)
-                maps = torch.from_numpy(np.ascontiguousarray(np.moveaxis(xambg[:, :, b0:b1], 2, 0), dtype=dt))
-                got = self.run_device(maps.to(tdev))
-                del got["cf"]
-                parts.append({k: v.cpu().numpy() for k, v in got.items()})
+        parts, N = [], 0
+        for maps in _host_batches(xambg, "xambg", "map", self.device, self.batch):
+            got = self.run_device(maps)
+            del got["cf"]
+            parts.append({k: v.cpu().numpy() for k, v in got.items()})
+            N += maps.shape[0]
         res = {k: np.concatenate([p[k] for p in parts]) for k in parts[0]}
         res["history"] = self.records(res["history"], N)
         return res
