@@ -183,6 +183,22 @@ int prc_frames_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframe
                    int mem_kind, int device, void* stream, unsigned flags);
 int prc_ls_status(int device, void* stream, int* status, int nframes);
 
+/* prc_frames_multi_c64: prc_frames_c64 for nchan surveillance channels that share one reference channel (one reference
+ * antenna and up to four surveillance antennas of one coherent receiver).  Frame f of the reference is at
+ * ref + f*frame_stride; frame f of surveillance channel k at srv + k*chan_stride + f*frame_stride (strides in samples,
+ * any chan_stride, 0 included: the inputs are only read).  maps receives [nchan][nframes][freq_bins][range_bins+1],
+ * taps_out (or NULL) [nchan][nframes][filter_len+peek]; the status words are [nchan][nframes] (prc_ls_status with
+ * nchan*nframes).  Channel k's taps and map are those of prc_frames_c64(ref, srv_k) on the same frames; where the
+ * one-pass frame runs and nchan >= 2 the reference's transforms, its lag sums and its part of the CAF block spectra are
+ * formed once for all channels (csrc/framemulti.cuh).  All pointers are DEVICE pointers (no mem_kind).  Flags:
+ * PRC_FLAG_ASYNC, PRC_FLAG_WINDOW_F32 as in prc_frames_c64.  Limits (PRC_E_INVALID before any CUDA call):
+ * 1 <= nchan <= 4, plus prc_frames_c64's.  nchan = 1 is exactly prc_frames_c64 on device pointers.
+ */
+int prc_frames_multi_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                         int nchan, int64_t chan_stride, int filter_len, int peek, float reg, int range_bins,
+                         int freq_bins, const void* window, prc_c64* maps, prc_c64* taps_out,
+                         int device, void* stream, unsigned flags);
+
 /* The other two operators of the path on nframes independent frames per call (same layout rules as prc_frames_c64):
  * prc_nlms_frames_c64 -- NLMS_filter / block_NLMS (clutter_removal.py:189-249): the recurrence of one frame is serial,
  *   so every frame gets its own CTA (one SM) and the batch fills the GPU; init_taps (filter_len + peek taps or NULL)

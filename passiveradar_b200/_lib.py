@@ -82,6 +82,9 @@ SIGNATURES = {
                                          C.c_uint]),
     "prc_ls_svd_frames_c64": (C.c_int, [_c64p, _c64p, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int, _c64p, _c64p,
                                         C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_frames_multi_c64": (C.c_int, [_c64p, _c64p, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_int,
+                                       C.c_float, C.c_int, C.c_int, C.c_void_p, _c64p, _c64p, C.c_int, C.c_void_p,
+                                       C.c_uint]),
     "prc_ls_status": (C.c_int,[C.c_int, C.c_void_p, C.POINTER(C.c_int), C.c_int]),
     "prc_set_option": (C.c_int, [C.c_char_p, C.c_int]),
     "prc_get_option": (C.c_int, [C.c_char_p, C.POINTER(C.c_int)]),

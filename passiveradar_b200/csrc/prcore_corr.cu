@@ -1,6 +1,7 @@
 // prcore_corr.cu -- the correlation family of libprcore.so: LS_Filter (direct form and FFT-domain), LS_Filter_Toeplitz
 // and LS_Filter_Multiple, fast_xambg, direct_xambg, and the frame (LS_Filter -> fast_xambg) with its one-pass FFT-domain
-// path; their planners, launches and C entry points, and the options that select their paths.
+// path and its shared-reference form for several surveillance channels; their planners, launches and C entry points,
+// and the options that select their paths.
 #include <cuda_runtime.h>
 
 #include <atomic>
@@ -14,6 +15,7 @@
 #include "lagstream.cuh"
 #include "fftcorr.cuh"
 #include "framepass.cuh"
+#include "framemulti.cuh"
 
 namespace prcore {
 
@@ -56,6 +58,7 @@ int corr_set_attrs(int lim) {
     PRC_FFT_ATTRS(16)
 #undef PRC_FFT_ATTRS
     CU(fftc::framepass_set_attrs(lim));
+    CU(fftc::framemulti_set_attrs(lim));
     return PRC_OK;
 }
 
@@ -794,6 +797,109 @@ int frame_device(Ctx* c, const FramePlan& fp, const float2* ref, const float2* s
     return PRC_OK;
 }
 
+// ---- several surveillance channels against one reference (framemulti.cuh)
+// The shared pass runs where the one-pass plan is on and at least this many channels share the reference: the
+// smallest K at which scripts/multichannel_bench.py measured it faster than K one-pass frames (DESIGN.md section 20)
+constexpr int FM_MIN_SHARED_K = 2;
+
+// nchan = K shared-reference frames of one chunk after another: the one-pass plan's partition, one frame_multi_pass
+// launch, then levinson_launch, taps_spectrum and caf_combine_multi on K nf problems ([k][f] within the chunk) and the
+// Doppler stage channel by channel.  The CTAs of a frame walk its units exactly as frame_onepass's do for the same
+// frames per launch, so each channel is bit for bit prc_frames_c64(ref, srv_k) when the batch fits one chunk of both.
+int frames_shared(Ctx* c, const OnePassPlan& op, const float2* ref, const float2* srv, long long n, Batch bt, int K,
+                  long long chan_stride, int filter_len, int peek, double reg, int R, int F, const float* win32,
+                  float2* maps, float2* taps_out) {
+    if (n >= (1ll << 31) - 4096) return fail(PRC_E_INVALID, "n=%lld unsupported", n);
+    if (op.dm.ntaps > (1ll << 30)) return fail(PRC_E_INVALID, "decimator too long");
+    constexpr int R3 = fftc::FP_R3;
+    constexpr int L = 256 * R3;
+    const int M = filter_len + peek;
+    const float2* tw;
+    TRY(fft_twiddles(c, R3, &tw));
+    const size_t per_frame = (size_t)(1 + K) * F * L * sizeof(float2);
+    const int chunk = (int)std::max<size_t>(1, std::min<size_t>((size_t)bt.nf, FP_ACC_CAP / per_frame));
+    const int HT = (M + 1) & ~1, HTc = (R + 2) & ~1;
+    const size_t map_elems = (size_t)F * (R + 1);
+    TRY(c->fpacc.ensure(per_frame * chunk));
+    TRY(c->lstaps.ensure((size_t)K * chunk * M * sizeof(float2)));
+    TRY(c->status.ensure((size_t)K * chunk * sizeof(int)));
+    TRY(c->mstatus.ensure((size_t)K * bt.nf * sizeof(int)));
+    TRY(c->fftP.ensure((size_t)K * chunk * F * HTc * sizeof(float2)));
+    const int units = F + op.ntail;
+    for (int f0 = 0; f0 < bt.nf; f0 += chunk) {
+        const int nf = std::min(chunk, bt.nf - f0);
+        const int np = K * nf;
+        // frame_onepass's grid for nf frames per launch (two of its CTAs per SM), so that the partitions agree
+        const long long slots = (long long)fft_ctas_per_sm(c, FK_FRAME, R3) * c->nsm;
+        const int ncta = (int)std::max<long long>(1, std::min<long long>(units, slots / nf));
+        TRY(c->partial.ensure((size_t)np * 2 * ncta * HT * sizeof(float2)));
+        fftc::FrameMultiParams p{};
+        fftc::FramePassParams& b = p.fp;
+        b.ref = ref + (size_t)f0 * bt.stride; b.srv = srv + (size_t)f0 * bt.stride; b.frame_stride = bt.stride;
+        b.win = win32;
+        b.n = (int)n; b.M = M; b.peek = peek; b.F = F;
+        b.D = op.dm.D; b.c0 = op.dm.c0; b.ntaps = (int)op.dm.ntaps; b.Bmax = op.Bmax;
+        b.tail_lo = (int)op.tail_lo; b.ntail = op.ntail; b.Bt = op.Bt;
+        b.acc = c->fpacc.as<float2>(); b.partial = c->partial.as<float2>(); b.HT = HT; b.tw = tw;
+        p.chan_stride = chan_stride;
+        {
+            ProfScope ps(c, K_FRAME_MULTI);
+            fftc::launch_frame_multi(p, K, ncta, nf, c->stream);
+        }
+        TRY(check_launch("frame_multi_pass_kernel"));
+        TRY(levinson_launch(c, ncta, HT, M, reg, np, c->lstaps.as<float2>(), c->status.as<int>()));
+        TRY(taps_spectrum(c, R3, M, np, &c->wp_caf));
+        fftc::CafCombineMultiParams q{};
+        q.acc = c->fpacc.as<float2>(); q.wp = c->wp_caf.as<float2>();
+        q.F = F; q.R = R; q.peek = peek; q.nf = nf; q.nchan = K;
+        q.P = c->fftP.as<float2>(); q.HT = HTc; q.tw = tw;
+        const long long cslots = (long long)fft_ctas_per_sm(c, FK_COMBINE, R3) * c->nsm;
+        const int gc = (int)std::max<long long>(1, std::min<long long>(F, cslots / np));
+        {
+            ProfScope ps(c, K_CAF_COMBINE);
+            fftc::launch_caf_combine_multi(q, gc, np, c->stream);
+        }
+        TRY(check_launch("caf_combine_multi_kernel"));
+        // the Doppler stage as frame_onepass runs it on nf frames: its kernel choice depends on the frame count
+        for (int k = 0; k < K; ++k)
+            TRY(doppler_stage(c, BlockSums{c->fftP.as<float2>() + (size_t)k * nf * F * HTc, 1, HTc, (int)op.dm.ntaps, 0}, R, F,
+                              nf, maps + ((size_t)k * bt.nf + f0) * map_elems));
+        // taps and status of the chunk's [k][f] problems -> [k][frame]
+        if (taps_out)
+            CU(cudaMemcpy2DAsync(taps_out + (size_t)f0 * M, (size_t)bt.nf * M * sizeof(float2), c->lstaps.p,
+                                 (size_t)nf * M * sizeof(float2), (size_t)nf * M * sizeof(float2), K, cudaMemcpyDeviceToDevice,
+                                 c->stream));
+        CU(cudaMemcpy2DAsync(c->mstatus.as<int>() + f0, (size_t)bt.nf * sizeof(int), c->status.p, (size_t)nf * sizeof(int),
+                             (size_t)nf * sizeof(int), K, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    TRY(c->status.ensure((size_t)K * bt.nf * sizeof(int)));
+    CU(cudaMemcpyAsync(c->status.p, c->mstatus.p, (size_t)K * bt.nf * sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+    return PRC_OK;
+}
+
+// nchan channels of bt.nf frames each, channel k's frames chan_stride samples after channel 0's; maps [k][frame][F][R+1],
+// taps_out [k][frame][M] or NULL, status words [k][frame] in c->status.  One channel is prc_frames_c64's frame_device
+// call; several take the shared pass where it pays (FM_MIN_SHARED_K) and otherwise frame_device channel by channel.
+int frames_multi_device(Ctx* c, const FramePlan& fp, const float2* ref, const float2* srv, long long n, Batch bt, int nchan,
+                        long long chan_stride, int filter_len, int peek, double reg, int R, int F, const float* win32,
+                        float2* maps, float2* taps_out) {
+    if (nchan == 1)
+        return frame_device(c, fp, ref, srv, n, bt, filter_len, peek, reg, R, F, win32, maps, taps_out, nullptr);
+    if (fp.one.on && nchan >= FM_MIN_SHARED_K)
+        return frames_shared(c, fp.one, ref, srv, n, bt, nchan, chan_stride, filter_len, peek, reg, R, F, win32, maps, taps_out);
+    const int M = filter_len + peek;
+    TRY(c->mstatus.ensure((size_t)nchan * bt.nf * sizeof(int)));
+    for (int k = 0; k < nchan; ++k) {
+        TRY(frame_device(c, fp, ref, srv + (long long)k * chan_stride, n, bt, filter_len, peek, reg, R, F, win32,
+                         maps + (size_t)k * bt.nf * F * (R + 1), taps_out ? taps_out + (size_t)k * bt.nf * M : nullptr, nullptr));
+        CU(cudaMemcpyAsync(c->mstatus.as<int>() + (size_t)k * bt.nf, c->status.p, (size_t)bt.nf * sizeof(int),
+                           cudaMemcpyDeviceToDevice, c->stream));
+    }
+    TRY(c->status.ensure((size_t)nchan * bt.nf * sizeof(int)));
+    CU(cudaMemcpyAsync(c->status.p, c->mstatus.p, (size_t)nchan * bt.nf * sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+    return PRC_OK;
+}
+
 // read-only names of the residency the one-wave grids are sized from (fft_ctas_per_sm, R3 = 8 -- the transform
 // length of up to 1024 LS taps and of the CAF at config 2): the FftKern they report, -1 for any other name
 int fft_ctas_option(const std::string& k) {
@@ -952,6 +1058,29 @@ int prc_frame_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int filter_
                   prc_c64* cleaned_out, int mem_kind, int device, void* stream, unsigned flags) {
     return prc_frames_c64(ref, srv, n, 1, n, filter_len, peek, reg, range_bins, freq_bins, window, out_map, taps_out,
                           cleaned_out, mem_kind, device, stream, flags);
+}
+
+int prc_frames_multi_c64(const prc_c64* ref, const prc_c64* srv, int64_t n, int nframes, int64_t frame_stride,
+                         int nchan, int64_t chan_stride, int filter_len, int peek, float reg, int range_bins,
+                         int freq_bins, const void* window, prc_c64* maps, prc_c64* taps_out,
+                         int device, void* stream, unsigned flags) {
+    if (nchan < 1 || nchan > fftc::FM_MAX_CHANNELS)
+        return fail(PRC_E_INVALID, "nchan=%d invalid (1 <= nchan <= %d)", nchan, fftc::FM_MAX_CHANNELS);
+    Batch bt;
+    TRY(stack_args(ref, srv, maps, "ref/srv/maps", PRC_MEM_DEVICE, n, nframes, frame_stride, &bt, range_bins, freq_bins));
+    if (filter_len < 0 || peek < 0 || filter_len + peek < 1)
+        return fail(PRC_E_INVALID, "filter_len=%d peek=%d invalid", filter_len, peek);
+    Ctx* c;
+    TRY(get_ctx(device, stream, &c));
+    std::lock_guard<std::mutex> lk(c->mu);
+    const FramePlan fp = frame_plan(c, n, nframes, filter_len, peek, range_bins, freq_bins);
+    const float* win32;
+    TRY(stage_window(c, window, n, PRC_MEM_DEVICE, flags, &win32));
+    TRY(frames_multi_device(c, fp, reinterpret_cast<const float2*>(ref), reinterpret_cast<const float2*>(srv), n, bt, nchan,
+                            chan_stride, filter_len, peek, (double)reg, range_bins, freq_bins, win32,
+                            reinterpret_cast<float2*>(maps), reinterpret_cast<float2*>(taps_out)));
+    TRY(check_ls_status(c, flags, nchan * nframes));
+    return finish(c, flags);
 }
 
 int prc_set_option(const char* name, int value) {
