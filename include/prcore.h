@@ -388,6 +388,32 @@ int prc_percentiles_frames(const double* x, int64_t n, int nframes, int64_t fram
 int prc_os_cfar2d_frames(const void* x, int rows, int cols, int nframes, int64_t frame_stride, int fw, int gw, int k,
                          void* cr_out, int64_t cr_stride, int device, void* stream, unsigned flags);
 
+/* ---- beamscan of several surveillance channels (not in the reference) -------------------------------------------
+ * prc_beamscan_frames: for nframes frames of nchan complex64 rows x cols maps (channel k of frame f at
+ *   maps + k*chan_stride + f*frame_stride elements, the layout prc_frames_multi_c64 writes, so its output is read in
+ *   place) and a steering table S of nangles x nchan complex64 values (row a: the array response of grid angle a),
+ *   per cell, in float32:
+ *     P[a]  = | sum_k S[a, k] * m_k |^2, a = 0 .. nangles-1
+ *     a*    = the first a with the largest P[a]
+ *     amp   = sqrt(P[a*])
+ *     den   = P[a*-1] - 2 P[a*] + P[a*+1]
+ *     delta = clamp(0.5 (P[a*-1] - P[a*+1]) / den, -0.5, 0.5) if den < 0, else 0
+ *     pos   = a* + delta  (a fractional grid index)
+ *   wrap = 0: a sector grid, delta = 0 at a* = 0 and a* = nangles-1.  wrap = 1: a full-circle grid, neighbours taken
+ *   mod nangles; pos lies in [-0.5, nangles - 0.5).  The CAF conjugates the surveillance channel, so an echo from
+ *   theta gives m_k = conj(a_k(theta)) * c: S is the array response itself, not its conjugate.  Per-channel complex
+ *   gains g_k are folded in by the caller as S[a, k] / conj(g_k).  A zero cell gives amp = 0, pos = 0; maps must be
+ *   finite.  Frame f's amp and pos go to amp_out / pos_out + f*out_stride (either may be NULL, not both); a frame's
+ *   results do not depend on nframes.
+ *   maps, amp_out and pos_out are DEVICE pointers (no mem_kind); steering is a HOST array, copied before the call
+ *   returns (PRC_FLAG_ASYNC included).  Limits (PRC_E_INVALID, naming the limit, before any CUDA call): rows, cols >= 1,
+ *   0 <= nframes <= 65535, 1 <= nchan <= 4, 1 <= nangles <= 4096, wrap 0 or 1, chan_stride >= 0, frame_stride and
+ *   out_stride >= rows*cols when nframes > 1, maps and steering not NULL.
+ */
+int prc_beamscan_frames(const prc_c64* maps, int rows, int cols, int nframes, int64_t frame_stride, int nchan,
+                        int64_t chan_stride, const prc_c64* steering, int nangles, int wrap, float* amp_out,
+                        float* pos_out, int64_t out_stride, int device, void* stream, unsigned flags);
+
 /* ---- Kalman target trackers ------------------------------------------------------------------------
  * Replace get_measurements(), multitarget_tracker() and simple_target_tracker(), reference
  * passiveRadar/target_detection.py:164-681.  The records below are byte for byte the reference's NumPy

@@ -22,6 +22,7 @@ from .target_detection import (CFAR_2D, OS_CFAR_2D, os_cfar_frames, get_measurem
 from .recording import RecordingPipeline                                     # noqa: F401
 from .plotting_tools import persistence, persistence_frames, RenderPipeline  # noqa: F401
 from .spectrum import psd, psd_frames, SignalPreview                         # noqa: F401
+from .beamforming import steering_vectors, ula_positions, uca_positions, beamscan_frames, bearing  # noqa: F401
 
 __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS", "LS_Filter_Toeplitz",
            "LS_Filter_Multiple", "GAL_JPE", "gal_jpe_frames", "LS_Filter_SVD", "ls_filter_svd_frames", "deinterleave_IQ", "frequency_shift", "resample", "frontend",
@@ -29,7 +30,8 @@ __all__ = ["fast_xambg", "direct_xambg", "LS_Filter", "NLMS_filter", "block_NLMS
            "normalize", "CFAR_2D", "OS_CFAR_2D", "os_cfar_frames",
            "get_measurements", "multitarget_tracker", "simple_target_tracker", "multitarget_tracker_frames",
            "simple_tracker_frames", "cfar_track", "TrackerPipeline", "RecordingPipeline", "persistence", "persistence_frames",
-           "RenderPipeline", "psd", "psd_frames", "SignalPreview"]
+           "RenderPipeline", "psd", "psd_frames", "SignalPreview", "steering_vectors", "ula_positions", "uca_positions",
+           "beamscan_frames", "bearing"]
 __version__ = "0.1.0"
 
 

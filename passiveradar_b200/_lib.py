@@ -105,6 +105,9 @@ SIGNATURES = {
                                     C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_os_cfar2d_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int,
                                        C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_uint]),
+    "prc_beamscan_frames": (C.c_int, [_c64p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int64, _c64p,
+                                      C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p,
+                                      C.c_uint]),
     "prc_persistence_frames": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_uint]),
     "prc_percentiles_frames": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_int,

@@ -1,6 +1,7 @@
 // prcore.cu -- runtime of libprcore.so: errors, workspaces and their teardown, kernel attributes, profiling, pinned
 // host staging and argument checks, and the C entry points that belong to no operator family.  The operator families'
-// host code lives in prcore_corr.cu, prcore_clutter.cu, prcore_signal.cu and prcore_detect.cu (prcore_host.h).
+// host code lives in prcore_corr.cu, prcore_clutter.cu, prcore_signal.cu, prcore_detect.cu and prcore_array.cu
+// (prcore_host.h).
 //
 // Build (see passiveradar_b200/build.py):
 //   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden \
@@ -31,7 +32,7 @@ const char* const kKernelNames[K_COUNT] = {"lagcorr_ls", "levinson", "fir_apply"
                                            "caf_combine", "frontend_chunks", "cfar_frames",
                                            "persistence", "percentile", "psd_segments", "psd_finish",
                                            "decimate", "norm_sum", "norm_scale", "os_cfar",
-                                           "frame_multi"};
+                                           "frame_multi", "beamscan"};
 std::atomic<int> g_prof_on{0};
 std::mutex g_prof_mu;
 double g_prof_ms[K_COUNT] = {0};
@@ -265,9 +266,13 @@ int unstage(Ctx* c, void* dst, const void* src, int mem_kind, size_t rows, size_
 // transfer below is from pageable memory this function owns, which the runtime stages before cudaMemcpyAsync returns,
 // so it is safe under PRC_FLAG_ASYNC even when the caller's array is page-locked and goes away right after the call
 int copy_params(Ctx* c, const double* src, int count, DBuf& buf) {
-    const std::vector<double> v(src, src + count);
-    TRY(buf.ensure((size_t)count * sizeof(double)));
-    CU(cudaMemcpyAsync(buf.p, v.data(), (size_t)count * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    return copy_param_bytes(c, src, (size_t)count * sizeof(double), buf);
+}
+
+int copy_param_bytes(Ctx* c, const void* src, size_t bytes, DBuf& buf) {
+    const std::vector<char> v(static_cast<const char*>(src), static_cast<const char*>(src) + bytes);
+    TRY(buf.ensure(bytes));
+    CU(cudaMemcpyAsync(buf.p, v.data(), bytes, cudaMemcpyHostToDevice, c->stream));
     return PRC_OK;
 }
 

@@ -6,7 +6,7 @@
 // buffer reuse is ordered by the stream.  Nothing here falls back to the CPU.
 //
 // Modules (DESIGN.md section 3): prcore.cu (runtime), prcore_corr.cu, prcore_clutter.cu, prcore_signal.cu,
-// prcore_detect.cu.  Each kernel header is included by exactly one of them; this header includes none.
+// prcore_detect.cu, prcore_array.cu.  Each kernel header is included by exactly one of them; this header includes none.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -26,7 +26,7 @@ constexpr size_t SMEM_LIMIT = 200 * 1024;
 enum KernelId { K_LAGCORR_LS = 0, K_LEVINSON, K_FIR, K_LAGCORR_CAF, K_DOPPLER, K_NLMS, K_MISC, K_GAL, K_TRK_MEAS, K_TRK_MULTI,
                 K_TRK_SIMPLE, K_CHANOFF_LOAD, K_CHANOFF_IIR, K_CHANOFF_FFT, K_CHANOFF_ARGMAX, K_SVD_CORR, K_SVD_EIG, K_SVD_FIR,
                 K_CAF_COMBINE, K_FRONTEND_CHUNKS, K_CFAR_FRAMES, K_PERSISTENCE,
-                K_PERCENTILE, K_PSD_SEGMENTS, K_PSD_FINISH, K_DECIMATE, K_NORM_SUM, K_NORM_SCALE, K_OS_CFAR, K_FRAME_MULTI, K_COUNT };
+                K_PERCENTILE, K_PSD_SEGMENTS, K_PSD_FINISH, K_DECIMATE, K_NORM_SUM, K_NORM_SCALE, K_OS_CFAR, K_FRAME_MULTI, K_BEAMSCAN, K_COUNT };
 struct ProfRec { int id; cudaEvent_t a, b; };
 
 int fail(int code, const char* fmt, ...);      // sets prc_last_error(); returns code
@@ -100,6 +100,7 @@ struct Ctx {
     DBuf fft_tw[3], wp_fir, wp_caf, fftP;     // FFT-domain path: twiddle tables (L = 1024 / 2048 / 4096), taps spectra, CAF block sums
     DBuf fpacc;                               // one-pass frame: AccP / AccQ spectra per Doppler block [nf][F][2][L]
     DBuf mstatus;                             // frames of several channels: Toeplitz-solve status [nchan][nframes]
+    DBuf bf_steer;                            // beamscan: the call's steering table [nangles][nchan]
     bool fft_tw_ready[3] = {false, false, false};
     int fft_ctas[4][3] = {};  // CTAs per SM of the one-wave FFT-domain kernels, [FftKern][r3_index] (0: not asked yet)
     std::vector<ProfRec> recs;
@@ -146,6 +147,7 @@ int rows_h2d(Ctx* c, void* dst, const void* src, size_t rows, size_t row_bytes, 
 int rows_d2h(Ctx* c, void* dst, const void* src, size_t rows, size_t row_bytes, size_t stride, unsigned flags);
 int unstage(Ctx* c, void* dst, const void* src, int mem_kind, size_t rows, size_t row_bytes, size_t stride, unsigned flags);
 int copy_params(Ctx* c, const double* src, int count, DBuf& buf);
+int copy_param_bytes(Ctx* c, const void* src, size_t bytes, DBuf& buf);
 int finish(Ctx* c, unsigned flags);
 
 // ---- arguments and operands of the C entry points
