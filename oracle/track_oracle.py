@@ -81,17 +81,25 @@ def _frame(data_frame):
     return np.ascontiguousarray(y.T[:, ::-1])
 
 
+def measurement_frame(data_frame):
+    """The normalised, transformed frame with its edge range rows and centre Doppler columns zeroed: what
+    get_measurements takes the percentile of."""
+    rows = np.shape(data_frame)[0]
+    y = _frame(data_frame)
+    y[:8, :] = 0
+    y[-8:, :] = 0
+    c = rows // 2
+    y[:, c - 4:c + 4] = 0
+    return y
+
+
 def get_measurements(data_frame, p, frame_extent):
     """(3, M): range, Doppler, strength of the cells at or above the 99.8th percentile, strongest first."""
     rext, dext = float(frame_extent[1]), float(frame_extent[0])
     rows, cols = np.shape(data_frame)
     rpts = np.linspace(rext, 0, cols)
     dpts = np.linspace(-1 * dext, dext, rows)
-    y = _frame(data_frame)
-    y[:8, :] = 0
-    y[-8:, :] = 0
-    c = rows // 2
-    y[:, c - 4:c + 4] = 0
+    y = measurement_frame(data_frame)
     thr = np.percentile(y, 99.8)
     ri, di = np.nonzero(y >= thr)
     s = y[ri, di]
